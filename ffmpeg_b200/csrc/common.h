@@ -1,7 +1,6 @@
 // common.h — internals shared by the translation units of libb200dsp.so
 #pragma once
 #include <cuda_runtime.h>
-#include <cuda.h>
 #include <cstdint>
 #include <cstddef>
 #include <cstdio>
@@ -45,12 +44,6 @@ void *b200_pinned(B200Device *dev, size_t bytes);        // pinned host scratch
             return B200_EEXTERNAL;                                                              \
         }                                                                                       \
     } while (0)
-
-// 2-D tensor map (TMA descriptor) over a byte plane: rows of `pitch` bytes (multiple of 16, base 16-byte aligned), box = box_w x box_h bytes,
-// swizzle = CU_TENSOR_MAP_SWIZZLE_NONE / _32B ...  The number of rows is unknown to the batched entry points (they take offsets, not
-// plane sizes), so the map claims 2^31 - 1 rows: boxes are only ever placed where the caller's operations point.  Encoded through the
-// driver entry point (no link-time dependency on libcuda).  Returns false when the driver call is unavailable or refuses the geometry.
-bool b200_tmap_2d_u8(CUtensorMap *out, const void *base, unsigned long long pitch, unsigned box_w, unsigned box_h, int swizzle);
 
 #define B200_LAUNCHED() (g_b200_launches.fetch_add(1, std::memory_order_relaxed))
 

@@ -156,28 +156,3 @@ B200_API int b200_memcpy_d2h(B200Device *d, void *dst, const void *src, size_t b
     B200_CUDA_OK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, d->stream));
     return 0;
 }
-
-bool b200_tmap_2d_u8(CUtensorMap *out, const void *base, unsigned long long pitch, unsigned box_w, unsigned box_h, int swizzle)
-{
-    typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
-                                 const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                 CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-    static EncodeFn fn = nullptr;
-    static bool tried = false;
-    {
-        std::lock_guard<std::mutex> lk(g_mu);
-        if (!tried) {
-            tried = true;
-            void *p = nullptr;
-            cudaDriverEntryPointQueryResult q;
-            if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-                fn = (EncodeFn)p;
-        }
-    }
-    if (!fn || ((uintptr_t)base & 15) || (pitch & 15) || pitch == 0 || pitch >= (1ULL << 32) || box_w > 256 || box_h > 256) return false;
-    const cuuint64_t dims[2] = { pitch, 0x7fffffffULL };
-    const cuuint64_t strides[1] = { pitch };
-    const cuuint32_t box[2] = { box_w, box_h }, estr[2] = { 1, 1 };
-    return fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void *>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-              (CUtensorMapSwizzle)swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}

@@ -393,29 +393,27 @@ template <int MB>
 int launch_esa(cudaStream_t st, const uint8_t *cur, const uint8_t *ref, int linesize, long long fs, int b_w, int b_h,
                int nframes, int search, int32_t *mv, unsigned long long *cost)
 {
-    static int v2 = -1;                                          // B200_ESA2=0: the first kernel
-    if (v2 < 0) { const char *e = getenv("B200_ESA2"); v2 = e ? atoi(e) : 1; }
-    if (v2) {
-        constexpr int MBS = 2;
-        const int wc = 2 * search + MB * MBS;                    // widest joint window in bytes
-        const int pitch = (wc + 3) / 4 + 1;
-        const int trows = 2 * search + MB + ESA2_NV - 1;
-        int copy_words = trows * pitch + 1;
-        copy_words += (8 - (copy_words & 31) + 32) & 31;         // copies 8 banks apart: the four phases of 8 neighbouring columns hit 32 banks
-        const size_t smem2 = ((size_t)MBS * MB * (MB / 4) + 4 * (size_t)copy_words) * 4;
-        if (smem2 <= 100 * 1024) {
-            if (smem2 > 48 * 1024)
-                B200_CUDA_OK(cudaFuncSetAttribute(esa2_kernel<MB, MBS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-            for (int f0 = 0; f0 < nframes; f0 += 65535) {
-                const int nf = nframes - f0 < 65535 ? nframes - f0 : 65535;
-                dim3 grid((b_w + MBS - 1) / MBS, b_h, nf);
-                esa2_kernel<MB, MBS><<<grid, ESA2_THREADS, smem2, st>>>(cur + (long long)f0 * fs, ref + (long long)f0 * fs, linesize, fs, b_w, b_h,
-                                                                        search, pitch, copy_words, mv + 2LL * f0 * b_w * b_h, cost + (long long)f0 * b_w * b_h);
-                B200_LAUNCHED();
-            }
-            B200_CUDA_OK(cudaGetLastError());
-            return 0;
+    // the second kernel while its four copies of the joint window fit in 100 KB of shared memory (up to search 64 for 16 x 16
+    // blocks), the first one for wider windows
+    constexpr int MBS = 2;
+    const int wc = 2 * search + MB * MBS;                    // widest joint window in bytes
+    const int pitch = (wc + 3) / 4 + 1;
+    const int trows = 2 * search + MB + ESA2_NV - 1;
+    int copy_words = trows * pitch + 1;
+    copy_words += (8 - (copy_words & 31) + 32) & 31;         // copies 8 banks apart: the four phases of 8 neighbouring columns hit 32 banks
+    const size_t smem2 = ((size_t)MBS * MB * (MB / 4) + 4 * (size_t)copy_words) * 4;
+    if (smem2 <= 100 * 1024) {
+        if (smem2 > 48 * 1024)
+            B200_CUDA_OK(cudaFuncSetAttribute(esa2_kernel<MB, MBS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
+        for (int f0 = 0; f0 < nframes; f0 += 65535) {
+            const int nf = nframes - f0 < 65535 ? nframes - f0 : 65535;
+            dim3 grid((b_w + MBS - 1) / MBS, b_h, nf);
+            esa2_kernel<MB, MBS><<<grid, ESA2_THREADS, smem2, st>>>(cur + (long long)f0 * fs, ref + (long long)f0 * fs, linesize, fs, b_w, b_h,
+                                                                    search, pitch, copy_words, mv + 2LL * f0 * b_w * b_h, cost + (long long)f0 * b_w * b_h);
+            B200_LAUNCHED();
         }
+        B200_CUDA_OK(cudaGetLastError());
+        return 0;
     }
     const int wcols = 2 * search + MB;                           // widest window in bytes
     const int win_pitch = (wcols + 3) / 4 + 1;                   // +1 word: the PRMT pair read one past the last needed word

@@ -23,14 +23,17 @@ constexpr int QW = 48;                 // window pitch in bytes (12 words: the 8
 constexpr int QX = 8;                  // so that every 8-pixel segment of a row starts 8-byte aligned in shared memory
 constexpr int WARPS = 4;
 
+// Shared memory per warp is held at 7456 bytes, which leaves room for 7 CTAs (28 warps) per SM.  The data below needs 5776 bytes, with
+// which 9 CTAs fit, and the kernel then ran 8 % slower (H100 SXM at a 400 W limit: 1.37 instead of 1.49 G blocks/s in bench.py).
+constexpr int QPEL_WARP_SMEM = 7456;
 struct __align__(16) QpelSmem {
-    uint8_t win[24 * QW];              // source rows -2 .. size+2; source column x is at byte QX + x (x = -2 .. size+2); rows 21..23: slack
-                                       // for the tensor-core path, which reads the window in blocks of 8 rows
+    uint8_t win[21 * QW];              // source rows -2 .. size+2; source column x is at byte QX + x (x = -2 .. size+2)
     short hraw[21 * 16];               // unrounded horizontal 6-tap sums for the same rows, block columns 0 .. 15
-    unsigned raw[12 * 32];             // scratch of stage_window (TMA-less single-window form): word k of lane l at raw[k * 32 + l]
-    uint8_t ring[4][16 + 21 * 48];     // qpel_kernel: raw 16-byte chunks of QD windows in flight (cp.async), window row r at ring[slot][16 + r * 48]
+    uint8_t ring[4][16 + 21 * 48];     // raw 16-byte chunks of QD windows in flight (cp.async), window row r at ring[slot][16 + r * 48]
                                        // (16 bytes of slack: the re-alignment may read the word in front of a row)
+    uint8_t pad[QPEL_WARP_SMEM - 21 * QW - 21 * 16 * 2 - 4 * (16 + 21 * 48)];   // unused: see QPEL_WARP_SMEM
 };
+static_assert(sizeof(QpelSmem) == QPEL_WARP_SMEM, "QpelSmem must keep the footprint that sets the kernel's occupancy");
 
 // ---- packed arithmetic helpers --------------------------------------------------------------------------------------
 // The 6-tap (1,-5,20,20,-5,1) is evaluated with the integer dot-product instructions: IDP.4A for the horizontal filter
@@ -96,8 +99,8 @@ __device__ __forceinline__ uint2 clip_pack8(const int *v)
 
 // The kernel is latency-bound if every operation waits for its descriptor, then its window, then (avg) its
 // destination.  Each warp therefore walks QK consecutive operations and software-pipelines them: while operation t is
-// computed, the window words of t+1 are already in flight into registers, the descriptor of t+2 is being fetched, and
-// the destination row of t (avg) was requested before the shared-memory staging started.
+// computed, the windows of the next QD - 1 operations are already in flight (below), every descriptor of the warp has been
+// fetched, and the destination row of t (avg) was requested before the shared-memory staging started.
 constexpr int QK = 32;               // operations per warp (one descriptor per lane): the start-up round trips (descriptors, first windows) are paid once per 32 blocks
 
 struct QMeta { int o; long long soff, doff; };
@@ -107,53 +110,10 @@ __device__ __forceinline__ QMeta load_meta(const uint8_t *op, const int64_t *src
     if (i < n) { m.o = __ldg(op + i); m.soff = __ldg(src_off + i); m.doff = __ldg(dst_off + i); }
     return m;
 }
-struct QWin { uint4 v[3]; unsigned sh; };
-// Window row `lane` (source row lane-2, columns -2 .. size+2) into registers: the one to three aligned 16-byte words that
-// contain at least one needed byte (nothing else is ever read), plus the byte offset of column -2 inside the first.
-__device__ __forceinline__ void load_window(QWin &w, const uint8_t *sp, long long stride, int wdim, int lane, bool valid)
-{
-    const uintptr_t first = reinterpret_cast<uintptr_t>(sp + (long long)(lane - 2) * stride - 2);
-    const uint4 *q = reinterpret_cast<const uint4 *>(first & ~(uintptr_t)15);
-    w.sh = (unsigned)(first & 15);
-    const int nv = (int)((w.sh + wdim + 15) >> 4);
-    w.v[0] = w.v[1] = w.v[2] = make_uint4(0, 0, 0, 0);
-    if (valid && lane < wdim) {
-        w.v[0] = __ldg(q);
-        if (nv > 1) w.v[1] = __ldg(q + 1);
-        if (nv > 2) w.v[2] = __ldg(q + 2);
-    }
-}
-// Each lane re-aligns its own row: raw words go through a private column of shared memory (a register array cannot be
-// indexed by the run-time word shift), come back as 7 words at the shifted position and are funnel-shifted so that block
-// column 0 sits at byte QX of the window row.  No cross-lane traffic, so no barrier between the two steps.
-__device__ __forceinline__ void stage_window(QpelSmem &s, const QWin &w, int wdim, int lane)
-{
-    if (lane >= wdim) return;
-    unsigned *raw = &s.raw[lane];
-#pragma unroll
-    for (int k = 0; k < 3; k++) {
-        raw[(4 * k + 0) * 32] = w.v[k].x; raw[(4 * k + 1) * 32] = w.v[k].y; raw[(4 * k + 2) * 32] = w.v[k].z; raw[(4 * k + 3) * 32] = w.v[k].w;
-    }
-    const int ws = (int)((w.sh + 2) >> 2) - 1;                   // window word j = raw bytes sh + 4j - 6 .. sh + 4j - 3
-    const unsigned fs = ((w.sh + 2) & 3) * 8;
-    unsigned x[7];
-#pragma unroll
-    for (int i = 0; i < 7; i++) x[i] = raw[max(ws + i, 0) * 32];   // ws + i <= 9; index -1 only feeds columns -4, -3 (unused)
-    uint4 *row = reinterpret_cast<uint4 *>(&s.win[lane * QW]);
-    row[0] = make_uint4(0u, __funnelshift_r(x[0], x[1], fs), __funnelshift_r(x[1], x[2], fs), __funnelshift_r(x[2], x[3], fs));
-    row[1] = make_uint4(__funnelshift_r(x[3], x[4], fs), __funnelshift_r(x[4], x[5], fs), __funnelshift_r(x[5], x[6], fs), 0u);
-}
-
-// Windows in flight.  One window per warp in flight (the register-staged form above) leaves the kernel bound by memory latency:
-// at 2.2 G blocks/s an SM needs ~25 windows under way and 28 resident warps provide just that — the tensor-core path computes a block
-// in half the instructions and was SLOWER with it (1.6 G blocks/s at 20 warps per SM).  So the raw 16-byte chunks now go global ->
-// shared with cp.async into a ring of QD windows per warp (no registers held while they fly), QD - 1 operations ahead of the one
-// being computed; the lane that copied a row re-aligns it out of the ring when its turn comes.
+// Windows in flight.  With one window per warp in flight the kernel is bound by memory latency, so the raw 16-byte chunks go
+// global -> shared with cp.async into a ring of QD windows per warp (no registers held while they fly), QD - 1 operations ahead of
+// the one being computed; the lane that copied a row re-aligns it out of the ring when its turn comes.
 constexpr int QD = 4;
-__device__ __forceinline__ void q_cp_async16(void *smem_dst, const void *g)
-{
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"((unsigned)__cvta_generic_to_shared(smem_dst)), "l"(g) : "memory");
-}
 __device__ __forceinline__ void q_cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void q_cp_wait() { asm volatile("cp.async.wait_group %0;" :: "n"(N) : "memory"); }
 // request window row `lane` (source row lane - 2, columns -2 .. size + 2) of one operation: the one to three aligned 16-byte words
@@ -170,7 +130,7 @@ __device__ __forceinline__ void issue_window(unsigned rl, uintptr_t first, int w
     }
     q_cp_commit();
 }
-// the lane's own row out of the ring, block column 0 moved to byte QX of the window row (same result as stage_window);
+// the lane's own row out of the ring, block column 0 moved to byte QX of the window row;
 // sh = low four bits of the row's first address, raw = the lane's row in the ring slot
 __device__ __forceinline__ void stage_from_ring(QpelSmem &s, const unsigned *raw, unsigned sh, int wdim, int lane)
 {
@@ -185,102 +145,13 @@ __device__ __forceinline__ void stage_from_ring(QpelSmem &s, const unsigned *raw
     row[1] = make_uint4(__funnelshift_r(x[3], x[4], fs), __funnelshift_r(x[4], x[5], fs), __funnelshift_r(x[5], x[6], fs), 0u);
 }
 
-// ---- 16 x 16 blocks on the tensor cores -------------------------------------------------------------------------------------------
-// The 6-tap filters are banded matrices.  With the staged window at a fixed phase (block column 0 at byte QX of a window row) the
-// horizontal filter of all 16 columns over 8 window rows is ONE mma.sync.m16n8k32:  D[x][r] = sum_k A[x][k] * B[k][r],  A[x][k] = tap[k - x - 2]
-// (s8, the same for every operation: built once per lane), B[k][r] = window byte 4 + k of row r (u8: the B fragment of a lane is two
-// aligned 32-bit loads of its row).  An A made of a single 1 per row instead (k = x + 4, or x + 5 for the +1 column positions) gives
-// the window itself in the same layout — which is what the vertical filter wants as ITS left operand:  D2[x][y] = sum_r T[x][r] * tapV[r - y].
-// A lane's accumulators of the three 8-row blocks (rows 2t, 2t+1, 8+2t, 9+2t, 16+2t, 17+2t of columns g and g + 8) are exactly six of the
-// contraction slots of its A fragment, so the first pass feeds the second straight out of registers (bytes picked by PRMT; the raw
-// horizontal sums of the centre position are split  h = 256 * hi + lo  into a signed and an unsigned byte plane, two MMAs); the matching
-// slot -> row permutation is folded into the constant B fragments of the vertical taps.  Every plane (F, H, V, J) comes out in the
-// layout  (column g / g + 8, rows 8 nb + 2t, + 1),  so rounding, clipping and the (a + b + 1) >> 1 combinations are element-wise.
-// A 16 x 16 centre position costs 6 LDS + 7 MMA + ~100 ALU per warp instead of ~370 instructions on the dot-product path.
-__device__ __forceinline__ void qmma_s8u8(int (&d)[4], const unsigned (&a)[4], unsigned b0, unsigned b1)
-{
-    asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.s8.u8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void qmma_u8s8(int (&d)[4], const unsigned (&a)[4], unsigned b0, unsigned b1)
-{
-    asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.u8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void qmma_s8s8(int (&d)[4], const unsigned (&a)[4], unsigned b0, unsigned b1)
-{
-    asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ int qtap(int j) { return j == 0 || j == 5 ? 1 : j == 1 || j == 4 ? -5 : j == 2 || j == 3 ? 20 : 0; }
-struct QmmaConst {
-    unsigned atap[4];                  // A of the horizontal filter
-    unsigned aid[2][4];                // A of the identity pick, column shift 0 / 1
-    unsigned bv[2][2];                 // B of the vertical filter for output rows 0..7 / 8..15 (contraction slots in accumulator order)
-};
-__device__ __forceinline__ void qmma_consts(QmmaConst &c, int lane)
-{
-    const int g = lane >> 2, t = lane & 3;
-#pragma unroll
-    for (int r = 0; r < 4; r++) {                                  // a0: row g, k 4t..; a1: row g + 8; a2 / a3: the same rows, k + 16
-        const int x = g + (r & 1) * 8, k0 = 4 * t + (r >> 1) * 16;
-        unsigned wt = 0, w0 = 0, w1 = 0;
-#pragma unroll
-        for (int b = 0; b < 4; b++) {
-            const int k = k0 + b;
-            wt |= ((unsigned)qtap(k - x - 2) & 0xffu) << (8 * b);   // window byte 4 + k = block column k - 4; taps start at column x - 2
-            w0 |= (k == x + 4 ? 1u : 0u) << (8 * b);
-            w1 |= (k == x + 5 ? 1u : 0u) << (8 * b);
-        }
-        c.atap[r] = wt; c.aid[0][r] = w0; c.aid[1][r] = w1;
-    }
-#pragma unroll
-    for (int nb = 0; nb < 2; nb++)
-#pragma unroll
-        for (int h = 0; h < 2; h++) {                              // b0: slots 4t .. 4t+3, b1: slots 16 + 4t .. ; column n = g -> output row 8 nb + g
-            unsigned w = 0;
-#pragma unroll
-            for (int b = 0; b < 4; b++) {
-                const int row = h == 0 ? (b < 2 ? 2 * t + b : 8 + 2 * t + (b - 2)) : (b < 2 ? 16 + 2 * t + b : 99);   // slot -> window row
-                const int j = row - (8 * nb + g);                  // output row y reads window rows y .. y + 5
-                w |= ((unsigned)(row < 24 ? qtap(j) : 0) & 0xffu) << (8 * b);
-            }
-            c.bv[nb][h] = w;
-        }
-}
-// bytes `sel` (0: bits 0..7, 1: bits 8..15) of four accumulators -> one word
-__device__ __forceinline__ unsigned qpick4(int r0, int r1, int r2, int r3, int sel)
-{
-    const unsigned s = sel ? 0x0051u : 0x0040u;
-    return __byte_perm(__byte_perm((unsigned)r0, (unsigned)r1, s), __byte_perm((unsigned)r2, (unsigned)r3, s), 0x5410);
-}
-// A fragments of the vertical pass out of the three base-0 accumulator blocks; sel picks the low or the high byte plane
-__device__ __forceinline__ void qfragV(unsigned (&a)[4], const int (&d0)[4], const int (&d1)[4], const int (&d2)[4], int sel)
-{
-    a[0] = qpick4(d0[0], d0[1], d1[0], d1[1], sel);                // column g:     rows 2t, 2t+1, 8+2t, 9+2t
-    a[1] = qpick4(d0[2], d0[3], d1[2], d1[3], sel);                // column g + 8
-    a[2] = qpick4(d2[0], d2[1], 0, 0, sel);                        // rows 16+2t, 17+2t, (no row), (no row)
-    a[3] = qpick4(d2[2], d2[3], 0, 0, sel);
-}
-
 // Lane l works on one 8-pixel (4 for size 4) row segment: row l>>1, half l&1 for 16x16.
-template <bool MMA>
 __global__ void __launch_bounds__(32 * WARPS)
 qpel_kernel(long long n, const uint8_t *op, uint8_t *dst, const int64_t *dst_off, const uint8_t *src,
             const int64_t *src_off, long long stride)
 {
     __shared__ QpelSmem sm[WARPS];
-    __shared__ unsigned qtab[16][32];                                                    // the per-lane MMA constants: [0..3] taps A, [4..7] / [8..11] pick A
-                                                                                         // (column shift 0 / 1), [12..15] vertical taps B (rows 0..7: b0 b1, 8..15: b0 b1)
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (MMA && warp == 0) {       // kept in shared memory: as loop-invariant registers ptxas rebuilt them (150 instructions) for every operation
-        QmmaConst qc;
-        qmma_consts(qc, lane);
-#pragma unroll
-        for (int r = 0; r < 4; r++) { qtab[r][lane] = qc.atap[r]; qtab[4 + r][lane] = qc.aid[0][r]; qtab[8 + r][lane] = qc.aid[1][r]; }
-        qtab[12][lane] = qc.bv[0][0]; qtab[13][lane] = qc.bv[0][1]; qtab[14][lane] = qc.bv[1][0]; qtab[15][lane] = qc.bv[1][1];
-    }
-    if (MMA) __syncthreads();
     const long long first_op = ((long long)blockIdx.x * WARPS + warp) * QK;
     if (first_op >= n) return;
     QpelSmem &s = sm[warp];
@@ -327,108 +198,6 @@ qpel_kernel(long long n, const uint8_t *op, uint8_t *dst, const int64_t *dst_off
                         ((unsigned)srcb + (unsigned)soff0) & 15u, wdim, lane);
         __syncwarp();
         const bool need_j = (qx == 2 && qy != 0) || (qy == 2 && qx != 0);                // positions built from the centre sample
-        if (MMA && size == 16) {
-            const int g = lane >> 2, tq = lane & 3;
-            const bool useF = (qy == 0 && qx != 2) || (qx == 0 && (qy & 1));
-            const bool useH = qx != 0 && qy != 2;
-            const bool useV = qy != 0 && qx != 2;
-            const int cs = qx == 3, rbase = 2 + (qy == 3);
-            unsigned aid[4] = { 0, 0, 0, 0 }, atap[4] = { 0, 0, 0, 0 }, bv[2][2] = { { 0, 0 }, { 0, 0 } };
-            if (useF || useV) {
-#pragma unroll
-                for (int r = 0; r < 4; r++) aid[r] = qtab[4 + 4 * cs + r][lane];
-            }
-            if (useH || need_j) {
-#pragma unroll
-                for (int r = 0; r < 4; r++) atap[r] = qtab[r][lane];
-            }
-            if (useV || need_j) { bv[0][0] = qtab[12][lane]; bv[0][1] = qtab[13][lane]; bv[1][0] = qtab[14][lane]; bv[1][1] = qtab[15][lane]; }
-            int res[2][4];
-            bool have = false;                                           // warp-uniform: the branch below is not divergent
-            auto add = [&](const int (&c0)[4], const int (&c1)[4]) {
-                if (have) {
-#pragma unroll
-                    for (int i = 0; i < 4; i++) { res[0][i] = (res[0][i] + c0[i] + 1) >> 1; res[1][i] = (res[1][i] + c1[i] + 1) >> 1; }
-                } else {
-#pragma unroll
-                    for (int i = 0; i < 4; i++) { res[0][i] = c0[i]; res[1][i] = c1[i]; }
-                }
-                have = true;
-            };
-            const uint8_t *wb = &s.win[g * QW + 4 + 4 * tq];            // this lane's B-fragment bytes of window row g
-            if (useF || useH) {                                          // planes taken at the output rows themselves
-                unsigned b0[2], b1[2];
-#pragma unroll
-                for (int nb = 0; nb < 2; nb++) {
-                    const uint8_t *p = wb + (rbase + 8 * nb) * QW;
-                    b0[nb] = *reinterpret_cast<const unsigned *>(p); b1[nb] = *reinterpret_cast<const unsigned *>(p + 16);
-                }
-                if (useF) {
-                    int f0[4] = { 0, 0, 0, 0 }, f1[4] = { 0, 0, 0, 0 };
-                    qmma_s8u8(f0, aid, b0[0], b1[0]); qmma_s8u8(f1, aid, b0[1], b1[1]);
-                    add(f0, f1);
-                }
-                if (useH) {
-                    int h0[4] = { 16, 16, 16, 16 }, h1[4] = { 16, 16, 16, 16 };
-                    qmma_s8u8(h0, atap, b0[0], b1[0]); qmma_s8u8(h1, atap, b0[1], b1[1]);
-#pragma unroll
-                    for (int i = 0; i < 4; i++) { h0[i] = clip8(h0[i] >> 5); h1[i] = clip8(h1[i] >> 5); }
-                    add(h0, h1);
-                }
-            }
-            if (useV || need_j) {                                        // planes filtered vertically: window rows 0 .. 20 as the contraction
-                unsigned b0[3], b1[3];
-#pragma unroll
-                for (int nb = 0; nb < 3; nb++) {
-                    const uint8_t *p = wb + (8 * nb) * QW;
-                    b0[nb] = *reinterpret_cast<const unsigned *>(p); b1[nb] = *reinterpret_cast<const unsigned *>(p + 16);
-                }
-                if (useV) {
-                    int t0[4] = { 0, 0, 0, 0 }, t1[4] = { 0, 0, 0, 0 }, t2[4] = { 0, 0, 0, 0 };
-                    qmma_s8u8(t0, aid, b0[0], b1[0]); qmma_s8u8(t1, aid, b0[1], b1[1]); qmma_s8u8(t2, aid, b0[2], b1[2]);
-                    unsigned a[4];
-                    qfragV(a, t0, t1, t2, 0);
-                    int v0[4] = { 16, 16, 16, 16 }, v1[4] = { 16, 16, 16, 16 };
-                    qmma_u8s8(v0, a, bv[0][0], bv[0][1]); qmma_u8s8(v1, a, bv[1][0], bv[1][1]);
-#pragma unroll
-                    for (int i = 0; i < 4; i++) { v0[i] = clip8(v0[i] >> 5); v1[i] = clip8(v1[i] >> 5); }
-                    add(v0, v1);
-                }
-                if (need_j) {
-                    int t0[4] = { 0, 0, 0, 0 }, t1[4] = { 0, 0, 0, 0 }, t2[4] = { 0, 0, 0, 0 };
-                    qmma_s8u8(t0, atap, b0[0], b1[0]); qmma_s8u8(t1, atap, b0[1], b1[1]); qmma_s8u8(t2, atap, b0[2], b1[2]);
-                    unsigned al[4], ah[4];
-                    qfragV(al, t0, t1, t2, 0);                           // h = 256 * (h >> 8) + (h & 255): unsigned low plane, signed high plane
-                    qfragV(ah, t0, t1, t2, 1);
-                    int jl0[4] = { 512, 512, 512, 512 }, jl1[4] = { 512, 512, 512, 512 }, jh0[4] = { 0, 0, 0, 0 }, jh1[4] = { 0, 0, 0, 0 };
-                    qmma_u8s8(jl0, al, bv[0][0], bv[0][1]); qmma_u8s8(jl1, al, bv[1][0], bv[1][1]);
-                    qmma_s8s8(jh0, ah, bv[0][0], bv[0][1]); qmma_s8s8(jh1, ah, bv[1][0], bv[1][1]);
-#pragma unroll
-                    for (int i = 0; i < 4; i++) { jl0[i] = clip8((jh0[i] * 256 + jl0[i]) >> 10); jl1[i] = clip8((jh1[i] * 256 + jl1[i]) >> 10); }
-                    add(jl0, jl1);
-                }
-            }
-            // the 16 x 16 result goes through a byte tile (the hraw array is free on this path) back to the row-segment mapping of the store
-            uint8_t *ot = reinterpret_cast<uint8_t *>(s.hraw);
-#pragma unroll
-            for (int nb = 0; nb < 2; nb++)
-#pragma unroll
-                for (int i = 0; i < 4; i++)
-                    ot[(8 * nb + 2 * tq + (i & 1)) * 16 + g + 8 * (i >> 1)] = (uint8_t)res[nb][i];
-            __syncwarp();
-            uint2 r8 = *reinterpret_cast<const uint2 *>(ot + y * 16 + x0);
-            if (vec) {
-                if (avg) { r8.x = __vavgu4(r8.x, pv.x); r8.y = __vavgu4(r8.y, pv.y); }
-                *reinterpret_cast<uint2 *>(d) = r8;
-            } else {
-                for (int k = 0; k < 8; k++) {
-                    const int v = (int)__byte_perm(k < 4 ? r8.x : r8.y, 0, 0x4440 | (k & 3));
-                    d[k] = (uint8_t)(avg ? (d[k] + v + 1) >> 1 : v);
-                }
-            }
-            __syncwarp();                                                                // tile and window are reused by the next operation
-            continue;
-        }
         if (need_j) {
             for (int k = lane; k < wdim * segs; k += 32) {
                 const int r = k / segs, xx = (k - r * segs) * 8;
@@ -501,204 +270,6 @@ qpel_kernel(long long n, const uint8_t *op, uint8_t *dst, const int64_t *dst_off
     q_cp_wait<0>();                                                                      // nothing of this warp's is in flight when it leaves
 }
 
-// ------------------------------------------------------------------------------------------------ qpel on TMA-staged windows
-// Same arithmetic as qpel_kernel; what changes is how a window reaches shared memory: one cp.async.bulk.tensor.2d (UTMALDG) per
-// operation completes on the operation's mbarrier.  A warp issues the boxes of all its TQK operations before it computes the first
-// one, so nothing of the load path runs on the LSU any more (no per-row 16-byte loads, no register -> shared staging).
-// The box origin is kept on a 16-byte column, so the box of a block at column x starts at (x - 2) & ~15 and is 48 bytes wide for 16-pixel blocks
-// (window of 21 bytes at phase 0..15) and 32 bytes for 8- and 4-pixel blocks (13 / 9 bytes); the window's byte phase inside the tile
-// row, ph = (x - 2) & 15, is folded into the word index and one funnel shift of the row readers.  Boxes that hang over the end of a
-// line are legal (the tensor map's column extent is the line pitch: the missing bytes arrive as zeros and are never used).
-// Blocks closer than 2 bytes to the start of a line or 2 rows to the start of the plane are filled by plain loads instead.
-constexpr int TQK = 8;                  // operations per warp
-constexpr int TILE_BYTES = 1024;        // 21 rows x 48 bytes, rounded up to the 128-byte alignment the copy engine wants
-struct WinT {
-    const unsigned *t;
-    int pw;                             // words per tile row (12 or 8)
-    int off0;                           // byte of block column 0 inside a tile row (ph + 2)
-    __device__ __forceinline__ unsigned w(int row, int k) const { return t[row * pw + k]; }
-};
-// 8 pixels of `row` starting at block column x0 + dx
-__device__ __forceinline__ uint2 t_row8p(const WinT &W, int row, int x0, int dx)
-{
-    const int o = W.off0 + x0 + dx, k = o >> 2;
-    const unsigned sh = (unsigned)(o & 3) * 8u;
-    const unsigned w0 = W.w(row, k), w1 = W.w(row, k + 1), w2 = W.w(row, k + 2);
-    return make_uint2(__funnelshift_r(w0, w1, sh), __funnelshift_r(w1, w2, sh));
-}
-// raw 6-tap horizontal sums of the 8 pixels at block columns x0 .. x0 + 7
-__device__ __forceinline__ void t_hsum8(const WinT &W, int row, int x0, int init, int *o)
-{
-    const int s = W.off0 + x0 - 2, k = s >> 2;
-    const unsigned q = (unsigned)(s & 3) * 8u;
-    const unsigned R[5] = { W.w(row, k), W.w(row, k + 1), W.w(row, k + 2), W.w(row, k + 3), W.w(row, k + 4) };
-    const unsigned A[4] = { __funnelshift_r(R[0], R[1], q), __funnelshift_r(R[1], R[2], q), __funnelshift_r(R[2], R[3], q), __funnelshift_r(R[3], R[4], q) };
-    unsigned S[12];                     // S[i] = window bytes i .. i + 3, byte 0 = block column x0 - 2
-#pragma unroll
-    for (int i = 0; i < 12; i++)
-        S[i] = (i & 3) ? __funnelshift_r(A[i >> 2], A[(i >> 2) + ((i >> 2) < 3 ? 1 : 0)], (i & 3) * 8) : A[i >> 2];
-#pragma unroll
-    for (int i = 0; i < 8; i++) o[i] = dp4a_us(S[i + 4], TAP4_B, dp4a_us(S[i], TAP4_A, init));
-}
-
-__device__ __forceinline__ uint32_t pel_smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void pel_mbar_wait(uint32_t a, uint32_t parity)
-{
-    uint32_t ok;
-    do {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(ok) : "r"(a), "r"(parity) : "memory");
-    } while (!ok);
-}
-__device__ __forceinline__ void pel_tma_2d(uint32_t dst, const CUtensorMap *tm, int c0, int c1, uint32_t mbar, uint32_t bytes)
-{
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(mbar), "r"(bytes) : "memory");
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-                 :: "r"(dst), "l"(tm), "r"(c0), "r"(c1), "r"(mbar) : "memory");
-}
-
-struct __align__(1024) QpelTmaSmem {
-    uint8_t tile[WARPS][TQK][TILE_BYTES];
-    short hraw[WARPS][21 * 16];
-    unsigned long long mbar[WARPS][TQK];
-};
-
-__global__ void __launch_bounds__(32 * WARPS)
-qpel_tma_kernel(const __grid_constant__ CUtensorMap tm16, const __grid_constant__ CUtensorMap tm8, const __grid_constant__ CUtensorMap tm4,
-                long long n, const uint8_t *op, uint8_t *dst, const int64_t *dst_off, const uint8_t *src, const int64_t *src_off,
-                long long stride, unsigned long long magic)
-{
-    __shared__ QpelTmaSmem sm;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const long long first_op = ((long long)blockIdx.x * WARPS + warp) * TQK;
-    if (first_op >= n) return;
-    // lanes 0 .. TQK-1 each own one operation's descriptor
-    int mo = -1, inb = 0, bx = 0, by = 0, mph = 0;
-    long long msoff = 0, mdoff = 0;
-    if (lane < TQK) {
-        const uint32_t mb = pel_smem_u32(&sm.mbar[warp][lane]);
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(mb) : "memory");
-        if (first_op + lane < n) {
-            mo = __ldg(op + first_op + lane); msoff = __ldg(src_off + first_op + lane); mdoff = __ldg(dst_off + first_op + lane);
-        }
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    __syncwarp();
-    if (mo >= 0 && msoff >= 0) {
-        // row and column of the block inside the plane: soff = y * stride + x (reciprocal multiply, corrected)
-        unsigned long long y = __umul64hi((unsigned long long)msoff, magic);
-        long long x = msoff - (long long)y * stride;
-        while (x >= stride) { x -= stride; y++; }
-        if (x >= 2 && y >= 2 && y < 0x7fffff00ULL) { inb = 1; mph = (int)(x - 2) & 15; bx = (int)(x - 2) - mph; by = (int)y - 2; }
-    }
-    // the copies are issued by one lane (TMA operands live in uniform registers): lane 0 walks the warp's operations
-    for (int k = 0; k < TQK; k++) {
-        const int kin = __shfl_sync(0xffffffffu, inb, k), kx = __shfl_sync(0xffffffffu, bx, k), ky = __shfl_sync(0xffffffffu, by, k);
-        const int ksize = 16 >> ((__shfl_sync(0xffffffffu, mo, k) >> 1) & 3);
-        if (kin && lane == 0) {
-            const CUtensorMap *tm = ksize == 16 ? &tm16 : ksize == 8 ? &tm8 : &tm4;
-            pel_tma_2d(pel_smem_u32(&sm.tile[warp][k][0]), tm, kx, ky, pel_smem_u32(&sm.mbar[warp][k]), (ksize == 16 ? 48u : 32u) * (ksize + 5));
-        }
-    }
-    short *hraw = sm.hraw[warp];
-    for (int t = 0; t < TQK; t++) {
-        const int o = __shfl_sync(0xffffffffu, mo, t);
-        if (o < 0) break;                                                                  // past the end (warp-uniform)
-        const long long doff = __shfl_sync(0xffffffffu, mdoff, t);
-        const int avg = o & 1, size = 16 >> ((o >> 1) & 3), qx = (o >> 3) & 3, qy = (o >> 5) & 3;
-        uint8_t *dp = dst + doff;
-        const int wdim = size + 5;
-        const int npx = size < 8 ? size : 8, segs = size >> 3 ? size >> 3 : 1;
-        const bool mine = lane < size * segs;
-        const int y = lane / segs, x0 = (lane - y * segs) * 8;
-        uint8_t *d = dp + (long long)y * stride + x0;
-        const bool vec = npx == 8 && ((reinterpret_cast<uintptr_t>(d)) & 7) == 0;
-        uint2 pv = make_uint2(0, 0);
-        if (mine && avg && vec) pv = *reinterpret_cast<const uint2 *>(d);                  // destination row requested early
-        uint8_t *tile = sm.tile[warp][t];
-        const int pwb = size == 16 ? 48 : 32;                                              // bytes per tile row
-        const int ph = __shfl_sync(0xffffffffu, mph, t);                                   // 0 for the plain-load fill
-        if (__shfl_sync(0xffffffffu, inb, t)) {
-            pel_mbar_wait(pel_smem_u32(&sm.mbar[warp][t]), 0);
-        } else {                                                                           // first columns / rows of the plane: plain loads
-            const long long soff = __shfl_sync(0xffffffffu, msoff, t);
-            if (lane < wdim) {
-                const uint8_t *rp = src + soff + (long long)(lane - 2) * stride - 2;
-                for (int k = 0; k < wdim; k++) tile[lane * pwb + k] = __ldg(rp + k);
-            }
-            __syncwarp();
-        }
-        const WinT W{ reinterpret_cast<const unsigned *>(tile), pwb >> 2, ph + 2 };
-        const bool need_j = (qx == 2 && qy != 0) || (qy == 2 && qx != 0);
-        if (need_j) {
-            for (int k = lane; k < wdim * segs; k += 32) {
-                const int r = k / segs, xx = (k - r * segs) * 8;
-                int h[8];
-                t_hsum8(W, r, xx, 0, h);
-                uint4 pk;
-                pk.x = __byte_perm(h[0], h[1], 0x5410); pk.y = __byte_perm(h[2], h[3], 0x5410);
-                pk.z = __byte_perm(h[4], h[5], 0x5410); pk.w = __byte_perm(h[6], h[7], 0x5410);
-                *reinterpret_cast<uint4 *>(&hraw[r * 16 + xx]) = pk;
-            }
-            __syncwarp();
-        }
-        if (mine) {
-            const bool useF = (qy == 0 && qx != 2) || (qx == 0 && (qy & 1));
-            const bool useH = qx != 0 && qy != 2;
-            const bool useV = qy != 0 && qx != 2;
-            uint2 res = make_uint2(0, 0);
-            bool have = false;
-            auto add = [&](const uint2 &c) {
-                if (have) { res.x = __vavgu4(res.x, c.x); res.y = __vavgu4(res.y, c.y); }
-                else { res = c; have = true; }
-            };
-            if (useF) add(t_row8p(W, y + 2 + (qy == 3), x0, qx == 3));
-            if (useH) {
-                int h[8];
-                t_hsum8(W, y + 2 + (qy == 3), x0, 16, h);
-                add(clip_pack8<5>(h));
-            }
-            if (useV) {
-                const int dx = qx == 3;
-                int a8[8];
-#pragma unroll
-                for (int k = 0; k < 8; k++) a8[k] = 16;
-#pragma unroll
-                for (int j = 0; j < 3; j++)
-                    vfold(tap2_16(j), t_row8p(W, y + 2 * j, x0, dx), t_row8p(W, y + 2 * j + 1, x0, dx), a8);
-                add(clip_pack8<5>(a8));
-            }
-            if (need_j) {
-                int j6[8];
-#pragma unroll
-                for (int k = 0; k < 8; k++) j6[k] = 512;
-#pragma unroll
-                for (int j = 0; j < 3; j++) {
-                    const uint4 pa = *reinterpret_cast<const uint4 *>(&hraw[(y + 2 * j) * 16 + x0]);
-                    const uint4 pb = *reinterpret_cast<const uint4 *>(&hraw[(y + 2 * j + 1) * 16 + x0]);
-                    const unsigned wa[4] = { pa.x, pa.y, pa.z, pa.w }, wb[4] = { pb.x, pb.y, pb.z, pb.w };
-#pragma unroll
-                    for (int k = 0; k < 4; k++) {
-                        j6[2 * k]     = dp2a_lo_ss(__byte_perm(wa[k], wb[k], 0x5410), tap2_8(j), j6[2 * k]);
-                        j6[2 * k + 1] = dp2a_lo_ss(__byte_perm(wa[k], wb[k], 0x7632), tap2_8(j), j6[2 * k + 1]);
-                    }
-                }
-                add(clip_pack8<10>(j6));
-            }
-            if (vec) {
-                if (avg) { res.x = __vavgu4(res.x, pv.x); res.y = __vavgu4(res.y, pv.y); }
-                *reinterpret_cast<uint2 *>(d) = res;
-            } else {
-                for (int k = 0; k < npx; k++) {
-                    const int v = (int)__byte_perm(k < 4 ? res.x : res.y, 0, 0x4440 | (k & 3));
-                    d[k] = (uint8_t)(avg ? (d[k] + v + 1) >> 1 : v);
-                }
-            }
-        }
-        __syncwarp();                                                                      // hraw is reused by the next operation
-    }
-}
-
 // hpel: one warp per operation, direct global reads (at most 4 taps per pixel, rows are contiguous)
 __global__ void __launch_bounds__(32 * WARPS)
 hpel_kernel(long long n, const uint8_t *op, const uint8_t *hh, uint8_t *dst, const int64_t *dst_off, const uint8_t *src,
@@ -752,149 +323,13 @@ __device__ __forceinline__ ChRow chroma_row(const uint8_t *p, int nbytes, bool o
     o.r0 = __funnelshift_r(t0, t1, fs); o.r1 = __funnelshift_r(t1, t2, fs); o.r2 = __funnelshift_r(t2, t3, fs);
     return o;
 }
-__global__ void __launch_bounds__(32 * WARPS)
+// CK operations per 8-lane group, with every global load of the CK windows (descriptors first, then window rows and, for avg,
+// destination rows) issued before the first result is computed: with one window per 8 lanes the kernel waits on three dependent
+// round trips to memory per operation.  CK = 2 at 8 CTAs per SM is the largest batch that fits in 64 registers without spilling.
+constexpr int CK = 2, CK_MINB = 8;
+__global__ void __launch_bounds__(32 * WARPS, CK_MINB)
 chroma_kernel(long long n, const uint8_t *op, const uint8_t *hh, const uint8_t *xy, uint8_t *dst, const int64_t *dst_off,
               const uint8_t *src, const int64_t *src_off, long long stride)
-{
-    const long long gi = ((long long)blockIdx.x * (32 * WARPS) + threadIdx.x) / CH_LANES;
-    const bool valid = gi < n;
-    const long long i = valid ? gi : n - 1;                       // every lane stays in the shuffles
-    const int sub = threadIdx.x & (CH_LANES - 1);
-    const int o = __ldg(op + i), h = __ldg(hh + i), pq = __ldg(xy + i), fx = pq & 7, fy = (pq >> 3) & 7;
-    const int avg = o & 1, w = 8 >> ((o >> 1) & 3);
-    const int kab = 4 * ((8 - fx) * (8 - fy)) | (4 * (fx * (8 - fy))) << 16;      // s16 pairs (4A, 4B) and (4C, 4D)
-    const int kcd = 4 * ((8 - fx) * fy) | (4 * (fx * fy)) << 16;
-    const uint8_t *sp = src + __ldg(src_off + i);
-    uint8_t *dp = dst + __ldg(dst_off + i);
-    const int nbytes = w + (fx != 0);
-    const int hmax = __reduce_max_sync(0xffffffffu, valid ? h : 0);   // the four operations of a warp may differ in height
-    for (int y0 = 0; y0 < hmax; y0 += CH_LANES) {
-        const int y = y0 + sub;
-        const bool mine = valid && y < h;
-        const uint8_t *rowp = sp + (long long)y * stride;
-        const ChRow t = chroma_row(rowp, nbytes, mine);
-        ChRow b;
-        b.r0 = __shfl_down_sync(0xffffffffu, t.r0, 1, CH_LANES); b.r1 = __shfl_down_sync(0xffffffffu, t.r1, 1, CH_LANES);
-        b.r2 = __shfl_down_sync(0xffffffffu, t.r2, 1, CH_LANES);
-        const bool last = sub == CH_LANES - 1 || y == h - 1;          // the row below is not held by the next lane
-        if (last) b = chroma_row(rowp + stride, nbytes, mine && fy != 0);
-        if (!mine) continue;
-        const unsigned ta = __funnelshift_r(t.r0, t.r1, 8), tb = __funnelshift_r(t.r1, t.r2, 8);
-        const unsigned ba = __funnelshift_r(b.r0, b.r1, 8), bb = __funnelshift_r(b.r1, b.r2, 8);
-        int v[8];
-        v[0] = dp2a_lo_su(kcd, b.r0, dp2a_lo_su(kab, t.r0, 128)); v[1] = dp2a_lo_su(kcd, ba, dp2a_lo_su(kab, ta, 128));
-        v[2] = dp2a_hi_su(kcd, b.r0, dp2a_hi_su(kab, t.r0, 128)); v[3] = dp2a_hi_su(kcd, ba, dp2a_hi_su(kab, ta, 128));
-        v[4] = dp2a_lo_su(kcd, b.r1, dp2a_lo_su(kab, t.r1, 128)); v[5] = dp2a_lo_su(kcd, bb, dp2a_lo_su(kab, tb, 128));
-        v[6] = dp2a_hi_su(kcd, b.r1, dp2a_hi_su(kab, t.r1, 128)); v[7] = dp2a_hi_su(kcd, bb, dp2a_hi_su(kab, tb, 128));
-        unsigned w0 = __byte_perm(__byte_perm(v[0], v[1], 0x5151), __byte_perm(v[2], v[3], 0x5151), 0x5410);
-        unsigned w1 = __byte_perm(__byte_perm(v[4], v[5], 0x5151), __byte_perm(v[6], v[7], 0x5151), 0x5410);
-        uint8_t *d = dp + (long long)y * stride;
-        const unsigned al = (unsigned)(reinterpret_cast<uintptr_t>(d) & 7);
-        if (w == 8 && al == 0) {
-            uint2 *d8 = reinterpret_cast<uint2 *>(d);
-            if (avg) { const uint2 pv = *d8; w0 = __vavgu4(pv.x, w0); w1 = __vavgu4(pv.y, w1); }
-            *d8 = make_uint2(w0, w1);
-        } else if (w >= 4 && (al & 3) == 0) {
-            unsigned *d4 = reinterpret_cast<unsigned *>(d);
-            d4[0] = avg ? __vavgu4(d4[0], w0) : w0;
-            if (w == 8) d4[1] = avg ? __vavgu4(d4[1], w1) : w1;
-        } else {
-            for (int k = 0; k < w; k++) {
-                const int px = (int)__byte_perm(k < 4 ? w0 : w1, 0, 0x4440 | (k & 3));
-                d[k] = (uint8_t)(avg ? (d[k] + px + 1) >> 1 : px);
-            }
-        }
-    }
-}
-
-// The batched form of chroma_kernel: the same arithmetic, CK operations per 8-lane group with every global load of the CK windows
-// (descriptors first, then window rows and — for avg — destination rows) issued before the first result is computed.  chroma_kernel
-// has one 9-byte window per 8 lanes in flight and three dependent round trips to memory per operation (ncu: long_scoreboard 38 per
-// issue, issue slots 32 % busy); here a warp keeps 4 * CK windows in flight.  Group g of a warp handles operations first + 4 * j + g.
-template <int CK, int MINB>
-__global__ void __launch_bounds__(32 * WARPS, MINB)
-chroma_kernel_k(long long n, const uint8_t *op, const uint8_t *hh, const uint8_t *xy, uint8_t *dst, const int64_t *dst_off,
-                const uint8_t *src, const int64_t *src_off, long long stride)
-{
-    const int lane = threadIdx.x & 31, grp = lane >> 3, sub = lane & (CH_LANES - 1);
-    const long long first = ((long long)blockIdx.x * WARPS + (threadIdx.x >> 5)) * (4 * CK);
-    if (first >= n) return;
-    int o[CK], h[CK], pq[CK];
-    long long so[CK], dof[CK];
-    bool valid[CK];
-#pragma unroll
-    for (int j = 0; j < CK; j++) {
-        const long long gi = first + 4 * j + grp;
-        valid[j] = gi < n;
-        const long long i = valid[j] ? gi : n - 1;
-        o[j] = __ldg(op + i); h[j] = __ldg(hh + i); pq[j] = __ldg(xy + i); so[j] = __ldg(src_off + i); dof[j] = __ldg(dst_off + i);
-    }
-    int hm = 0;
-#pragma unroll
-    for (int j = 0; j < CK; j++) hm = max(hm, valid[j] ? h[j] : 0);
-    const int hmax = __reduce_max_sync(0xffffffffu, hm);
-    for (int y0 = 0; y0 < hmax; y0 += CH_LANES) {
-        const int y = y0 + sub;
-        ChRow t[CK], bl[CK];
-        uint2 pv[CK];
-        bool mine[CK], vec[CK];
-        // every load of the CK windows
-#pragma unroll
-        for (int j = 0; j < CK; j++) {
-            const int fx = pq[j] & 7, fy = (pq[j] >> 3) & 7, w = 8 >> ((o[j] >> 1) & 3);
-            const int nbytes = w + (fx != 0);
-            mine[j] = valid[j] && y < h[j];
-            const uint8_t *rowp = src + so[j] + (long long)y * stride;
-            t[j] = chroma_row(rowp, nbytes, mine[j]);
-            const bool last = sub == CH_LANES - 1 || y == h[j] - 1;      // the row below is not held by the next lane
-            bl[j] = chroma_row(rowp + stride, nbytes, mine[j] && last && fy != 0);
-            const uint8_t *d = dst + dof[j] + (long long)y * stride;
-            vec[j] = w == 8 && (reinterpret_cast<uintptr_t>(d) & 7) == 0;
-            pv[j] = make_uint2(0, 0);
-            if (mine[j] && vec[j] && (o[j] & 1)) pv[j] = *reinterpret_cast<const uint2 *>(d);
-        }
-#pragma unroll
-        for (int j = 0; j < CK; j++) {
-            const int fx = pq[j] & 7, fy = (pq[j] >> 3) & 7, avg = o[j] & 1, w = 8 >> ((o[j] >> 1) & 3);
-            const int kab = 4 * ((8 - fx) * (8 - fy)) | (4 * (fx * (8 - fy))) << 16;      // s16 pairs (4A, 4B) and (4C, 4D)
-            const int kcd = 4 * ((8 - fx) * fy) | (4 * (fx * fy)) << 16;
-            ChRow b;
-            b.r0 = __shfl_down_sync(0xffffffffu, t[j].r0, 1, CH_LANES); b.r1 = __shfl_down_sync(0xffffffffu, t[j].r1, 1, CH_LANES);
-            b.r2 = __shfl_down_sync(0xffffffffu, t[j].r2, 1, CH_LANES);
-            if (sub == CH_LANES - 1 || y == h[j] - 1) b = bl[j];
-            if (!mine[j]) continue;
-            const ChRow &tt = t[j];
-            const unsigned ta = __funnelshift_r(tt.r0, tt.r1, 8), tb = __funnelshift_r(tt.r1, tt.r2, 8);
-            const unsigned ba = __funnelshift_r(b.r0, b.r1, 8), bb = __funnelshift_r(b.r1, b.r2, 8);
-            int v[8];
-            v[0] = dp2a_lo_su(kcd, b.r0, dp2a_lo_su(kab, tt.r0, 128)); v[1] = dp2a_lo_su(kcd, ba, dp2a_lo_su(kab, ta, 128));
-            v[2] = dp2a_hi_su(kcd, b.r0, dp2a_hi_su(kab, tt.r0, 128)); v[3] = dp2a_hi_su(kcd, ba, dp2a_hi_su(kab, ta, 128));
-            v[4] = dp2a_lo_su(kcd, b.r1, dp2a_lo_su(kab, tt.r1, 128)); v[5] = dp2a_lo_su(kcd, bb, dp2a_lo_su(kab, tb, 128));
-            v[6] = dp2a_hi_su(kcd, b.r1, dp2a_hi_su(kab, tt.r1, 128)); v[7] = dp2a_hi_su(kcd, bb, dp2a_hi_su(kab, tb, 128));
-            unsigned w0 = __byte_perm(__byte_perm(v[0], v[1], 0x5151), __byte_perm(v[2], v[3], 0x5151), 0x5410);
-            unsigned w1 = __byte_perm(__byte_perm(v[4], v[5], 0x5151), __byte_perm(v[6], v[7], 0x5151), 0x5410);
-            uint8_t *d = dst + dof[j] + (long long)y * stride;
-            if (vec[j]) {
-                if (avg) { w0 = __vavgu4(pv[j].x, w0); w1 = __vavgu4(pv[j].y, w1); }
-                *reinterpret_cast<uint2 *>(d) = make_uint2(w0, w1);
-            } else if (w >= 4 && (reinterpret_cast<uintptr_t>(d) & 3) == 0) {
-                unsigned *d4 = reinterpret_cast<unsigned *>(d);
-                d4[0] = avg ? __vavgu4(d4[0], w0) : w0;
-                if (w == 8) d4[1] = avg ? __vavgu4(d4[1], w1) : w1;
-            } else {
-                for (int k = 0; k < w; k++) {
-                    const int px = (int)__byte_perm(k < 4 ? w0 : w1, 0, 0x4440 | (k & 3));
-                    d[k] = (uint8_t)(avg ? (d[k] + px + 1) >> 1 : px);
-                }
-            }
-        }
-    }
-}
-
-template <int CK, int MINB>
-__global__ void __launch_bounds__(32 * WARPS, MINB)
-chroma_kernel_p(long long n, const uint8_t *op, const uint8_t *hh, const uint8_t *xy, uint8_t *dst, const int64_t *dst_off,
-                const uint8_t *src, const int64_t *src_off, long long stride)
 {
     const int lane = threadIdx.x & 31, grp = lane >> 3, sub = lane & (CH_LANES - 1);
     // persistent warps: batch b = 4 * CK consecutive operations; the descriptors of the next batch are requested before this one is
@@ -988,124 +423,6 @@ chroma_kernel_p(long long n, const uint8_t *op, const uint8_t *hh, const uint8_t
     }
 }
 
-// ------------------------------------------------------------------------------------------------ h264chroma on TMA-staged windows
-// Same arithmetic as chroma_kernel.  Every operation's source window arrives as one cp.async.bulk.tensor.2d box of 32 bytes x
-// (h + 1) rows (h rows when y == 0: the row below the block is never touched then, as in the reference) whose origin is the block's
-// row and its column rounded down to 16 (the copy engine only takes 16-byte-aligned box columns, see the qpel kernel above): the 9
-// window bytes sit at phase ph = x & 15 of each 32-byte tile row, and the row readers fold ph into a word index and one funnel shift.
-// A warp owns CQ x 4 operations (8 lanes each, lane = row) and issues all their boxes before it computes the first: 16 windows in
-// flight per warp.  Heights other than 2 / 4 / 8 / 16 take plain loads into the same tile.  The box may read up to 31 bytes around
-// the reference's own window inside the line (zeros beyond the line pitch).
-constexpr int CQ = 4;                   // operations per 8-lane group
-constexpr int CTILE = 640;              // 17 rows x 32 bytes, rounded to the 128-byte alignment TMA wants
-struct ChromaMaps { CUtensorMap m[8]; };                                // [2 * log2(h / 2) + (y != 0)]: box heights 2,3, 4,5, 8,9, 16,17
-struct __align__(128) ChromaTmaSmem {
-    uint8_t tile[WARPS][4 * CQ][CTILE];
-    unsigned long long mbar[WARPS][4 * CQ];
-};
-
-__global__ void __launch_bounds__(32 * WARPS)
-chroma_tma_kernel(const __grid_constant__ ChromaMaps maps, long long n, const uint8_t *op, const uint8_t *hh, const uint8_t *xy, uint8_t *dst,
-                  const int64_t *dst_off, const uint8_t *src, const int64_t *src_off, long long stride, unsigned long long magic)
-{
-    __shared__ ChromaTmaSmem sm;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, grp = lane >> 3, sub = lane & 7;
-    constexpr int PER_WARP = 4 * CQ;
-    const long long first_op = ((long long)blockIdx.x * WARPS + warp) * PER_WARP;
-    if (first_op >= n) return;
-    // lanes 0 .. 15 own one operation's descriptor each (slot = lane: group lane / CQ, round lane % CQ) and issue its box
-    int mo = -1, mh = 0, mpq = 0, inb = 0, bx = 0, by = 0, mph = 0;
-    long long msoff = 0, mdoff = 0;
-    if (lane < PER_WARP) {
-        const uint32_t mb = pel_smem_u32(&sm.mbar[warp][lane]);
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(mb) : "memory");
-        const long long i = first_op + lane;
-        if (i < n) { mo = __ldg(op + i); mh = __ldg(hh + i); mpq = __ldg(xy + i); msoff = __ldg(src_off + i); mdoff = __ldg(dst_off + i); }
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    __syncwarp();
-    if (mo >= 0 && msoff >= 0 && (mh == 2 || mh == 4 || mh == 8 || mh == 16)) {
-        unsigned long long y = __umul64hi((unsigned long long)msoff, magic);
-        long long x = msoff - (long long)y * stride;
-        while (x >= stride) { x -= stride; y++; }
-        if (y < 0x7fffff00ULL) { inb = 1; mph = (int)x & 15; bx = (int)x - mph; by = (int)y; }
-    }
-    for (int k = 0; k < PER_WARP; k++) {                            // issued by one lane: TMA operands live in uniform registers
-        const int kin = __shfl_sync(0xffffffffu, inb, k), kx = __shfl_sync(0xffffffffu, bx, k), ky = __shfl_sync(0xffffffffu, by, k);
-        const int kh = __shfl_sync(0xffffffffu, mh, k), kfy = (__shfl_sync(0xffffffffu, mpq, k) >> 3) & 7;
-        if (kin && lane == 0) {
-            const int rows = kh + (kfy != 0);
-            const int mi = 2 * (kh == 2 ? 0 : kh == 4 ? 1 : kh == 8 ? 2 : 3) + (kfy != 0);
-            pel_tma_2d(pel_smem_u32(&sm.tile[warp][k][0]), &maps.m[mi], kx, ky, pel_smem_u32(&sm.mbar[warp][k]), 32u * rows);
-        }
-    }
-    for (int r = 0; r < CQ; r++) {
-        const int slot = grp * CQ + r;
-        const int o = __shfl_sync(0xffffffffu, mo, slot);
-        const bool valid = o >= 0;
-        const int h = __shfl_sync(0xffffffffu, mh, slot), pq = __shfl_sync(0xffffffffu, mpq, slot);
-        const long long doff = __shfl_sync(0xffffffffu, mdoff, slot), soff = __shfl_sync(0xffffffffu, msoff, slot);
-        const int tma = __shfl_sync(0xffffffffu, inb, slot);
-        const int ph = __shfl_sync(0xffffffffu, mph, slot);                               // 0 for the plain-load fill
-        const int fx = pq & 7, fy = (pq >> 3) & 7;
-        const int avg = o & 1, w = 8 >> ((o >> 1) & 3);
-        const int kab = 4 * ((8 - fx) * (8 - fy)) | (4 * (fx * (8 - fy))) << 16;      // s16 pairs (4A, 4B) and (4C, 4D)
-        const int kcd = 4 * ((8 - fx) * fy) | (4 * (fx * fy)) << 16;
-        uint8_t *dp = dst + doff;
-        uint8_t *tile = sm.tile[warp][slot];
-        const int nbytes = w + (fx != 0);
-        if (valid && tma) pel_mbar_wait(pel_smem_u32(&sm.mbar[warp][slot]), 0);
-        if (!valid) continue;
-        for (int y0 = 0; y0 < h; y0 += 16) {
-            if (!tma) {                                                                  // plain loads: rows y0 .. y0 + 16 of the window
-                __syncwarp(0xffu << (8 * grp));
-                const int rows = min(h - y0, 16) + (fy != 0);
-                for (int rr = sub; rr < rows; rr += 8) {
-                    const uint8_t *rp = src + soff + (long long)(y0 + rr) * stride;
-                    for (int k = 0; k < nbytes; k++) tile[rr * 32 + k] = __ldg(rp + k);
-                }
-                __syncwarp(0xffu << (8 * grp));
-            }
-#pragma unroll 1
-            for (int yy = sub; yy < min(h - y0, 16); yy += 8) {
-                uint4 tq, bq;                                                            // .x .y .z = window bytes 0..3, 4..7, 8..11
-                {
-                    const unsigned *tw = reinterpret_cast<const unsigned *>(tile + yy * 32) + (ph >> 2), *bw = tw + 8;
-                    const unsigned sh = (unsigned)(ph & 3) * 8u;
-                    const unsigned t0 = tw[0], t1 = tw[1], t2 = tw[2], t3 = tw[3], b0 = bw[0], b1 = bw[1], b2 = bw[2], b3 = bw[3];
-                    tq.x = __funnelshift_r(t0, t1, sh); tq.y = __funnelshift_r(t1, t2, sh); tq.z = __funnelshift_r(t2, t3, sh); tq.w = 0;
-                    bq.x = __funnelshift_r(b0, b1, sh); bq.y = __funnelshift_r(b1, b2, sh); bq.z = __funnelshift_r(b2, b3, sh); bq.w = 0;
-                }
-                const unsigned ta = __funnelshift_r(tq.x, tq.y, 8), tb = __funnelshift_r(tq.y, tq.z, 8);
-                const unsigned ba = __funnelshift_r(bq.x, bq.y, 8), bb = __funnelshift_r(bq.y, bq.z, 8);
-                int v[8];
-                v[0] = dp2a_lo_su(kcd, bq.x, dp2a_lo_su(kab, tq.x, 128)); v[1] = dp2a_lo_su(kcd, ba, dp2a_lo_su(kab, ta, 128));
-                v[2] = dp2a_hi_su(kcd, bq.x, dp2a_hi_su(kab, tq.x, 128)); v[3] = dp2a_hi_su(kcd, ba, dp2a_hi_su(kab, ta, 128));
-                v[4] = dp2a_lo_su(kcd, bq.y, dp2a_lo_su(kab, tq.y, 128)); v[5] = dp2a_lo_su(kcd, bb, dp2a_lo_su(kab, tb, 128));
-                v[6] = dp2a_hi_su(kcd, bq.y, dp2a_hi_su(kab, tq.y, 128)); v[7] = dp2a_hi_su(kcd, bb, dp2a_hi_su(kab, tb, 128));
-                unsigned w0 = __byte_perm(__byte_perm(v[0], v[1], 0x5151), __byte_perm(v[2], v[3], 0x5151), 0x5410);
-                unsigned w1 = __byte_perm(__byte_perm(v[4], v[5], 0x5151), __byte_perm(v[6], v[7], 0x5151), 0x5410);
-                uint8_t *d = dp + (long long)(y0 + yy) * stride;
-                const unsigned al = (unsigned)(reinterpret_cast<uintptr_t>(d) & 7);
-                if (w == 8 && al == 0) {
-                    uint2 *d8 = reinterpret_cast<uint2 *>(d);
-                    if (avg) { const uint2 pv = *d8; w0 = __vavgu4(pv.x, w0); w1 = __vavgu4(pv.y, w1); }
-                    *d8 = make_uint2(w0, w1);
-                } else if (w >= 4 && (al & 3) == 0) {
-                    unsigned *d4 = reinterpret_cast<unsigned *>(d);
-                    d4[0] = avg ? __vavgu4(d4[0], w0) : w0;
-                    if (w == 8) d4[1] = avg ? __vavgu4(d4[1], w1) : w1;
-                } else {
-                    for (int k = 0; k < w; k++) {
-                        const int px = (int)__byte_perm(k < 4 ? w0 : w1, 0, 0x4440 | (k & 3));
-                        d[k] = (uint8_t)(avg ? (d[k] + px + 1) >> 1 : px);
-                    }
-                }
-            }
-        }
-    }
-}
-
 // emulated_edge_mc (videodsp_template.c:24-101) as a clamped gather: one warp per window, lanes across columns.
 // geom[4*i..] = block_w, block_h, src_x, src_y; origin[i] = offset of that picture's sample (0, 0) from `src`.
 __global__ void __launch_bounds__(32 * WARPS)
@@ -1126,6 +443,32 @@ edge_kernel(long long n, uint8_t *buf, const int64_t *buf_off, long long buf_ls,
             out[(long long)y * buf_ls + x] = __ldg(pic + (long long)py * src_ls + px);
         }
     }
+}
+
+// The dot-product form is the one qpel path: the filter arithmetic is a minority of the instructions per block, the rest is per-block
+// scaffolding (descriptor shuffles, window re-alignment, destination addressing, stores), so moving the filters to the tensor cores
+// does not pay.  Windows arrive by cp.async rather than TMA: small 2-D boxes (one 48 x 21-byte box per operation) are bound by the
+// copy engine's per-row requests, not by the LSU they bypass.
+int qpel_launch(cudaStream_t st, int64_t n, const uint8_t *op, uint8_t *dst, const int64_t *dst_off, const uint8_t *src,
+                const int64_t *src_off, ptrdiff_t stride)
+{
+    const long long blocks = (n + WARPS * QK - 1) / (WARPS * QK);
+    if (blocks > 0x7fffffffLL) return B200_EINVAL;
+    qpel_kernel<<<(unsigned)blocks, 32 * WARPS, 0, st>>>(n, op, dst, dst_off, src, src_off, stride);
+    B200_LAUNCHED();
+    B200_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+// persistent warps: one per batch of 4 * CK operations, at most CK_MINB CTAs per SM (sms = the device's SM count)
+int chroma_launch(cudaStream_t st, int sms, int64_t n, const uint8_t *op, const uint8_t *h, const uint8_t *xy, uint8_t *dst,
+                  const int64_t *dst_off, const uint8_t *src, const int64_t *src_off, ptrdiff_t stride)
+{
+    const long long nbatch = (n + 4 * CK - 1) / (4 * CK), want = (nbatch + WARPS - 1) / WARPS, cap = (long long)sms * CK_MINB;
+    chroma_kernel<<<(unsigned)(want < cap ? want : cap), 32 * WARPS, 0, st>>>(n, op, h, xy, dst, dst_off, src, src_off, stride);
+    B200_LAUNCHED();
+    B200_CUDA_OK(cudaGetLastError());
+    return 0;
 }
 
 void die(const char *what)
@@ -1161,10 +504,11 @@ void host_op(HostKind kind, int o, int h, int w, uint8_t *dst, const uint8_t *sr
     const int64_t *doff = (const int64_t *)meta, *soff = doff + 1;
     const uint8_t *dop = meta + 16, *dh = meta + 17, *dxy = meta + 18;
     // dst and src live in one buffer with the same pitch, like the reference's single stride
-    if (kind == HOST_QPEL)      qpel_kernel<true><<<1, 32 * WARPS, 0, st>>>(1, dop, ddst, doff, dsrc, soff, (long long)pitch);
-    else if (kind == HOST_HPEL) hpel_kernel<<<1, 32 * WARPS, 0, st>>>(1, dop, dh, ddst, doff, dsrc, soff, (long long)pitch);
-    else                        chroma_kernel<<<1, 32 * WARPS, 0, st>>>(1, dop, dh, dxy, ddst, doff, dsrc, soff, (long long)pitch);
-    B200_LAUNCHED();
+    int err = 0;
+    if (kind == HOST_QPEL)        err = qpel_launch(st, 1, dop, ddst, doff, dsrc, soff, pitch);
+    else if (kind == HOST_CHROMA) err = chroma_launch(st, dev->sm_count, 1, dop, dh, dxy, ddst, doff, dsrc, soff, pitch);
+    else { hpel_kernel<<<1, 32 * WARPS, 0, st>>>(1, dop, dh, ddst, doff, dsrc, soff, (long long)pitch); B200_LAUNCHED(); }
+    if (err) die("launch");
     if (b200_d2h_rows(dst, stride, ddst, pitch, w, h, st) != cudaSuccess) die("d2h");
     if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
 }
@@ -1304,81 +648,7 @@ B200_API int b200_h264chroma_batch_device(B200Device *dev, int64_t n, const uint
     if (!dev || n < 0 || !op || !h || !xy || !dst || !dst_off || !src || !src_off) return B200_EINVAL;
     if (n == 0) return 0;
     B200_CUDA_OK(cudaSetDevice(dev->ordinal));
-    static int mode = -1;                                         // B200_CHROMA_TMA: 0 (default) batched LDG kernel, 1 TMA boxes, 2 one-window LDG kernel
-    if (mode < 0) { const char *e = getenv("B200_CHROMA_TMA"); mode = e ? atoi(e) : 0; }
-    ChromaMaps maps;
-    bool tma = mode == 1 && stride >= 32;
-    for (int k = 0; k < 8 && tma; k++)
-        tma = b200_tmap_2d_u8(&maps.m[k], src, (unsigned long long)stride, 32, (2u << (k >> 1)) + (k & 1), (int)CU_TENSOR_MAP_SWIZZLE_NONE);
-    if (tma) {
-        const long long blocks = (n + WARPS * 4 * CQ - 1) / (WARPS * 4 * CQ);
-        if (blocks > 0x7fffffffLL) return B200_EINVAL;
-        chroma_tma_kernel<<<(unsigned)blocks, 32 * WARPS, 0, dev->stream>>>(maps, n, op, h, xy, dst, dst_off, src, src_off, stride,
-                                                                            ~0ULL / (unsigned long long)stride);
-    } else if (mode == 0) {
-        static int var = -1;                                      // tuning knob: windows per 8-lane group / register budget
-        // measured (scripts/quick_bench.py chroma, fraction of the HBM roofline): one-shot warps 0 -> 0.239, 1 -> 0.247, 2 -> 0.253, 3 -> 0.177;
-        // persistent warps that request the next batch's descriptors before working on the current one: <4,4> (121 registers) 0.264,
-        // <2,8> (64 registers, no spills) 0.277 = the default; every persistent shape that spills (<4,8>, <4,6>, <3,8>, <2,10>, <2,12>) loses
-        if (var < 0) { const char *e = getenv("B200_CHROMA_VAR"); var = e ? atoi(e) : 7; }
-        const int ck = var == 1 ? 2 : var == 3 ? 8 : 4;
-        const int per_cta = WARPS * 4 * ck;
-        const long long blocks = (n + per_cta - 1) / per_cta;
-        if (blocks > 0x7fffffffLL) return B200_EINVAL;
-        if (var == 6 || var == 7) {                                // persistent warps with the next batch's descriptors in flight
-            int sms = 132;
-            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev->ordinal);
-            const int ckp = var == 7 ? 2 : 4, minb = var == 7 ? 8 : 4;
-            const long long nbatch = (n + 4 * ckp - 1) / (4 * ckp), want = (nbatch + WARPS - 1) / WARPS;
-            const long long cap = (long long)sms * minb;
-            const unsigned g = (unsigned)(want < cap ? want : cap);
-            if (var == 6) chroma_kernel_p<4, 4><<<g, 32 * WARPS, 0, dev->stream>>>(n, op, h, xy, dst, dst_off, src, src_off, stride);
-            else          chroma_kernel_p<2, 8><<<g, 32 * WARPS, 0, dev->stream>>>(n, op, h, xy, dst, dst_off, src, src_off, stride);
-        }
-        else if (var == 1) chroma_kernel_k<2, 12><<<(unsigned)blocks, 32 * WARPS, 0, dev->stream>>>(n, op, h, xy, dst, dst_off, src, src_off, stride);
-        else if (var == 2) chroma_kernel_k<4, 8><<<(unsigned)blocks, 32 * WARPS, 0, dev->stream>>>(n, op, h, xy, dst, dst_off, src, src_off, stride);
-        else if (var == 3) chroma_kernel_k<8, 2><<<(unsigned)blocks, 32 * WARPS, 0, dev->stream>>>(n, op, h, xy, dst, dst_off, src, src_off, stride);
-        else               chroma_kernel_k<4, 4><<<(unsigned)blocks, 32 * WARPS, 0, dev->stream>>>(n, op, h, xy, dst, dst_off, src, src_off, stride);
-    } else {
-        const int per_cta = 32 * WARPS / CH_LANES;
-        const long long blocks = (n + per_cta - 1) / per_cta;
-        if (blocks > 0x7fffffffLL) return B200_EINVAL;
-        chroma_kernel<<<(unsigned)blocks, 32 * WARPS, 0, dev->stream>>>(n, op, h, xy, dst, dst_off, src, src_off, stride);
-    }
-    B200_LAUNCHED();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
-}
-
-// B200_QPEL_TMA: 0 (default) = LDG-staged kernel, 1 = TMA boxes.  Both are bit-exact; the LDG form is the default because small 2-D
-// boxes (one 48 x 21-byte box per operation) are bound by the copy engine's per-row requests, not by the LSU they bypass.
-static int qpel_launch(cudaStream_t st, int64_t n, const uint8_t *op, uint8_t *dst, const int64_t *dst_off, const uint8_t *src,
-                       const int64_t *src_off, ptrdiff_t stride)
-{
-    static int mode = -1;
-    if (mode < 0) { const char *e = getenv("B200_QPEL_TMA"); mode = e ? atoi(e) : 0; }
-    CUtensorMap tm16, tm8, tm4;
-    const int swz = (int)CU_TENSOR_MAP_SWIZZLE_NONE;
-    if (mode > 0 && stride >= 48 && b200_tmap_2d_u8(&tm16, src, (unsigned long long)stride, 48, 21, swz) &&
-        b200_tmap_2d_u8(&tm8, src, (unsigned long long)stride, 32, 13, swz) && b200_tmap_2d_u8(&tm4, src, (unsigned long long)stride, 32, 9, swz)) {
-        const long long blocks = (n + WARPS * TQK - 1) / (WARPS * TQK);
-        if (blocks > 0x7fffffffLL) return B200_EINVAL;
-        const unsigned long long magic = ~0ULL / (unsigned long long)stride;              // floor((2^64 - 1) / stride): the quotient estimate is never too large
-        qpel_tma_kernel<<<(unsigned)blocks, 32 * WARPS, 0, st>>>(tm16, tm8, tm4, n, op, dst, dst_off, src, src_off, stride, magic);
-    } else {
-        const long long blocks = (n + WARPS * QK - 1) / (WARPS * QK);
-        if (blocks > 0x7fffffffLL) return B200_EINVAL;
-        // B200_QPEL_MMA=1: 16 x 16 blocks on the tensor cores, bit-exact.  The filter arithmetic is a minority of the instructions per
-        // block on either path, the rest is per-block scaffolding (descriptor shuffles, window re-alignment, destination addressing,
-        // stores), so the dot-product path stays the default.
-        static int mma = -1;
-        if (mma < 0) { const char *e = getenv("B200_QPEL_MMA"); mma = e ? atoi(e) : 0; }
-        if (mma) qpel_kernel<true><<<(unsigned)blocks, 32 * WARPS, 0, st>>>(n, op, dst, dst_off, src, src_off, stride);
-        else     qpel_kernel<false><<<(unsigned)blocks, 32 * WARPS, 0, st>>>(n, op, dst, dst_off, src, src_off, stride);
-    }
-    B200_LAUNCHED();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    return chroma_launch(dev->stream, dev->sm_count, n, op, h, xy, dst, dst_off, src, src_off, stride);
 }
 
 B200_API int b200_h264qpel_batch_device(B200Device *dev, int64_t n, const uint8_t *op, uint8_t *dst, const int64_t *dst_off,
@@ -1434,13 +704,9 @@ B200_API int b200_h264qpel_frames_host(B200Device *dev, int nframes, int64_t fra
             B200_CUDA_OK(cudaMemcpyAsync(ddo, dst_off + o0, (size_t)n * 8, cudaMemcpyHostToDevice, st));
             B200_CUDA_OK(cudaMemcpyAsync(dso, src_off + o0, (size_t)n * 8, cudaMemcpyHostToDevice, st));
             B200_CUDA_OK(cudaMemcpyAsync(dop, op + o0, (size_t)n, cudaMemcpyHostToDevice, st));
-            const long long blocks = (n + WARPS * QK - 1) / (WARPS * QK);
-            if (blocks > 0x7fffffffLL) return B200_EINVAL;
             // the lists keep their offsets from the start of the whole buffers: hand the kernel bases moved back by the chunk's origin
-            qpel_kernel<true><<<(unsigned)blocks, 32 * WARPS, 0, st>>>(n, dop, ddst - (size_t)f0 * frame_bytes, ddo,
-                                                                 dsrc - (size_t)f0 * frame_bytes, dso, stride);
-            B200_LAUNCHED();
-            B200_CUDA_OK(cudaGetLastError());
+            const int r = qpel_launch(st, n, dop, ddst - (size_t)f0 * frame_bytes, ddo, dsrc - (size_t)f0 * frame_bytes, dso, stride);
+            if (r) return r;
         }
         B200_CUDA_OK(cudaMemcpyAsync(dst + (size_t)f0 * frame_bytes, ddst, (size_t)nf * frame_bytes, cudaMemcpyDeviceToHost, st));
     }

@@ -1050,7 +1050,7 @@ static int upload_tables(B200SwsContext *c)
         if (sl > 60000 || sc > 60000) c->fast_x = false;         // (2^18 + 32640 * sum|coef|) must stay below 2^31
         if (p.vLum.size != 1 || p.vLum.coef[y] != 4096) c->lum_identity = false;
     }
-    c->pair_ok = c->fast_x && c->lum_identity && p.vChr.size == 4 && p.dstH >= 4 && !getenv("B200_SWS_NO_PAIR");
+    c->pair_ok = c->fast_x && c->lum_identity && p.vChr.size == 4 && p.dstH >= 4;
     for (int y = 1; y + 1 < p.dstH && c->pair_ok; y += 2)
         if (p.vChr.pos[y] != p.vChr.pos[y + 1]) c->pair_ok = false;
     return upload_mma_tables(c);
@@ -1531,21 +1531,6 @@ static int fused_rows_needed(const SwsFilterBank &v, int srcH, int dstH, int TR)
     }
     return mx;
 }
-// B200_SWS_FUSED: 0 = two passes through int16 line planes, 1 = fused CUDA-core kernels, 2 (default) = fused with the tensor-core horizontal pass
-static int fused_mode()
-{
-    static int on = -1;
-    if (on < 0) { const char *e = getenv("B200_SWS_FUSED"); on = e ? atoi(e) : 2; }
-    return on;
-}
-static bool fused_enabled() { return fused_mode() != 0; }
-static int fused_tr(int dflt)
-{
-    static int tr = -1;
-    if (tr < 0) { const char *e = getenv("B200_SWS_TR"); tr = e ? atoi(e) : 0; }
-    return tr > 0 ? tr : dflt;
-}
-
 static bool aligned16(const void *p, long long stride, long long fstride)
 {
     return (((uintptr_t)p) & 15) == 0 && (stride & 15) == 0 && (fstride & 15) == 0;
@@ -1765,7 +1750,7 @@ static int launch_batch(B200SwsContext *c, cudaStream_t stream, const uint8_t *c
             }
         } else {
             // scaled path.  Whole frames through the `_X` writer: one fused kernel (no int16 planes in HBM)
-            if (!rows && fused_mode() == 2 && c->mma_tables && p.chrDstHSub && c->all_x && p.dstW % 16 == 0 && p.chrDstW * 2 == p.dstW &&
+            if (!rows && c->mma_tables && p.chrDstHSub && c->all_x && p.dstW % 16 == 0 && p.chrDstW * 2 == p.dstW &&
                 aligned16(dst, ds, dfs) && aligned16(b.y, b.ys, b.yfs) && aligned16(b.u, b.us, b.ufs) && aligned16(b.v, b.vs, b.vfs)) {
                 auto need = [&](int rl_, int rc_) {
                     const size_t RL = (size_t)((rl_ + 15) & ~15), RC = (size_t)((rc_ + 15) & ~15);
@@ -1775,7 +1760,7 @@ static int launch_batch(B200SwsContext *c, cudaStream_t stream, const uint8_t *c
                 // fewest of them (e.g. 29 lines at 2:1 with 8 taps = exactly 64 source lines) among those that leave room for 4 CTAs per SM
                 // (measured, 4K -> 1080p rgb24: 16 lines 0.197 of the HBM roofline, 29 lines 0.179 — three planes' tiles leave 2 CTAs per SM —
                 // 13 lines 0.172: 16 is tried first, the search below only runs when 16 does not fit)
-                int TR = fused_tr(16), rl = -1, rc = -1;
+                int TR = 16, rl = -1, rc = -1;
                 rl = fused_rows_needed(p.vLum, p.srcH, p.dstH, TR); rc = fused_rows_needed(p.vChr, p.chrSrcH, p.dstH, TR);
                 if (rl <= 0 || rc <= 0 || need(rl, rc) > 80 * 1024) {
                     TR = 0; rl = rc = -1;
@@ -1813,7 +1798,7 @@ static int launch_batch(B200SwsContext *c, cudaStream_t stream, const uint8_t *c
                     continue;
                 }
             }
-            if (!rows && fused_enabled() && !p.fast_bilinear && p.chrDstHSub && c->all_x && p.dstW % 8 == 0 && aligned16(dst, ds, dfs) &&
+            if (!rows && !p.fast_bilinear && p.chrDstHSub && c->all_x && p.dstW % 8 == 0 && aligned16(dst, ds, dfs) &&
                 p.hLum.size <= 16 && p.hChr.size <= 16) {
                 int TR = 32;
                 int rl = fused_rows_needed(p.vLum, p.srcH, p.dstH, TR), rc = fused_rows_needed(p.vChr, p.chrSrcH, p.dstH, TR);
@@ -2155,23 +2140,20 @@ static int launch_planar3(B200SwsContext *c, cudaStream_t stream, const uint8_t 
                 // fused horizontal + vertical pass for this plane when the writer below would be the 8-sample one
                 uint8_t *dplf = dst[pl] + (long long)f0 * dfs[pl];
                 const SwsFilterBank &vb = pl ? p.vChr : p.vLum;
-                const bool m8 = fused_mode() == 2 && c->mma_tables && !p.range_conv && dw[pl] % 8 == 0 &&
+                const bool m8 = c->mma_tables && !p.range_conv && dw[pl] % 8 == 0 &&
                                 (((uintptr_t)dplf | (uintptr_t)dstr[pl] | (uintptr_t)dfs[pl]) & 7) == 0 &&
                                 aligned16(src[pl] + (long long)f0 * sfs[pl], sstr[pl], sfs[pl]);
                 if (m8) {
                     const SwsFilterBank &vbm = pl ? p.vChr : p.vLum;
                     const int SP = pl ? c->mma_pitchC : c->mma_pitchL;
                     auto needb = [&](int r) { return MT_HDR + (size_t)((r + 15) & ~15) * (SP + MT_TPB); };
-                    int TRm = fused_tr(0), nr = -1;
-                    if (TRm > 0) nr = fused_rows_needed(vbm, sh[pl], dh[pl], TRm);
-                    else {
-                        double best = 1e30;
-                        for (int cand = 32; cand >= 8; cand--) {                   // see the packed-RGB launch: fewest wasted 16-line blocks
-                            const int a_ = fused_rows_needed(vbm, sh[pl], dh[pl], cand);
-                            if (a_ <= 0 || needb(a_) > 112 * 1024) continue;
-                            const double cost = (double)((a_ + 15) >> 4) / cand * (1.0 + (needb(a_) > 56 * 1024 ? 0.15 : 0.0) + (needb(a_) > 75 * 1024 ? 0.15 : 0.0));
-                            if (cost < best - 1e-9) { best = cost; TRm = cand; nr = a_; }
-                        }
+                    int TRm = 0, nr = -1;
+                    double best = 1e30;
+                    for (int cand = 32; cand >= 8; cand--) {                       // see the packed-RGB launch: fewest wasted 16-line blocks
+                        const int a_ = fused_rows_needed(vbm, sh[pl], dh[pl], cand);
+                        if (a_ <= 0 || needb(a_) > 112 * 1024) continue;
+                        const double cost = (double)((a_ + 15) >> 4) / cand * (1.0 + (needb(a_) > 56 * 1024 ? 0.15 : 0.0) + (needb(a_) > 75 * 1024 ? 0.15 : 0.0));
+                        if (cost < best - 1e-9) { best = cost; TRm = cand; nr = a_; }
                     }
                     if (nr > 0 && needb(nr) <= 112 * 1024) {
                         const size_t smem = needb(nr);
@@ -2185,7 +2167,7 @@ static int launch_planar3(B200SwsContext *c, cudaStream_t stream, const uint8_t 
                         continue;
                     }
                 }
-                const bool f8 = fused_enabled() && !p.range_conv && hs[pl] <= 16 && dw[pl] % 8 == 0 &&
+                const bool f8 = !p.range_conv && hs[pl] <= 16 && dw[pl] % 8 == 0 &&
                                 (((uintptr_t)dplf | (uintptr_t)dstr[pl] | (uintptr_t)dfs[pl]) & 7) == 0;
                 int TR = 32, need_rows = f8 ? fused_rows_needed(vb, sh[pl], dh[pl], TR) : -1;
                 if (need_rows > 96) { TR = 16; need_rows = fused_rows_needed(vb, sh[pl], dh[pl], TR); }

@@ -574,10 +574,6 @@ static int tx_build(B200TXContext *c, float scale)
     d.leaf16 = (const int *)(b + o_l16); d.n_leaf16 = (int)leaf16.size();
     d.leaf8 = (const int *)(b + o_l8); d.n_leaf8 = (int)leaf8.size();
     c->tb = n <= 1024 ? 4 : n <= 2048 ? 2 : 1;                     // transforms per CTA (about 35 KB of shared memory up to n = 2048)
-    if (const char *e = getenv("B200_TX_TB")) {                    // tuning knob (1, 2 or 4); the default above is what the bench uses
-        const int v = atoi(e);
-        if ((v == 1 || v == 2 || v == 4) && (size_t)v * (n + (n >> 4) + 1) * sizeof(float2) <= 200 * 1024) c->tb = v;
-    }
     c->smem = (size_t)c->tb * (n + (n >> 4) + 1) * sizeof(float2);
     if (c->smem > 48 * 1024) {
 #define TX_SMEM(K) B200_CUDA_OK(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem))
@@ -636,12 +632,7 @@ static int tx_launch_half(B200TXContext *c, cudaStream_t st, void *out, const vo
     if (c->dbl) return tx_dbl_launch(c->dbl, st, out, in, stride, count, out_step, in_step);
     if (c->r16 && (c->type == 0 || stride == 4) && tx_r16_accepts(c->r16, out, in, out_step, in_step))
         return tx_r16_launch(c->r16, st, out, in, out_step, in_step, count);
-    // threads per CTA grow with the transform (scripts/quick_bench.py tx with B200_TX_TB / B200_TX_THREADS compares other choices)
-    int threads = c->d.n >= 1024 ? 256 : c->d.n >= 256 ? 128 : 64;
-    if (const char *e = getenv("B200_TX_THREADS")) {               // tuning knob
-        const int v = atoi(e);
-        if (v == 64 || v == 128 || v == 256) threads = v;
-    }
+    const int threads = c->d.n >= 1024 ? 256 : c->d.n >= 256 ? 128 : 64;     // threads per CTA grow with the transform
     const long long per = 0x7fffffffLL / 4 * c->tb;              // transforms per launch (grid.x limit)
     for (int64_t c0 = 0; c0 < count; c0 += per) {
         const long long cnt = count - c0 < per ? count - c0 : per;

@@ -23,7 +23,6 @@
 #include <vector>
 #include <cmath>
 #include <cstring>
-#include <cstdlib>
 
 namespace {
 
@@ -417,7 +416,6 @@ static std::vector<uint32_t> r16_plan(int n, const int *gather, int *logn_out)
 
 TxR16 *tx_r16_create(int mode, int n, const int *gather, const float2 *exp_nat, int sm_count)
 {
-    if (getenv("B200_TX_OLD")) return nullptr;                     // A/B knob: keep the level-by-level kernels of tx.cu
     if (mode != 0 && mode != 1) return nullptr;
     int logn = 0;
     const std::vector<uint32_t> plan = r16_plan(n, gather, &logn);
@@ -425,10 +423,9 @@ TxR16 *tx_r16_create(int mode, int n, const int *gather, const float2 *exp_nat, 
     const int G = n / 16;
     TxR16 *p = new TxR16();
     p->mode = mode; p->n = n; p->logn = logn; p->G = G; p->groups = 256 / G;
-    // measured (scripts/quick_bench.py tx, B200_TX_LEAF=0/1): the conflict-free leaf assignment gains 30-45 % at 2048 points and 6 % at 512,
-    // but the 1024-point FFT (not bound by shared memory) runs 5 % slower with it
+    // the conflict-free leaf assignment pays where shared memory bounds the transform (2048 and 512 points), but the 1024-point FFT,
+    // which it does not bound, runs slower with it
     p->leaf_perm = !(logn == 10 && mode == 0);
-    if (const char *e = getenv("B200_TX_LEAF")) p->leaf_perm = atoi(e) != 0;                  // A/B knob
     const size_t zs = (size_t)n + n / 16;
     p->smem = (size_t)p->groups * 2 * zs * 8 + (mode == 1 ? (size_t)n * 8 : 0) + (size_t)p->groups * 2 * 8;
     int rc = -1;

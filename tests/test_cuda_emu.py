@@ -1451,11 +1451,12 @@ def _aligned(shape, align=64):
 
 
 @pytest.mark.parametrize("case", [(320, 96, 160, 48, FATE), (352, 64, 208, 40, FATE), (192, 48, 384, 96, cl.SWS_BICUBIC), (1024, 64, 96, 16, FATE),
-                                  (640, 40, 272, 24, cl.SWS_BILINEAR | 0x40000 | 0x80000)])
+                                  (640, 40, 272, 24, cl.SWS_BILINEAR | 0x40000 | 0x80000), (320, 96, 168, 48, FATE)])
 def test_sws_tensor_core_scaler_on_the_emulated_device(emusws, case):
     """The fused scaler with the mma.m16n8k32 horizontal pass (csrc/sws_mma.cuh): whole kernels — staging, fragment addressing, hi / lo
     coefficient split, 15-bit lines, vertical pass and writers — through the batched device entry points, against the checker; the
-    context must report that the tensor-core kernels ran."""
+    context must report that the tensor-core kernels ran.  A destination width that is a multiple of 8 but not of 16 reaches the
+    fallbacks: the fused CUDA-core kernel and the two passes."""
     L = emusws
     L.b200_sws_last_path.argtypes = [C.c_void_p]
     w, h, dw, dh, fl = case
@@ -1472,19 +1473,22 @@ def test_sws_tensor_core_scaler_on_the_emulated_device(emusws, case):
     ctx = _emu_ctx(L, w, h, 0, dw, dh, 0, fl)
     assert L.b200_sws_scale_batch_device_planar(ctx, srcp, srcs, srcf, arr(C.c_void_p, [DY.ctypes.data, DU.ctypes.data, DV.ctypes.data]),
                                                 arr(C.c_int32, [dw, cdw, cdw]), arr(C.c_int64, [dw * dh, cdw * cdh, cdw * cdh]), n) == 0
-    assert L.b200_sws_last_path(ctx) == 4
+    assert L.b200_sws_last_path(ctx) == (4 if cdw % 8 == 0 else 4 | 1)
     L.b200_sws_freeContext(ctx)
     for i in range(n):
         e = cl.orc_sws_planar(w, h, dw, dh, fl, *frames[i])
         assert np.array_equal(DY[i], e[0]) and np.array_equal(DU[i], e[1]) and np.array_equal(DV[i], e[2]), (case, i)
     # packed destinations (rgb24 and one 32-bit order)
-    if dw % 16 == 0:
+    if dw % 8 == 0:
         for fmt, bpp in ((cl.PIX_FMT_RGB24, 3), (cl.PIX_FMT_BGRA, 4)):
             D = _aligned((n, dh, dw * bpp))
             ctx = _emu_ctx(L, w, h, 0, dw, dh, fmt, fl)
             assert L.b200_sws_scale_batch_device(ctx, srcp, srcs, srcf, D.ctypes.data, dw * bpp, dw * dh * bpp, n) == 0
             path = L.b200_sws_last_path(ctx)
-            assert path == 4 or (w > 4 * dw and path == 1), path     # a 10:1 tile of three planes does not fit in shared memory: two passes
+            # widths in multiples of 16 run on the tensor cores; other multiples of 8 on the fused CUDA-core kernel if the rows are 16-byte
+            # aligned, else in two passes
+            want = 4 if dw % 16 == 0 else 2 if dw * bpp % 16 == 0 else 1
+            assert path == want or (w > 4 * dw and path == 1), path     # a 10:1 tile of three planes does not fit in shared memory: two passes
             L.b200_sws_freeContext(ctx)
             for i in range(n):
                 assert np.array_equal(D[i], cl.orc_sws(w, h, dw, dh, fl, *frames[i], fmt=fmt)), (case, fmt, i)

@@ -812,12 +812,32 @@ B200_API void b200_tx_uninit(B200TXContext **ctx)
     *ctx = nullptr;
 }
 
+// Power-of-two float transforms: the level-by-level kernels above move the complex side of a transform as 8-byte float2 words
+// (FFT in and out, RDFT r2c in (sample pairs) and out, c2r in and out, inverse-MDCT out) and everything else as single floats.
+// The register-resident route asks for more (tx_r16_accepts) but falls back to those kernels, so their rule is the one to meet.
+// The compound, DCT, int32 and double routes check their own rules in their launch functions.
+static int tx_check_align(const B200TXContext *c, const void *out, const void *in, ptrdiff_t out_step, ptrdiff_t in_step)
+{
+    if (c->pfa || c->dct || c->i32 || c->dbl) return 0;
+    const uintptr_t ia = c->type == 1 ? 3 : 7, oa = c->type == 1 && !c->inv ? 3 : 7;
+    if (((uintptr_t)in | (uintptr_t)in_step) & ia) {
+        b200_set_error("b200_tx_batch_device: input pointer and in_step must be multiples of %d bytes for this transform", (int)ia + 1);
+        return B200_EINVAL;
+    }
+    if (((uintptr_t)out | (uintptr_t)out_step) & oa) {
+        b200_set_error("b200_tx_batch_device: output pointer and out_step must be multiples of %d bytes for this transform", (int)oa + 1);
+        return B200_EINVAL;
+    }
+    return 0;
+}
+
 B200_API int b200_tx_batch_device(B200TXContext *c, void *out, const void *in, ptrdiff_t stride, int64_t count,
                                   ptrdiff_t out_step, ptrdiff_t in_step)
 {
     if (!c || !out || !in || count < 0) return B200_EINVAL;
     if ((c->type == 1 || c->type == B200_TX_INT32_MDCT) && (stride & 3)) return B200_EINVAL;
     if (c->full && stride != 4) return B200_EINVAL;                  // the reference mirrors with the input stride: only sizeof(float) is meaningful
+    if (tx_check_align(c, out, in, out_step, in_step) < 0) return B200_EINVAL;
     B200_CUDA_OK(cudaSetDevice(c->dev->ordinal));
     return tx_launch(c, c->dev->stream, out, in, (c->type == 1 || c->type == B200_TX_INT32_MDCT || c->type == B200_TX_DOUBLE_MDCT || (c->type == 0 && c->pfa)) ? stride : 8, count, out_step, in_step);
 }

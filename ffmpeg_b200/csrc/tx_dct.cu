@@ -155,6 +155,15 @@ void tx_dct_free(TxDct *p)
 int tx_dct_launch(TxDct *p, cudaStream_t st, void *out, const void *in, int64_t count, ptrdiff_t out_step, ptrdiff_t in_step)
 {
     if (count <= 0) return 0;
+    // the stages around the DFT move single floats; the inverse's c2r writes the caller's output as float2 words
+    if (((uintptr_t)in | (uintptr_t)in_step) & 3) {
+        b200_set_error("b200_tx_batch_device: DCT input pointer and in_step must be multiples of 4 bytes");
+        return B200_EINVAL;
+    }
+    if (((uintptr_t)out | (uintptr_t)out_step) & (p->inv ? 7 : 3)) {
+        b200_set_error("b200_tx_batch_device: DCT output pointer and out_step must be multiples of %d bytes", p->inv ? 8 : 4);
+        return B200_EINVAL;
+    }
     const int n = p->n;
     const size_t line = (size_t)n + 2;                                  // floats per transform in each scratch area
     const int64_t chunk_max = (int64_t)((size_t)(256u << 20) / (2 * line * sizeof(float)));

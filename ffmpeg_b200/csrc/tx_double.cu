@@ -302,7 +302,10 @@ int tx_dbl_launch(TxDbl *p, cudaStream_t st, void *out, const void *in, ptrdiff_
     const bool mdct = p->type == B200_TX_DOUBLE_MDCT;
     const int oa = (!mdct || p->inv) ? 15 : 7;                     // complex stores (16 bytes) except for the forward MDCT
     const int ia = mdct ? 7 : 15;
-    if (((reinterpret_cast<uintptr_t>(out) | (uintptr_t)out_step) & oa) || ((reinterpret_cast<uintptr_t>(in) | (uintptr_t)in_step) & ia)) return B200_EINVAL;
+    if (((reinterpret_cast<uintptr_t>(out) | (uintptr_t)out_step) & oa) || ((reinterpret_cast<uintptr_t>(in) | (uintptr_t)in_step) & ia)) {
+        b200_set_error("b200_tx_batch_device: double transform pointers and steps must be multiples of 16 bytes on the complex side, 8 on the real side");
+        return B200_EINVAL;
+    }
     if (mdct && ((stride & 7) || stride <= 0)) return B200_EINVAL;
     const unsigned nb = (unsigned)(count < p->grid_cap ? count : p->grid_cap);
     if (!mdct)       tx_dbl_fft_kernel<<<nb, DBL_THREADS, p->smem, st>>>(p->d, (double2 *)out, (const double2 *)in, out_step, in_step, count);

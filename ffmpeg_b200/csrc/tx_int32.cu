@@ -312,7 +312,10 @@ int tx_i32_launch(TxI32 *p, cudaStream_t st, void *out, const void *in, ptrdiff_
     // asks for 32 unless AV_TX_UNALIGNED), the real side 4
     const uintptr_t oa = reinterpret_cast<uintptr_t>(out) | (uintptr_t)out_step, ia = reinterpret_cast<uintptr_t>(in) | (uintptr_t)in_step;
     const bool cplx_out = p->type == B200_TX_INT32_FFT || p->inv, cplx_in = p->type == B200_TX_INT32_FFT;
-    if ((oa & (cplx_out ? 7 : 3)) || (ia & (cplx_in ? 7 : 3))) return B200_EINVAL;
+    if ((oa & (cplx_out ? 7 : 3)) || (ia & (cplx_in ? 7 : 3))) {
+        b200_set_error("b200_tx_batch_device: int32 transform pointers and steps must be multiples of 8 bytes on the complex side, 4 on the real side");
+        return B200_EINVAL;
+    }
     const unsigned nb = (unsigned)(count < p->grid_cap ? count : p->grid_cap);
     const long long sf = (long long)(stride / 4);
     if (p->type == B200_TX_INT32_FFT) tx_i32_kernel<0><<<nb, I32_THREADS, p->smem, st>>>(p->d, (int *)out, (const int *)in, sf, out_step, in_step, count);

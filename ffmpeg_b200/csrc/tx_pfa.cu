@@ -598,8 +598,10 @@ int tx_pfa_launch(TxPfa *p, cudaStream_t st, void *out, const void *in, ptrdiff_
 {
     if (count <= 0) return 0;
     if (p->fft) {                                          // complex in, complex out with a stride in bytes
-        if (((reinterpret_cast<uintptr_t>(out) | (uintptr_t)out_step | reinterpret_cast<uintptr_t>(in) | (uintptr_t)in_step | (uintptr_t)stride) & 7) || stride <= 0)
+        if (((reinterpret_cast<uintptr_t>(out) | (uintptr_t)out_step | reinterpret_cast<uintptr_t>(in) | (uintptr_t)in_step | (uintptr_t)stride) & 7) || stride <= 0) {
+            b200_set_error("b200_tx_batch_device: compound FFT pointers, steps and stride must be multiples of 8 bytes");
             return B200_EINVAL;
+        }
         const unsigned nbf = (unsigned)(count < p->grid_cap ? count : p->grid_cap);
         tx_fft_pfa_kernel<<<nbf, PFA_THREADS, p->smem, st>>>(p->d, (float2 *)out, (const float2 *)in, (long long)(stride / 8), out_step, in_step, count);
         B200_LAUNCHED();
@@ -607,8 +609,10 @@ int tx_pfa_launch(TxPfa *p, cudaStream_t st, void *out, const void *in, ptrdiff_
         return 0;
     }
     // the inverse writes its outputs as complex pairs (8-byte words); everything else moves single floats
-    if (((reinterpret_cast<uintptr_t>(out) | (uintptr_t)out_step) & (p->inv ? 7 : 3)) || ((reinterpret_cast<uintptr_t>(in) | (uintptr_t)in_step) & 3))
+    if (((reinterpret_cast<uintptr_t>(out) | (uintptr_t)out_step) & (p->inv ? 7 : 3)) || ((reinterpret_cast<uintptr_t>(in) | (uintptr_t)in_step) & 3)) {
+        b200_set_error("b200_tx_batch_device: compound MDCT input must be 4-byte aligned, output %d-byte aligned (pointers and steps)", p->inv ? 8 : 4);
         return B200_EINVAL;
+    }
     // one CTA per transform, CTAs stride over the batch
     const unsigned nb = (unsigned)(count < p->grid_cap ? count : p->grid_cap);
     if (p->inv) tx_mdct_pfa_inv_kernel<<<nb, PFA_THREADS, p->smem, st>>>(p->d, (float *)out, (const float *)in, (long long)(stride / 4), out_step, in_step, count);

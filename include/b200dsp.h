@@ -627,7 +627,16 @@ int  b200_tx_init_device(B200Device *dev, B200TXContext **ctx, b200_tx_fn *tx, i
                          const void *scale, uint64_t flags);
 void b200_tx_uninit(B200TXContext **ctx);
 /* batched, DEVICE pointers: transform i reads in + i*in_step and writes out + i*out_step (bytes); `stride` as av_tx_fn
- * (bytes between MDCT input samples for the inverse / output samples for the forward transform; unused for FFT). */
+ * (bytes between MDCT input samples for the inverse / output samples for the forward transform; unused for FFT).
+ * Alignment: the kernels move complex values as whole words, so a pointer and its step must both be multiples of
+ *   FLOAT_FFT, FLOAT_RDFT (both directions): 8 for in and out (the real samples of r2c / c2r are read / written in pairs)
+ *   FLOAT_MDCT power of two: in 4; out 8 for the inverse (AV_TX_FULL_IMDCT too), 4 for the forward; stride a multiple of 4
+ *   FLOAT_MDCT compound: in 4; out 8 for the inverse, 4 for the forward (AV_TX_FULL_IMDCT: out + len / 2 floats 8-aligned)
+ *   FLOAT_FFT compound: 8 for in, out and stride
+ *   FLOAT_DCT: in 4; out 8 for the inverse (DCT-III), 4 for the forward
+ *   INT32_FFT: 8 for in and out; INT32_MDCT: in 4, out 8 for the inverse and 4 for the forward
+ *   DOUBLE_FFT: 16 for in and out; DOUBLE_MDCT: in 8, out 16 for the inverse and 8 for the forward, stride a multiple of 8
+ * Other pointers or steps return B200_EINVAL (message in b200_last_error()) and launch nothing. */
 int  b200_tx_batch_device(B200TXContext *ctx, void *out, const void *in, ptrdiff_t stride, int64_t count,
                           ptrdiff_t out_step, ptrdiff_t in_step);
 /* same on HOST buffers (pinned memory for real overlap): chunks of transforms rotate over three streams, each chunk = one linear H2D

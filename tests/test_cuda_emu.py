@@ -1020,6 +1020,47 @@ def test_tx_whole_path_on_emulated_device(emutx):
     assert _emu_tx(emutx, 0, 0, 90, 1.0, x, 180) == -38 and _emu_tx(emutx, 6, 0, 96, 1.0, x, 98) == -38
 
 
+# (type, inv, len, flags, bytes per input / output value, values in / out, alignment of in / out in bytes): what include/b200dsp.h
+# promises for b200_tx_batch_device; the alignments are the widest word each route's kernels move on that side
+TX_ALIGN_RULES = [
+    ("fft", 0, 0, 64, 0, 4, 128, 128, 8, 8), ("fft r16 size", 0, 1, 1024, 0, 4, 2048, 2048, 8, 8), ("fft compound", 0, 0, 120, 0, 4, 240, 240, 8, 8),
+    ("rdft r2c", 6, 0, 64, 0, 4, 64, 66, 8, 8), ("rdft c2r", 6, 1, 64, 0, 4, 66, 64, 8, 8),
+    ("imdct", 1, 1, 64, 0, 4, 64, 64, 4, 8), ("mdct", 1, 0, 64, 0, 4, 128, 64, 4, 4), ("imdct full", 1, 1, 64, 4, 4, 64, 128, 4, 8),
+    ("imdct compound", 1, 1, 120, 0, 4, 120, 120, 4, 8), ("mdct compound", 1, 0, 120, 0, 4, 240, 120, 4, 4),
+    ("dct-ii", 9, 0, 64, 0, 4, 64, 64, 4, 4), ("dct-iii", 9, 1, 32, 0, 4, 64, 64, 4, 8),
+    ("int32 fft", 4, 0, 64, 0, 4, 128, 128, 8, 8), ("int32 imdct", 5, 1, 64, 0, 4, 64, 64, 4, 8), ("int32 mdct", 5, 0, 64, 0, 4, 128, 64, 4, 4),
+    ("double fft", 2, 0, 64, 0, 8, 128, 128, 16, 16), ("double imdct", 3, 1, 64, 0, 8, 64, 64, 8, 16), ("double mdct", 3, 0, 64, 0, 8, 128, 64, 8, 8),
+]
+
+
+def test_tx_batch_refuses_unaddressable_buffers(emutx):
+    """b200_tx_batch_device refuses (B200_EINVAL, with a message) a pointer or step its kernels cannot address, for every transform
+    type, before anything runs; the same call on addresses that meet the rule exactly (not more) still works"""
+    from ffmpeg_b200._lib import TX_FN
+    L = emutx
+    L.b200_last_error.restype = C.c_char_p
+    for name, typ, inv, n, flags, vb, nin, nout, ia, oa in TX_ALIGN_RULES:
+        ctx, fn = C.c_void_p(), TX_FN()
+        sc = (C.c_double if typ in (2, 3) else C.c_float)(1.0)
+        assert L.b200_tx_init_device(L.dev, C.byref(ctx), C.byref(fn), typ, inv, n, C.byref(sc), flags) == 0, name
+        stride = vb if typ in (1, 3, 5) else 8 if typ in (0, 4) else 4
+        step = (max(nin, nout) * vb + 64 + 15) & ~15               # 16-byte multiple: every rule holds with no offset
+        bi, bo = np.zeros(3 * step + 128, np.uint8), np.zeros(3 * step + 128, np.uint8)
+        pi, po = (bi.ctypes.data + 63) & ~63, (bo.ctypes.data + 63) & ~63
+
+        def call(di=0, do=0, dsi=0, dso=0):
+            return L.b200_tx_batch_device(ctx, po + do, pi + di, stride, 2, step + dso, step + dsi)
+        assert call() == 0, name
+        for d in sorted({1, ia // 2} - {0}):
+            assert call(di=d) == -22 and b"b200_tx_batch_device" in L.b200_last_error(), (name, "in", d)
+            assert call(dsi=d) == -22, (name, "in_step", d)
+        for d in sorted({1, oa // 2} - {0}):
+            assert call(do=d) == -22, (name, "out", d)
+            assert call(dso=d) == -22, (name, "out_step", d)
+        assert call(di=ia, dsi=ia) == 0 and call(do=oa, dso=oa) == 0, (name, "aligned to the rule")
+        L.b200_tx_uninit(C.byref(ctx))
+
+
 # ------------------------------------------------------------------ the library's own host code on the stand-in runtime
 def test_host_float_dsp_entry_points(emuhost):
     """b200_float_dsp_batch_device (strides, shared operand, more vectors than one grid holds, argument checks) and the

@@ -247,6 +247,98 @@ def test_tx_oracle_is_a_dft():
         assert np.abs(got[0::2] - ref.real).max() < 5e-4 * n and np.abs(got[1::2] - ref.imag).max() < 5e-4 * n
 
 
+def _tx_strided(L, pre, typ, inv, n, scale, x, stride):
+    """MDCT with `stride` floats between the inverse's input / the forward's output samples; returns the samples gathered"""
+    h = getattr(L, pre + "_tx_open")(typ, inv, n, scale, 0)
+    assert h
+    if inv:
+        xs = np.zeros((x.shape[0], n * stride), np.float32)
+        xs[:, ::stride] = x
+        out = np.zeros((x.shape[0], n), np.float32)
+        getattr(L, pre + "_tx_run")(h, out.ctypes.data, xs.ctypes.data, 4 * stride, x.shape[0], out.strides[0], xs.strides[0])
+    else:
+        out = np.zeros((x.shape[0], n * stride), np.float32)
+        getattr(L, pre + "_tx_run")(h, out.ctypes.data, x.ctypes.data, 4 * stride, x.shape[0], out.strides[0], x.strides[0])
+        out = np.ascontiguousarray(out[:, ::stride])           # (the reference's forward MDCT uses dst[0, n) as scratch: the gaps hold leftovers)
+    getattr(L, pre + "_tx_close")(h)
+    return out
+
+
+def test_tx_float64_definitions_are_the_cosine_sums():
+    """tests/txref.py's FFT-based MDCT / iMDCT equal the direct cosine definitions, and AV_TX_FULL_IMDCT's output is imdct_full"""
+    import txref as T
+    O = cl.oracle()
+    rng = np.random.default_rng(21)
+    for n in (4, 16, 64):
+        x = rng.uniform(-1, 1, (2, 2 * n))
+        i, k = np.arange(2 * n), np.arange(n)
+        cos = np.cos(np.pi / n * (i[:, None] + 0.5 + n / 2) * (k[None, :] + 0.5))            # [2n, n]
+        assert np.abs(T.mdct(x, 0.5) - 0.5 * x @ cos).max() < 1e-12
+        assert np.abs(T.imdct_full(x[:, :n], 2.0) + 2.0 * x[:, :n] @ cos.T).max() < 1e-12
+        xf = x[:, :n].astype(np.float32)
+        full = _tx(O, "orc", 1, 1, n, 1.0 / n, xf, 2 * n, flags=4)
+        assert np.abs(full - T.imdct_full(xf, 1.0 / n)).max() < 1e-5
+        assert np.array_equal(T.imdct(xf, 1.0), T.imdct_full(xf, 1.0)[:, n // 2: n // 2 + n])
+
+
+def test_tx_oracle_vs_float64_definitions():
+    """the checker against the float64 transforms at every power-of-two size the CUDA kernels take: FFT 2 ... 16384 both ways, MDCT and
+    iMDCT 4 ... 32768 (five scales; the inverse also with a sample stride of 2), RDFT 4 ... 32768 both ways, on all finite input
+    classes but subnormals.  Like the reference, the checker's forward MDCT uses its output buffer as the FFT's work area, so with an
+    output stride above one float its later stores overwrite samples not yet read: only the contiguous forward MDCT is an MDCT there
+    (the library's kernels work in shared memory and write the contiguous result's values at the stride).
+    The worst relative L2 error, in units of log2(n) 2^-24, must stay 4x under txref.TOL_C, the bound the GPU tests use."""
+    import txref as T
+    O = cl.oracle()
+    rng = np.random.default_rng(22)
+    cls = tuple(c for c in T.CLASSES if c != "subnormal")
+    worst = {}
+
+    def note(what, n, got, ref):
+        e = float(T.rel_l2(got, ref).max()) / (max(1, int(np.log2(n))) * 2.0 ** -24)
+        worst[what] = max(worst.get(what, 0.0), e)
+    for lg in range(1, 15):
+        n = 1 << lg
+        x, _ = T.rows(rng, 12, 2 * n, cls)
+        for inv in (0, 1):
+            note("fft", n, _tx(O, "orc", 0, inv, n, 1.0, x, 2 * n), T.fft(x, inv))
+    for lg in range(2, 16):
+        n = 1 << lg
+        for sc in (1.0 / n, 1.0, -1.0, -1.0 / 32768, 0.5):
+            x, _ = T.rows(rng, 6, 2 * n, cls)
+            xi = np.ascontiguousarray(x[:, :n])
+            note("mdct", n, _tx(O, "orc", 1, 0, n, sc, x, n), T.mdct(x, sc))
+            for st in (1, 2):
+                note("imdct", n, _tx_strided(O, "orc", 1, 1, n, sc, xi, st), T.imdct(xi, sc))
+        for sc in (1.0, 1.0 / n):
+            x, _ = T.rows(rng, 6, n, cls)
+            note("r2c", n, _tx(O, "orc", 6, 0, n, sc, x.copy(), n + 2), T.rdft(x, 0, sc))
+            s, _ = T.rows(rng, 6, n + 2, cls)
+            note("c2r", n, _tx(O, "orc", 6, 1, n, sc, s.copy(), n), T.rdft(s, 1, sc))
+    assert max(worst.values()) * 4 <= T.TOL_C, worst
+
+
+def test_tx_large_oracle_vs_ref():
+    """the checker against the compiled reference where the goldens stop: FFT 8192 / 16384 both ways, MDCT len 8192 ... 32768 both ways
+    with a sample stride of 2 floats and a negative scale"""
+    O = cl.oracle()
+    rng = np.random.default_rng(23)
+    with cl.RefCheck() as rc:
+        for n in (8192, 16384):
+            x = rng.uniform(-1, 1, (2, 2 * n)).astype(np.float32)
+            for inv in (0, 1):
+                got = _tx(O, "orc", 0, inv, n, 1.0, x, 2 * n)
+                assert rc.same(got.view(np.uint32), lambda: _tx(cl.ref(), "ffref", 0, inv, n, 1.0, x, 2 * n).view(np.uint32)), (n, inv)
+    with cl.RefCheck() as rc:
+        for n in (8192, 16384, 32768):
+            x = rng.uniform(-1, 1, (2, 2 * n)).astype(np.float32)
+            for inv in (0, 1):
+                xin = np.ascontiguousarray(x[:, :n]) if inv else x
+                for sc in (-1.0 / n, -1.0):
+                    got = _tx_strided(O, "orc", 1, inv, n, sc, xin, 2)
+                    assert rc.same(got.view(np.uint32), lambda: _tx_strided(cl.ref(), "ffref", 1, inv, n, sc, xin, 2).view(np.uint32)), (n, inv, sc)
+
+
 def test_more_oracles_vs_reference_live():
     O = cl.oracle()
     R = cl.ref() if cl.have_ref() else None

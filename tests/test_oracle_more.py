@@ -279,6 +279,21 @@ def test_tx_float64_definitions_are_the_cosine_sums():
         full = _tx(O, "orc", 1, 1, n, 1.0 / n, xf, 2 * n, flags=4)
         assert np.abs(full - T.imdct_full(xf, 1.0 / n)).max() < 1e-5
         assert np.array_equal(T.imdct(xf, 1.0), T.imdct_full(xf, 1.0)[:, n // 2: n // 2 + n])
+    for n in (6, 10, 14, 18, 30, 12, 20, 28, 36, 60):                   # compound lengths, and the long double forms
+        x = rng.uniform(-1, 1, (2, 2 * n))
+        i, k = np.arange(2 * n), np.arange(n)
+        cos = np.cos(np.pi / n * (i[:, None] + 0.5 + n / 2) * (k[None, :] + 0.5))
+        for ld in (False, True):
+            assert np.abs(T.mdct(x, 0.5, ld) - 0.5 * x @ cos).max() < 1e-12
+            assert np.abs(T.imdct_full(x[:, :n], 2.0, ld) + 2.0 * x[:, :n] @ cos.T).max() < 1e-12
+            for inv in (0, 1):
+                w = np.exp((2j if inv else -2j) * np.pi * np.outer(k, k) / n)
+                assert np.abs(T.cpx(T.fft(x, inv, ld)) - T.cpx(x) @ w).max() < 1e-12
+        c2 = np.cos(np.pi / n * np.outer(k, k + 0.5))                     # DCT-II [k, i]
+        assert np.abs(T.dct(x[:, :n], 0, 0.5) - x[:, :n] @ c2.T).max() < 1e-12
+        w3 = 2 * c2.T
+        w3[:, 0] = 1                                                       # DCT-III [k, i]: x[0] + 2 sum x[i] cos(pi i (k + 1/2) / n)
+        assert np.abs(T.dct(x[:, :n], 1, 3.0) - 3.0 * x[:, :n] @ w3.T).max() < 1e-12
 
 
 def test_tx_oracle_vs_float64_definitions():
@@ -316,6 +331,133 @@ def test_tx_oracle_vs_float64_definitions():
             s, _ = T.rows(rng, 6, n + 2, cls)
             note("c2r", n, _tx(O, "orc", 6, 1, n, sc, s.copy(), n), T.rdft(s, 1, sc))
     assert max(worst.values()) * 4 <= T.TOL_C, worst
+
+
+PFA_FACTORS = (3, 5, 7, 9, 15)
+PFA_MS = tuple(1 << k for k in range(1, 10))                        # the power-of-two part of a compound length: 2 ... 512
+
+
+def pfa_fft_lengths():
+    """every compound FFT length the library builds, N x m"""
+    return [nf * m for nf in PFA_FACTORS for m in PFA_MS]
+
+
+def _txd(L, pre, typ, inv, n, scale, x, out_doubles):
+    """AV_TX_DOUBLE_FFT (2) / AV_TX_DOUBLE_MDCT (3), contiguous, on the checker (orc) or the compiled reference (ffref)"""
+    op = getattr(L, pre + "_txd_open")
+    op.restype, op.argtypes = C.c_void_p, [C.c_int, C.c_int, C.c_int, C.c_double, C.c_uint]
+    ru, clo = (L.orc_txd_run, L.orc_txd_close) if pre == "orc" else (L.ffref_tx_run, L.ffref_tx_close)
+    ru.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_int, C.c_ssize_t, C.c_ssize_t]
+    clo.argtypes = [C.c_void_p]
+    h = op(typ, inv, n, scale, 0)
+    assert h
+    out, xin = np.zeros((x.shape[0], out_doubles)), x.copy()
+    ru(h, out.ctypes.data, xin.ctypes.data, 16 if typ == 2 else 8, x.shape[0], out.strides[0], xin.strides[0])
+    clo(h)
+    return out
+
+
+def test_tx_route_oracles_vs_definitions():
+    """the checker of the compound, DCT, int32 and double routes against their high-precision definitions (tests/txref.py) at every
+    length the library builds: compound FFT and MDCT at all 45 N x m lengths (five scales), DCT-II / DCT-III 4 ... 32768 points (scales
+    1, 0.5 / n, -1; the bound grows like sqrt(n) there), int32 FFT 2 ... 4096 and MDCT 4 ... 8192 (headroom-safe rows), double FFT 2 ... 8192 and MDCT 4 ... 16384 (against
+    long double).  The worst constant of each route, in units of its bound's log2(n) eps, must stay 4x under the constant the GPU
+    tests use (txref.TOL_C, DCT_TOL_C, I32_TOL_C, DBL_TOL_C)."""
+    import txref as T
+    O = cl.oracle()
+    rng = np.random.default_rng(24)
+    cls = tuple(c for c in T.CLASSES if c != "subnormal")
+    worst = {}
+
+    def note(what, n, err, eps=2.0 ** -24, grow=None):
+        worst[what] = max(worst.get(what, 0.0), float(np.max(err)) / ((grow or max(1, int(np.log2(n)))) * eps))
+    for n in pfa_fft_lengths():
+        x, _ = T.rows(rng, 6, 2 * n, cls)
+        for inv in (0, 1):
+            note("pfa-fft", n, T.rel_l2(_tx(O, "orc", 0, inv, n, 1.0, x, 2 * n), T.fft(x, inv)))
+        ln = 2 * n
+        for sc in (1.0 / ln, 1.0, -1.0, -1.0 / 32768, 0.5):
+            x, _ = T.rows(rng, 5, 2 * ln, cls)
+            xi = np.ascontiguousarray(x[:, :ln])
+            note("pfa-mdct", ln, T.rel_l2(_tx(O, "orc", 1, 0, ln, sc, x, ln), T.mdct(x, sc)))
+            note("pfa-imdct", ln, T.rel_l2(_tx(O, "orc", 1, 1, ln, sc, xi, ln), T.imdct(xi, sc)))
+    for lg in range(2, 16):
+        n = 1 << lg
+        for sc in (1.0, 0.5 / n, -1.0):
+            x, _ = T.rows(rng, 6, n + 2, T.DCT_CLASSES)
+            for inv, asked in ((0, n), (1, n // 2)):
+                note("dct3" if inv else "dct2", n, T.rel_l2(_dct(O, "orc", inv, asked, sc, x, n), T.dct(x[:, :n], inv, sc)), grow=np.sqrt(n))
+    for lg in range(1, 14):
+        n = 1 << lg
+        if n <= 4096:
+            for inv in (0, 1):
+                x, _ = T.rows_i32(rng, 4, 2 * n, T.i32_headroom(4, inv, n), ("headroom",))
+                note("i32-fft", n, T.rel_l2_i32(_txi(O, "orc", 4, inv, n, 1.0, x, 2 * n), T.i32_transform(4, inv, x, 1.0)))
+        if n >= 4:
+            for sc in (1.0 / n, 1.0, -1.0 / 32768):
+                for inv in (0, 1):
+                    x, _ = T.rows_i32(rng, 4, n if inv else 2 * n, T.i32_headroom(5, inv, n), ("headroom",))
+                    note("i32-imdct" if inv else "i32-mdct", n, T.rel_l2_i32(_txi(O, "orc", 5, inv, n, sc, x, n), T.i32_transform(5, inv, x, sc)))
+    dcls = tuple(c for c in T.DBL_CLASSES if c != "subnormal")
+    for lg in range(1, 15):
+        n = 1 << lg
+        if n <= 8192:
+            x, _ = T.rows_dbl(rng, 5, 2 * n, dcls)
+            for inv in (0, 1):
+                note("dbl-fft", n, T.rel_l2(_txd(O, "orc", 2, inv, n, 1.0, x, 2 * n), T.fft(x, inv, ld=True)), 2.0 ** -53)
+        if n >= 4:
+            for sc in (1.0 / n, 1.0, -1.0, 0.5):
+                x, _ = T.rows_dbl(rng, 5, 2 * n, dcls)
+                xi = np.ascontiguousarray(x[:, :n])
+                note("dbl-mdct", n, T.rel_l2(_txd(O, "orc", 3, 0, n, sc, x, n), T.mdct(x, sc, ld=True)), 2.0 ** -53)
+                note("dbl-imdct", n, T.rel_l2(_txd(O, "orc", 3, 1, n, sc, xi, n), T.imdct(xi, sc, ld=True)), 2.0 ** -53)
+    print({k: round(v, 3) for k, v in worst.items()})
+    for what, c in (("pfa", T.TOL_C), ("dct", T.DCT_TOL_C), ("i32", T.I32_TOL_C), ("dbl", T.DBL_TOL_C)):
+        got = {k: v for k, v in worst.items() if k.startswith(what)}
+        assert got and max(got.values()) * 4 <= c, (what, got)
+
+
+def test_tx_route_oracles_vs_ref():
+    """the checker of the compound, int32, double and DCT routes against the compiled reference where the goldens stop: compound FFT and
+    MDCT at m = 2 and m = 512 for every odd factor and at every 7 x m and 9 x m length (a codelet tree the reference picked differently
+    would show here), int32 FFT 4096 / MDCT 8192, double FFT 8192 / MDCT 16384, DCT-II / DCT-III of 32768 points; both directions"""
+    O = cl.oracle()
+    rng = np.random.default_rng(25)
+    lengths = sorted({nf * m for nf in PFA_FACTORS for m in (2, 512)} | {nf * m for nf in (7, 9) for m in PFA_MS})
+    u32 = lambda a: a.view(np.uint32)  # noqa: E731
+    with cl.RefCheck() as rc:
+        for n in lengths:
+            x = rng.uniform(-1, 1, (2, 2 * n)).astype(np.float32)
+            for inv in (0, 1):
+                assert rc.same(u32(_tx(O, "orc", 0, inv, n, 1.0, x, 2 * n)), lambda: u32(_tx(cl.ref(), "ffref", 0, inv, n, 1.0, x, 2 * n))), (n, inv)
+    with cl.RefCheck() as rc:
+        for n in lengths:
+            ln = 2 * n
+            x = rng.uniform(-1, 1, (2, 2 * ln)).astype(np.float32)
+            for inv in (0, 1):
+                xin = np.ascontiguousarray(x[:, :ln]) if inv else x
+                for sc in (1.0 / ln, -1.0, -1.0 / 32768):
+                    assert rc.same(u32(_tx(O, "orc", 1, inv, ln, sc, xin, ln)), lambda: u32(_tx(cl.ref(), "ffref", 1, inv, ln, sc, xin, ln))), (ln, inv, sc)
+    with cl.RefCheck() as rc:
+        x = rng.integers(-(1 << 31), 1 << 31, (2, 2 * 8192)).astype(np.int32)
+        for inv in (0, 1):
+            assert rc.same(_txi(O, "orc", 4, inv, 4096, 1.0, x[:, :8192], 8192), lambda: _txi(cl.ref(), "ffref", 4, inv, 4096, 1.0, x[:, :8192], 8192)), inv
+            xi = np.ascontiguousarray((x >> 5)[:, :8192]) if inv else x >> 5
+            for sc in (1.0 / 8192, -1.0 / 32768):
+                assert rc.same(_txi(O, "orc", 5, inv, 8192, sc, xi, 8192), lambda: _txi(cl.ref(), "ffref", 5, inv, 8192, sc, xi, 8192)), (inv, sc)
+    with cl.RefCheck() as rc:
+        x = rng.uniform(-1, 1, (2, 2 * 16384))
+        for inv in (0, 1):
+            assert rc.same(_txd(O, "orc", 2, inv, 8192, 1.0, x[:, :16384], 16384), lambda: _txd(cl.ref(), "ffref", 2, inv, 8192, 1.0, x[:, :16384], 16384)), inv
+            xi = np.ascontiguousarray(x[:, :16384]) if inv else x
+            for sc in (1.0 / 16384, -1.0):
+                assert rc.same(_txd(O, "orc", 3, inv, 16384, sc, xi, 16384), lambda: _txd(cl.ref(), "ffref", 3, inv, 16384, sc, xi, 16384)), (inv, sc)
+    with cl.RefCheck() as rc:
+        n = 32768
+        x = rng.uniform(-1, 1, (2, n + 2)).astype(np.float32)
+        for inv, asked in ((0, n), (1, n // 2)):
+            for sc in (1.0, -1.0):
+                assert rc.same(u32(_dct(O, "orc", inv, asked, sc, x, n)), lambda: u32(_dct(cl.ref(), "ffref", inv, asked, sc, x, n))), (inv, sc)
 
 
 def test_tx_large_oracle_vs_ref():

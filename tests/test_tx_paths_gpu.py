@@ -10,12 +10,11 @@ and the input must come back unchanged.  Every non-subnormal row is also held to
 import numpy as np
 import pytest
 
-import cpulibs as cl
 import txref as T
 
 pytestmark = pytest.mark.gpu
 
-SENT = 0x7FC0DEAD                          # a NaN payload: no finite input makes a kernel write it
+SENT = T.SENT
 H100_SMS, R16_CTAS_PER_SM = 132, 3         # shared memory holds at most 3 CTAs of tx_r16_kernel per SM
 MDCT_SCALES = ("1/len", 1.0, -1.0, -1.0 / 32768, 0.5)
 
@@ -72,11 +71,6 @@ def _shape(kind, ln):
             "r2c": (ln, ln + 2, 6), "c2r": (ln + 2, ln, 6)}[kind]
 
 
-def _positions(count, width, step, off, elem):
-    """float index of logical element k of transform r in a buffer: byte off + r * step + k * elem"""
-    return (off + np.arange(count, dtype=np.int64)[:, None] * step + np.arange(width, dtype=np.int64)[None, :] * elem) // 4
-
-
 def _float64(kind, x, scale):
     if kind in ("fft", "ifft"):
         return T.fft(x, kind == "ifft")
@@ -85,16 +79,6 @@ def _float64(kind, x, scale):
     if kind == "mdct":
         return T.mdct(x, scale)
     return T.rdft(x, kind == "c2r", scale)
-
-
-def _oracle(typ, inv, ln, scale, x, out_w):
-    O = cl.oracle()
-    h = O.orc_tx_open(typ, inv, ln, scale, 0)
-    assert h
-    out, xin = np.zeros((x.shape[0], out_w), np.float32), x.copy()        # c2r rewrites its input
-    O.orc_tx_run(h, out.ctypes.data, xin.ctypes.data, 8 if typ == 0 else 4, x.shape[0], out.strides[0], xin.strides[0])
-    O.orc_tx_close(h)
-    return out
 
 
 @pytest.mark.parametrize("kind, inv, ln, counts, stride, in_off, in_pad, out_pad", _cases())
@@ -108,8 +92,8 @@ def test_tx_path_vs_checker(device, kind, inv, ln, counts, stride, in_off, in_pa
     rows = max(counts)
     rng = np.random.default_rng([typ, inv, ln, stride, in_off, in_pad, out_pad])
     x, cls = T.rows(rng, rows, in_w)
-    pin = _positions(rows, in_w, in_step, in_off, in_elem)
-    pout = _positions(rows, out_w, out_step, 0, out_elem)
+    pin = T.positions(rows, in_w, in_step, in_off, in_elem)
+    pout = T.positions(rows, out_w, out_step, 0, out_elem)
     host_in = np.full(pin.max() + 1 + 64, SENT, np.uint32)
     host_in[pin] = x.view(np.uint32)
     out_len = pout.max() + 1 + 64
@@ -120,7 +104,7 @@ def test_tx_path_vs_checker(device, kind, inv, ln, counts, stride, in_off, in_pa
         dout = torch.empty(out_len, dtype=torch.int32, device="cuda")
         for sc in scales:
             sc = 1.0 / ln if sc == "1/len" else sc
-            exp = _oracle(typ, inv, ln, sc, x, out_w)
+            exp = T.checker(typ, inv, ln, sc, x, out_w)
             c = tx.av_tx_init(typ, inv, ln, scale=None if typ == 0 else sc, device=device)
             try:                                                 # a failing check must not leave the context to outlive the device
                 for cnt in counts:
@@ -169,6 +153,6 @@ def test_tx_fft1024_batch_over_2g(device):
         assert bool(torch.isnan(dout[cnt]).all()), "the row after the batch was written"
         del din, dout
         torch.cuda.empty_cache()
-    exp = _oracle(0, 0, n, 1.0, x, 2 * n)
+    exp = T.checker(0, 0, n, 1.0, x, 2 * n)
     bad = np.nonzero((got.view(np.uint32) != exp.view(np.uint32)).any(axis=1))[0]
     assert not len(bad), f"transforms {pick[bad][:8].tolist()} differ from the checker"

@@ -122,6 +122,21 @@ class H264LoopFilterContext(C.Structure):
                 ("v_loop_filter_chroma_intra", _LF_INTRA), ("h_loop_filter_chroma_intra", _LF_INTRA), ("h_loop_filter_chroma_mbaff_intra", _LF_INTRA)]
 
 
+_PRED4 = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t)
+_PRED8L = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_int, C.c_ssize_t)
+_PRED = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t)
+_PRED_ADD = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t)
+_PRED_FADD = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_ssize_t)
+_PRED_TADD = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_void_p, C.c_ssize_t)
+
+
+class H264PredContext(C.Structure):
+    """libavcodec/h264pred.h:94-114 (same member order and table sizes)"""
+    _fields_ = [("pred4x4", _PRED4 * 15), ("pred8x8l", _PRED8L * 12), ("pred8x8", _PRED * 11), ("pred16x16", _PRED * 9),
+                ("pred4x4_add", _PRED_ADD * 2), ("pred8x8l_add", _PRED_ADD * 2), ("pred8x8l_filter_add", _PRED_FADD * 2),
+                ("pred8x8_add", _PRED_TADD * 3), ("pred16x16_add", _PRED_TADD * 3)]
+
+
 class ProresDSPContext(C.Structure):
     """libavcodec/proresdsp.h:28-35"""
     _fields_ = [("idct_permutation_type", C.c_int), ("idct_permutation", C.c_uint8 * 64),
@@ -227,6 +242,9 @@ PROTOTYPES = {
     "b200_pixelutils_sad_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_ssize_t, vp, C.c_ssize_t, vp, vp, C.c_int64, vp]),
     "b200_h264_loop_filter_init": (C.c_int, [vp, C.c_int, C.c_int]),
     "b200_h264_loop_filter_batch_device": (C.c_int, [vp, C.c_int64, vp, vp, vp, C.c_ssize_t, vp, vp, vp]),
+    "b200_h264_pred_init": (C.c_int, [vp, C.c_int, C.c_int, C.c_int]),
+    "b200_h264_pred_batch_device": (C.c_int, [vp, C.c_int, C.c_int64, vp, vp, vp, vp, C.c_ssize_t]),
+    "b200_h264_pred_add_batch_device": (C.c_int, [vp, C.c_int, C.c_int64, vp, vp, vp, vp, C.c_ssize_t, vp, vp]),
     "b200_proresdsp_init": (C.c_int, [vp, C.c_int]),
     "b200_prores_idct_put_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, vp, vp, vp, C.c_int]),
     "b200_float_dsp_init": (C.c_int, [vp]),

@@ -136,3 +136,33 @@ def h264_loop_filter_batch_device(device, nedges, kinds, pix, pix_off, stride, a
     """one independent set of edges; kinds / alpha / beta uint8 [n], pix_off int64 [n], tc0 int8 [n, 4] (device)"""
     return check(lib().b200_h264_loop_filter_batch_device(device.handle, nedges, vp(_dptr(kinds)), vp(_dptr(pix)), vp(_dptr(pix_off)), stride,
                                                           vp(_dptr(alpha)), vp(_dptr(beta)), vp(_dptr(tc0))), "h264_loop_filter_batch_device")
+
+
+H264_CODEC_ID = 27          # AV_CODEC_ID_H264
+PRED4x4, PRED8x8L, PRED8x8, PRED8x16, PRED16x16 = range(5)                                   # b200_h264_pred_batch_device tables
+PRED4x4_ADD, PRED8x8L_ADD, PRED8x8L_FILTER_ADD, PRED8x8_ADD, PRED8x16_ADD, PRED16x16_ADD = range(6)   # b200_h264_pred_add_batch_device tables
+
+
+def pred_kind(table, mode):
+    return (table << 4) | mode
+
+
+def ff_h264_pred_init(codec_id=H264_CODEC_ID, bit_depth=8, chroma_format_idc=1):
+    """H264PredContext as ff_h264_pred_init installs it (libavcodec/h264pred.c:437-539) on HOST pointers"""
+    from ._lib import H264PredContext
+    c = H264PredContext()
+    check(lib().b200_h264_pred_init(C.byref(c), codec_id, bit_depth, chroma_format_idc), "ff_h264_pred_init")
+    return c
+
+
+def h264_pred_batch_device(device, bit_depth, nops, kinds, flags, pix, pix_off, stride):
+    """one independent set of intra predictions; kinds / flags uint8 [n], pix_off int64 [n] in bytes (device)"""
+    return check(lib().b200_h264_pred_batch_device(device.handle, bit_depth, nops, vp(_dptr(kinds)), vp(_dptr(flags)), vp(_dptr(pix)),
+                                                   vp(_dptr(pix_off)), stride), "h264_pred_batch_device")
+
+
+def h264_pred_add_batch_device(device, bit_depth, nops, kinds, flags, pix, pix_off, stride, coef, coef_off):
+    """one independent set of lossless prediction + residual adds; coef int16 (8 bit) / int32 (above), coef_off int64 [n] in coefficients"""
+    return check(lib().b200_h264_pred_add_batch_device(device.handle, bit_depth, nops, vp(_dptr(kinds)), vp(_dptr(flags)), vp(_dptr(pix)),
+                                                       vp(_dptr(pix_off)), stride, vp(_dptr(coef)), vp(_dptr(coef_off))),
+                 "h264_pred_add_batch_device")

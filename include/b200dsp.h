@@ -287,6 +287,49 @@ int  b200_h264_loop_filter_batch_device(B200Device *dev, int64_t nedges, const u
 int  b200_h264_loop_filter_hbd_batch_device(B200Device *dev, int bit_depth, int64_t nedges, const uint8_t *kinds, uint8_t *pix,
                                             const int64_t *pix_off, ptrdiff_t stride, const uint8_t *alpha, const uint8_t *beta, const int8_t *tc0);
 
+/* H.264 intra prediction: H264PredContext (libavcodec/h264pred.h:94-114) in the reference's member order and table sizes, as
+ * ff_h264_pred_init(h, AV_CODEC_ID_H264, bit_depth, chroma_format_idc) fills it (libavcodec/h264pred.c:437-539; functions
+ * libavcodec/h264pred_template.c).  HOST pointers, the reference's signatures: samples are uint8 at 8 bit and uint16 above, strides in
+ * bytes, coefficients (`block`) int16 at 8 bit and int32 above; the _add members clear their coefficients.  Members the reference
+ * leaves NULL for H.264 stay NULL.  pred4x4's topright may point anywhere (the decoder passes a stack word, h264_mb.c:676-691). */
+#define B200_CODEC_ID_H264 27           /* AV_CODEC_ID_H264 */
+typedef struct B200H264PredContext {
+    void (*pred4x4[9 + 3 + 3])(uint8_t *src, const uint8_t *topright, ptrdiff_t stride);
+    void (*pred8x8l[9 + 3])(uint8_t *src, int topleft, int topright, ptrdiff_t stride);
+    void (*pred8x8[4 + 3 + 4])(uint8_t *src, ptrdiff_t stride);
+    void (*pred16x16[4 + 3 + 2])(uint8_t *src, ptrdiff_t stride);
+    void (*pred4x4_add[2])(uint8_t *pix, int16_t *block, ptrdiff_t stride);
+    void (*pred8x8l_add[2])(uint8_t *pix, int16_t *block, ptrdiff_t stride);
+    void (*pred8x8l_filter_add[2])(uint8_t *pix, int16_t *block, int topleft, int topright, ptrdiff_t stride);
+    void (*pred8x8_add[3])(uint8_t *pix, const int *block_offset, int16_t *block, ptrdiff_t stride);
+    void (*pred16x16_add[3])(uint8_t *pix, const int *block_offset, int16_t *block, ptrdiff_t stride);
+} B200H264PredContext;
+/* 0, or B200_ENOSYS for other codec ids (the SVQ3 / RV40 / VP7 / VP8 replacements) and depths other than 8 / 9 / 10 / 12 / 14,
+ * B200_EINVAL for h == NULL or chroma_format_idc outside 0..3, B200_ENODEV.  chroma_format_idc <= 1 selects the 8x8 chroma functions,
+ * 2 and 3 the 8x16 ones. */
+int  b200_h264_pred_init(B200H264PredContext *h, int codec_id, int bit_depth, int chroma_format_idc);
+/* Batched, DEVICE pointers.  Op i predicts the block whose top-left sample is at pix + pix_off[i] (bytes; stride in bytes; uint8 samples at
+ * 8 bit, uint16 above).  kinds[i] = table << 4 | mode, mode being the index into the reference's table:
+ *   b200_h264_pred_batch_device:      0 pred4x4 (modes 0-11), 1 pred8x8l (0-11), 2 pred8x8 as 8x8 (0-10), 3 pred8x8 as 8x16 (0-10),
+ *                                     4 pred16x16 (0-6)
+ *   b200_h264_pred_add_batch_device:  0 pred4x4_add, 1 pred8x8l_add, 2 pred8x8l_filter_add (modes 0 VERT, 1 HOR), 3 pred8x8_add as 8x8,
+ *                                     4 pred8x8_add as 8x16, 5 pred16x16_add (modes 1 HOR, 2 VERT)
+ * An op whose kind names a member the reference leaves NULL changes nothing.  flags[i]: bit 0 has_topleft, bit 1 has_topright for
+ * pred8x8l and pred8x8l_filter_add; for pred4x4, bit 1 set reads the four top-right samples at src + 4 - stride, clear uses four
+ * copies of src[3 - stride] (the decoder's substitute); other tables ignore it.
+ * The add forms wrap (modulo 2^8 at 8 bit, 2^16 above; no clipping) and clear the coefficients they read.  Op i's coefficients start
+ * at coef + coef_off[i] (in coefficients: int16 at 8 bit, int32 above); 4x4 sub-block k of the 8x8 / 8x16 / 16x16 add forms is at
+ * + 16 k and sits where h264_slice.c:554-563 puts block k (scan8 order; 8x16: the 4x4 rows 0-3 in pairs), relative to the call's
+ * stride.  The sub-blocks chain as in the reference: each predicts from its neighbour's already added samples.
+ * The ops of one call must be independent: no op may write samples another op of the same call reads or writes.  The decoder's
+ * sequential order (macroblocks in raster order, the 4x4 / 8x8 blocks of one in scan order) becomes one call per wavefront step.
+ * Returns 0, or B200_EINVAL (launching nothing) for NULL pointers, a negative nops or stride, an odd stride or pix above 8 bit, or a
+ * depth other than 8 / 9 / 10 / 12 / 14; nops == 0 returns 0. */
+int  b200_h264_pred_batch_device(B200Device *dev, int bit_depth, int64_t nops, const uint8_t *kinds, const uint8_t *flags, uint8_t *pix,
+                                 const int64_t *pix_off, ptrdiff_t stride);
+int  b200_h264_pred_add_batch_device(B200Device *dev, int bit_depth, int64_t nops, const uint8_t *kinds, const uint8_t *flags, uint8_t *pix,
+                                     const int64_t *pix_off, ptrdiff_t stride, void *coef, const int64_t *coef_off);
+
 /* mpegvideo inverse quantisers: the members of MPVUnquantDSPContext (libavcodec/mpegvideo_unquantize.h:31-44) as
  * ff_mpv_unquantize_init() installs them (libavcodec/mpegvideo_unquantize.c:50-290), i.e. what runs in front of the IDCT in
  * mpv_reconstruct_mb's put_dct / add_dequant_dct (libavcodec/mpegvideo_dec.c).  The reference functions take the whole

@@ -16,6 +16,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import cpulibs as cl  # noqa: E402
+import h264predlib as hp  # noqa: E402
 from cases import SWS_SMALL_CASES, SWS_HASH_CASES, idct_blocks  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
@@ -256,6 +257,19 @@ def gen_h264lf_hbd():
         case = cl.h264lf_hbd_case(50 + depth, 1024, depth)
         lines.append(f"{depth} {sha(cl.ref_h264lf_hbd(depth, *case))}")
     open(os.path.join(OUT, "h264lf_hbd_hashes.txt"), "w").write("\n".join(lines) + "\n")
+
+
+def gen_h264pred():
+    """H264PredContext from ff_h264_pred_init(AV_CODEC_ID_H264, depth, 1 / 2): sha256 of the reference's picture followed by its
+    coefficients after one seeded batch of predictions ("pred") and of lossless adds ("add"), per depth and 4:2:0 / 4:2:2"""
+    lines = []
+    for depth in (8, 9, 10, 12, 14):
+        for idc in (1, 2):
+            for add in (0, 1):
+                pic, cf = hp.ref_h264pred(depth, idc, add, *hp.h264pred_fixture_case(depth, idc, add))
+                h = hashlib.sha256(np.ascontiguousarray(pic).tobytes() + np.ascontiguousarray(cf).tobytes()).hexdigest()
+                lines.append(f"{depth} {idc} {'add' if add else 'pred'} {h}")
+    open(os.path.join(OUT, "h264pred_hashes.txt"), "w").write("\n".join(lines) + "\n")
 
 
 def gen_tx_double():
@@ -784,6 +798,7 @@ if __name__ == "__main__":
     gen_h264_weight_hbd()
     gen_h264_idct_hbd()
     gen_h264lf_hbd()
+    gen_h264pred()
     gen_tx_double()
     gen_sws_rgb2rgb()
     gen_tx_full_imdct()

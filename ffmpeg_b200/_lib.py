@@ -137,6 +137,33 @@ class H264PredContext(C.Structure):
                 ("pred8x8_add", _PRED_TADD * 3), ("pred16x16_add", _PRED_TADD * 3)]
 
 
+_QP = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_int, C.c_ssize_t, C.c_ssize_t, C.c_int)
+_QP_UNI = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_ssize_t, C.c_int, C.c_ssize_t, C.c_ssize_t, C.c_int)
+_QP_UNI_W = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_ssize_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_ssize_t,
+                        C.c_ssize_t, C.c_int)
+_QP_BI = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_int, C.c_ssize_t, C.c_ssize_t, C.c_int)
+_QP_BI_W = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                       C.c_ssize_t, C.c_ssize_t, C.c_int)
+
+
+class HEVCDSPContext(C.Structure):
+    """libavcodec/hevc/dsp.h:47-125 (same member order; the members this library does not fill are plain pointers here)"""
+    _fields_ = ([("put_pcm", vp), ("add_residual", vp * 4), ("dequant", vp), ("transform_rdpcm", vp), ("transform_4x4_luma", vp),
+                 ("idct", vp * 4), ("idct_dc", vp * 4), ("sao_band_filter", vp * 5), ("sao_edge_filter", vp * 5), ("sao_edge_restore", vp * 2)] +
+                [(f"put_hevc_{p}{s}", t * 2 * 2 * 10) for p in ("qpel", "epel")
+                 for s, t in (("", _QP), ("_uni", _QP_UNI), ("_uni_w", _QP_UNI_W), ("_bi", _QP_BI), ("_bi_w", _QP_BI_W))] +
+                [(n, vp) for n in ("hevc_h_loop_filter_luma", "hevc_v_loop_filter_luma", "hevc_h_loop_filter_chroma", "hevc_v_loop_filter_chroma",
+                                   "hevc_h_loop_filter_luma_c", "hevc_v_loop_filter_luma_c", "hevc_h_loop_filter_chroma_c",
+                                   "hevc_v_loop_filter_chroma_c")])
+
+
+class HevcMcOp(C.Structure):
+    """B200HevcMcOp (include/b200dsp.h), 64 bytes"""
+    _fields_ = [("dst_off", C.c_int64), ("ref_off", C.c_int64 * 2), ("x", C.c_int32 * 2), ("y", C.c_int32 * 2), ("mx", C.c_uint8 * 2),
+                ("my", C.c_uint8 * 2), ("w", C.c_uint8), ("h", C.c_uint8), ("kind", C.c_uint8), ("denom", C.c_uint8), ("wx0", C.c_int32),
+                ("wx1", C.c_int32), ("ox", C.c_int32), ("reserved", C.c_uint8 * 4)]
+
+
 class ProresDSPContext(C.Structure):
     """libavcodec/proresdsp.h:28-35"""
     _fields_ = [("idct_permutation_type", C.c_int), ("idct_permutation", C.c_uint8 * 64),
@@ -245,6 +272,8 @@ PROTOTYPES = {
     "b200_h264_pred_init": (C.c_int, [vp, C.c_int, C.c_int, C.c_int]),
     "b200_h264_pred_batch_device": (C.c_int, [vp, C.c_int, C.c_int64, vp, vp, vp, vp, C.c_ssize_t]),
     "b200_h264_pred_add_batch_device": (C.c_int, [vp, C.c_int, C.c_int64, vp, vp, vp, vp, C.c_ssize_t, vp, vp]),
+    "b200_hevc_dsp_init": (C.c_int, [vp, C.c_int]),
+    "b200_hevc_mc_batch_device": (C.c_int, [vp, C.c_int, C.c_int, C.c_int64, vp, vp, C.c_ssize_t, vp, C.c_ssize_t, C.c_int, C.c_int]),
     "b200_proresdsp_init": (C.c_int, [vp, C.c_int]),
     "b200_prores_idct_put_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, vp, vp, vp, C.c_int]),
     "b200_float_dsp_init": (C.c_int, [vp]),

@@ -330,6 +330,96 @@ int  b200_h264_pred_batch_device(B200Device *dev, int bit_depth, int64_t nops, c
 int  b200_h264_pred_add_batch_device(B200Device *dev, int bit_depth, int64_t nops, const uint8_t *kinds, const uint8_t *flags, uint8_t *pix,
                                      const int64_t *pix_off, ptrdiff_t stride, void *coef, const int64_t *coef_off);
 
+/* HEVC motion compensation: HEVCDSPContext (libavcodec/hevc/dsp.h:47-125) in the reference's member order and types.
+ * b200_hevc_dsp_init() fills the six inter-prediction tables put_hevc_{q,e}pel, _uni, _uni_w, _bi, _bi_w ([10][2][2] each, every
+ * width index) as ff_hevc_dsp_init does (hevc/dsp.c:140-196, :230-235); every other member stays NULL.  HOST pointers, the
+ * reference's signatures: samples uint8 at 8 bit and uint16 above, strides in bytes, the int16 `dst` of put_hevc_?pel and `src2` of
+ * the _bi forms at the MAX_PB_SIZE (64) element stride, 1 <= width, height <= 64, mx / my 0..3 (qpel) or 0..7 (epel); the width
+ * index is ignored, as the reference does.  A member reads exactly the samples its reference function reads: columns -3..+4 (qpel) /
+ * -1..+2 (epel) around the block only where it filters horizontally, the same rows only where it filters vertically. */
+struct GetBitContext;
+struct SAOParams;
+typedef struct B200HEVCDSPContext {
+    void (*put_pcm)(uint8_t *_dst, ptrdiff_t _stride, int width, int height, struct GetBitContext *gb, int pcm_bit_depth);
+    void (*add_residual[4])(uint8_t *dst, const int16_t *res, ptrdiff_t stride);
+    void (*dequant)(int16_t *coeffs, int16_t log2_size);
+    void (*transform_rdpcm)(int16_t *coeffs, int16_t log2_size, int mode);
+    void (*transform_4x4_luma)(int16_t *coeffs);
+    void (*idct[4])(int16_t *coeffs, int col_limit);
+    void (*idct_dc[4])(int16_t *coeffs);
+    void (*sao_band_filter[5])(uint8_t *_dst, const uint8_t *_src, ptrdiff_t _stride_dst, ptrdiff_t _stride_src,
+                               const int16_t *sao_offset_val, int sao_left_class, int width, int height);
+    void (*sao_edge_filter[5])(uint8_t *_dst, const uint8_t *_src, ptrdiff_t stride_dst, const int16_t *sao_offset_val,
+                               int sao_eo_class, int width, int height);
+    void (*sao_edge_restore[2])(uint8_t *_dst, const uint8_t *_src, ptrdiff_t _stride_dst, ptrdiff_t _stride_src,
+                                const struct SAOParams *sao, const int *borders, int _width, int _height, int c_idx,
+                                const uint8_t *vert_edge, const uint8_t *horiz_edge, const uint8_t *diag_edge);
+    void (*put_hevc_qpel[10][2][2])(int16_t *dst, const uint8_t *src, ptrdiff_t srcstride, int height, intptr_t mx, intptr_t my, int width);
+    void (*put_hevc_qpel_uni[10][2][2])(uint8_t *dst, ptrdiff_t dststride, const uint8_t *src, ptrdiff_t srcstride, int height,
+                                        intptr_t mx, intptr_t my, int width);
+    void (*put_hevc_qpel_uni_w[10][2][2])(uint8_t *_dst, ptrdiff_t _dststride, const uint8_t *_src, ptrdiff_t _srcstride, int height,
+                                          int denom, int wx, int ox, intptr_t mx, intptr_t my, int width);
+    void (*put_hevc_qpel_bi[10][2][2])(uint8_t *dst, ptrdiff_t dststride, const uint8_t *_src, ptrdiff_t _srcstride, const int16_t *src2,
+                                       int height, intptr_t mx, intptr_t my, int width);
+    void (*put_hevc_qpel_bi_w[10][2][2])(uint8_t *dst, ptrdiff_t dststride, const uint8_t *_src, ptrdiff_t _srcstride, const int16_t *src2,
+                                         int height, int denom, int wx0, int wx1, int ox, intptr_t mx, intptr_t my, int width);
+    void (*put_hevc_epel[10][2][2])(int16_t *dst, const uint8_t *src, ptrdiff_t srcstride, int height, intptr_t mx, intptr_t my, int width);
+    void (*put_hevc_epel_uni[10][2][2])(uint8_t *dst, ptrdiff_t dststride, const uint8_t *_src, ptrdiff_t _srcstride, int height,
+                                        intptr_t mx, intptr_t my, int width);
+    void (*put_hevc_epel_uni_w[10][2][2])(uint8_t *_dst, ptrdiff_t _dststride, const uint8_t *_src, ptrdiff_t _srcstride, int height,
+                                          int denom, int wx, int ox, intptr_t mx, intptr_t my, int width);
+    void (*put_hevc_epel_bi[10][2][2])(uint8_t *dst, ptrdiff_t dststride, const uint8_t *_src, ptrdiff_t _srcstride, const int16_t *src2,
+                                       int height, intptr_t mx, intptr_t my, int width);
+    void (*put_hevc_epel_bi_w[10][2][2])(uint8_t *dst, ptrdiff_t dststride, const uint8_t *_src, ptrdiff_t _srcstride, const int16_t *src2,
+                                         int height, int denom, int wx0, int wx1, int ox, intptr_t mx, intptr_t my, int width);
+    void (*hevc_h_loop_filter_luma)(uint8_t *pix, ptrdiff_t stride, int beta, const int32_t *tc, const uint8_t *no_p, const uint8_t *no_q);
+    void (*hevc_v_loop_filter_luma)(uint8_t *pix, ptrdiff_t stride, int beta, const int32_t *tc, const uint8_t *no_p, const uint8_t *no_q);
+    void (*hevc_h_loop_filter_chroma)(uint8_t *pix, ptrdiff_t stride, const int32_t *tc, const uint8_t *no_p, const uint8_t *no_q);
+    void (*hevc_v_loop_filter_chroma)(uint8_t *pix, ptrdiff_t stride, const int32_t *tc, const uint8_t *no_p, const uint8_t *no_q);
+    void (*hevc_h_loop_filter_luma_c)(uint8_t *pix, ptrdiff_t stride, int beta, const int32_t *tc, const uint8_t *no_p, const uint8_t *no_q);
+    void (*hevc_v_loop_filter_luma_c)(uint8_t *pix, ptrdiff_t stride, int beta, const int32_t *tc, const uint8_t *no_p, const uint8_t *no_q);
+    void (*hevc_h_loop_filter_chroma_c)(uint8_t *pix, ptrdiff_t stride, const int32_t *tc, const uint8_t *no_p, const uint8_t *no_q);
+    void (*hevc_v_loop_filter_chroma_c)(uint8_t *pix, ptrdiff_t stride, const int32_t *tc, const uint8_t *no_p, const uint8_t *no_q);
+} B200HEVCDSPContext;
+/* 0; B200_EINVAL for c == NULL; B200_ENOSYS for depths other than 8, 9, 10 and 12 (the reference installs its 8-bit functions for
+ * those, but its decoder refuses such streams before it initialises the context, hevc/ps.c:1193-1215); B200_ENODEV. */
+int  b200_hevc_dsp_init(B200HEVCDSPContext *c, int bit_depth);
+
+/* One prediction unit of b200_hevc_mc_batch_device.  Reference r (0, 1) is the picture whose sample (0, 0) is at ref + ref_off[r]
+ * (bytes, may be negative); the block's integer-sample position in it is (x[r], y[r]) (any value), its phase (mx[r], my[r]) (0..3
+ * for qpel, 0..7 for epel).  The block is w x h samples at dst + dst_off (bytes).  kind:
+ *   B200_HEVC_MC_UNI    put_hevc_?pel_uni[idx][!!my0][!!mx0] on reference 0
+ *   B200_HEVC_MC_UNI_W  put_hevc_?pel_uni_w[..] on reference 0 with (denom, wx0, ox)
+ *   B200_HEVC_MC_BI     put_hevc_?pel[..](tmp, reference 0), then put_hevc_?pel_bi[idx][!!my1][!!mx1](dst, reference 1, tmp)
+ *   B200_HEVC_MC_BI_W   the same with put_hevc_?pel_bi_w[..](denom, wx0, wx1, ox); ox = o0 + o1 (hevcdec.c:1853-1859)
+ * ox is the slice header's 8-bit offset; the functions scale it by 1 << (depth - 8). */
+enum { B200_HEVC_MC_UNI = 0, B200_HEVC_MC_UNI_W = 1, B200_HEVC_MC_BI = 2, B200_HEVC_MC_BI_W = 3 };
+typedef struct B200HevcMcOp {
+    int64_t dst_off;
+    int64_t ref_off[2];
+    int32_t x[2], y[2];
+    uint8_t mx[2], my[2];
+    uint8_t w, h, kind, denom;
+    int32_t wx0, wx1, ox;
+    uint8_t reserved[4];
+} B200HevcMcOp;
+#ifdef __cplusplus
+static_assert(sizeof(B200HevcMcOp) == 64, "B200HevcMcOp is 64 bytes");
+#else
+_Static_assert(sizeof(B200HevcMcOp) == 64, "B200HevcMcOp is 64 bytes");
+#endif
+/* Batched HEVC inter prediction of one plane, DEVICE pointers: epel 0 = luma (8-tap qpel), 1 = chroma (4-tap epel).  Every op's
+ * result is the reference's call sequence above, its source samples read with edge replication: coordinates clamped to
+ * [0, pic_w) x [0, pic_h), which is what the decoder's emulated_edge_mc windows give (hevcdec.c:1813-1845, :1906-1923), so no
+ * separate edge emulation pass is needed.  Both references share ref_stride and the picture size.  The caller guarantees that the
+ * ops of one call write disjoint blocks and that no op reads samples another op of the call writes (the current-picture reference
+ * of screen-content coding needs a call of its own).  An op whose w or h is outside 1..64, whose kind is undefined, whose phase is
+ * out of range or whose dst_off / ref_off is not a multiple of the sample size writes nothing.
+ * Returns 0, or B200_EINVAL (launching nothing) for NULL pointers, nops < 0, epel not 0 / 1, a stride not a multiple of the sample
+ * size, pic_w or pic_h < 1, or a depth other than 8, 9, 10 or 12; nops == 0 returns 0. */
+int  b200_hevc_mc_batch_device(B200Device *dev, int bit_depth, int epel, int64_t nops, const B200HevcMcOp *ops,
+                               uint8_t *dst, ptrdiff_t dst_stride, const uint8_t *ref, ptrdiff_t ref_stride, int pic_w, int pic_h);
+
 /* mpegvideo inverse quantisers: the members of MPVUnquantDSPContext (libavcodec/mpegvideo_unquantize.h:31-44) as
  * ff_mpv_unquantize_init() installs them (libavcodec/mpegvideo_unquantize.c:50-290), i.e. what runs in front of the IDCT in
  * mpv_reconstruct_mb's put_dct / add_dequant_dct (libavcodec/mpegvideo_dec.c).  The reference functions take the whole

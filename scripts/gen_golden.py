@@ -17,6 +17,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import cpulibs as cl  # noqa: E402
 import h264predlib as hp  # noqa: E402
+import hevcmclib as hm  # noqa: E402
 from cases import SWS_SMALL_CASES, SWS_HASH_CASES, idct_blocks  # noqa: E402
 
 OUT = os.path.join(ROOT, "tests", "golden")
@@ -270,6 +271,16 @@ def gen_h264pred():
                 h = hashlib.sha256(np.ascontiguousarray(pic).tobytes() + np.ascontiguousarray(cf).tobytes()).hexdigest()
                 lines.append(f"{depth} {idc} {'add' if add else 'pred'} {h}")
     open(os.path.join(OUT, "h264pred_hashes.txt"), "w").write("\n".join(lines) + "\n")
+
+
+def gen_hevcmc():
+    """HEVC motion compensation: sha256 of the reference's destination picture after the seeded batch of hm.fixture_case (the decoder's
+    emulated_edge_mc windows and put_hevc_* calls, oracle/ref/ref_hevcdsp.c) per depth x luma (qpel) / chroma (epel)"""
+    lines = []
+    for depth in hm.DEPTHS:
+        for epel in (0, 1):
+            lines.append(f"{depth} {'chroma' if epel else 'luma'} {hm.digest(hm.ref_batch(depth, epel, *hm.fixture_case(depth, epel)))}")
+    open(os.path.join(OUT, "hevcmc_hashes.txt"), "w").write("\n".join(lines) + "\n")
 
 
 def gen_tx_double():
@@ -799,6 +810,7 @@ if __name__ == "__main__":
     gen_h264_idct_hbd()
     gen_h264lf_hbd()
     gen_h264pred()
+    gen_hevcmc()
     gen_tx_double()
     gen_sws_rgb2rgb()
     gen_tx_full_imdct()

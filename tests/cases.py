@@ -201,3 +201,52 @@ SWS_FILTER_CASES = [
     (50, 40, 25, 20, 0x10, "bgra", (None, None, None, None), (3, 0, 3, 0)),                                      # destination vectors only: wider rows, same taps
     (128, 64, 96, 80, 0x20, "yuv420p", ([1.0], [1.0], [1.0], [1.0]), (1, 1, 1, 1)),                              # one-tap vectors: nothing changes
 ]
+
+
+# The scaled path's three kernels (csrc/sws.cu launch_batch / launch_planar3), as b200_sws_last_path reports them: 4 the fused tensor-core
+# kernels (csrc/sws_mma.cuh), 2 the fused CUDA-core kernels, 1 two passes through int16 line planes; a yuv420p destination ORs the bits of
+# its three planes.  Each row: geometry, flags, optional `param` / `src_filter` (lumH, lumV, chrH, chrV) / nv12 or nv21 `src_fmt`, the
+# kernels expected for each destination in the three memory layouts of tests/test_sws_scaled_paths_gpu.py (A: everything 16-byte aligned;
+# B: source planes at base + 1 with odd strides; C: destination at base + 1 with an odd stride), and what the row is there to reach
+# (tests/test_sws_mma_plan.py REACHES says what each name means and checks it on the host).
+_SHARPEN = [-0.5, 2.0, -0.5]
+_P = (4, 2, 1)                  # tensor-core kernel where aligned, CUDA-core fused kernel from misaligned sources, two passes into a misaligned destination
+_TWO = (1, 1, 1)
+_STD = {"rgb24": _P, "bgra": _P, "yuv420p": _P}
+SWS_PATH_CASES = [
+    dict(geom=(3840, 2160, 1920, 1080), flags=FATE, paths=_STD, reaches=("nch=1", "dstH%TR")),
+    dict(geom=(1920, 1080, 3840, 2160), flags=FATE, paths=_STD, reaches=("up2x",)),
+    dict(geom=(3840, 2160, 1280, 720), flags=FATE, paths=_STD, reaches=("nch=1",)),
+    dict(geom=(3840, 2160, 960, 540), flags=FATE, paths=_STD, reaches=("nch=2", "smem>75K", "ngc<8")),
+    dict(geom=(1920, 1080, 240, 540), flags=FATE, paths={"rgb24": (4, 1, 1), "bgra": (4, 1, 1), "yuv420p": (4, 1, 1)},
+         reaches=("nch>=3", "taps>16", "smem>75K", "dstH%TR")),
+    dict(geom=(1920, 1080, 960, 540), flags=SWS_LANCZOS | SWS_ACCURATE_RND | SWS_BITEXACT, param=(5.0, 123456.0),
+         paths={"rgb24": (4, 1, 1), "bgra": (4, 1, 1), "yuv420p": (4, 1, 1)}, reaches=("taps>16", "nch=2")),
+    dict(geom=(1024, 608, 96, 64), flags=FATE, paths={"rgb24": _TWO, "bgra": _TWO, "yuv420p": _TWO}, reaches=("no tile fits",)),
+    dict(geom=(1280, 720, 640, 360), flags=SWS_POINT, paths={"rgb24": _TWO, "bgra": _TWO, "yuv420p": _P}, reaches=("vfs=1",)),
+    dict(geom=(1920, 1080, 1280, 1080), flags=FATE, paths=_STD, reaches=("vfs=1", "hscaled")),
+    dict(geom=(1920, 1080, 640, 352), flags=SWS_AREA, paths=_STD, reaches=("rgb row tile of 1",)),
+    dict(geom=(640, 360, 1280, 720), flags=SWS_AREA, paths={"rgb24": _TWO, "bgra": _TWO, "yuv420p": _P}, reaches=("2-tap",)),
+    dict(geom=(1280, 720, 1920, 1080), flags=SWS_BILINEAR | SWS_ACCURATE_RND | SWS_BITEXACT, paths={"rgb24": _TWO, "bgra": _TWO, "yuv420p": _P},
+         reaches=("2-tap",)),
+    dict(geom=(1920, 1080, 1280, 720), flags=SWS_BICUBLIN, paths=_STD, reaches=("bicublin",)),
+    dict(geom=(1366, 768, 1920, 1080), flags=FATE, paths=_STD, reaches=("srcW%16",)),
+    dict(geom=(1365, 765, 640, 352), flags=FATE, paths=_STD, reaches=("srcW%16", "odd chroma")),
+    dict(geom=(8, 6, 32, 24), flags=FATE, paths=_STD, reaches=("srcW<16", "2-tap")),
+    dict(geom=(12, 2, 48, 8), flags=FATE, paths={"rgb24": _TWO, "bgra": _TWO, "yuv420p": _P}, reaches=("srcW<16", "vfs=1")),
+    dict(geom=(200, 120, 16, 16), flags=FATE, paths={"rgb24": (4, 1, 1), "bgra": (4, 1, 1), "yuv420p": (4, 1, 1)}, reaches=("one tile of 2 groups",)),
+    dict(geom=(400, 300, 144, 100), flags=FATE, paths=_STD, reaches=("second tile of 2 groups",)),
+    dict(geom=(2000, 64, 1040, 40), flags=FATE, paths=_STD, reaches=("partial column tile", "ngc<8")),
+    dict(geom=(640, 360, 256, 161), flags=FATE, paths=_STD, reaches=("rgb row tile of 1",)),
+    dict(geom=(640, 480, 512, 163), flags=FATE, paths=_STD, reaches=("luma row tile of 1",)),
+    dict(geom=(400, 300, 136, 90), flags=FATE, paths={"yuv420p": (5, 3, 1)}, reaches=("chroma dstW%8",)),
+    dict(geom=(1920, 1080, 1280, 720), flags=FATE, src_filter=(_SHARPEN, None, _SHARPEN, None), paths=_STD, reaches=("coef>16384", "clamp")),
+    dict(geom=(1920, 1080, 1280, 720), flags=FATE, src_fmt=23, paths={"rgb24": _P, "bgra": _P, "yuv420p": (4, 6, 1)}, reaches=("nv",)),
+    dict(geom=(1920, 1080, 1280, 720), flags=FATE, src_fmt=24, paths={"rgb24": _P, "bgra": _P, "yuv420p": (4, 6, 1)}, reaches=("nv",)),
+    dict(geom=(1366, 768, 1024, 576), flags=FATE, src_fmt=23, paths={"rgb24": _P, "bgra": _P, "yuv420p": (4, 6, 1)}, reaches=("nv", "srcW%16")),
+    dict(geom=(1366, 768, 1024, 576), flags=FATE, src_fmt=24, paths={"rgb24": _P, "bgra": _P, "yuv420p": (4, 6, 1)}, reaches=("nv", "srcW%16")),
+    dict(geom=(640, 368, 320, 184), flags=FATE, paths=_STD, reaches=("nch=1",)),
+    dict(geom=(1920, 1088, 1280, 720), flags=FATE, paths={k: _P for k in ("rgb24", "bgr24", "rgba", "bgra", "argb", "abgr", "yuv420p")},
+         reaches=("nch=1",)),
+    dict(geom=(704, 576, 1408, 1152), flags=SWS_BICUBIC, paths=_STD, reaches=("up2x",)),
+]

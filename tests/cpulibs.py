@@ -211,6 +211,15 @@ def yuv_frame(w, h, seed, kind="random", pad=0):
         y = rng.integers(0, 256, (h, w + pad), dtype=np.uint8)
         u = rng.integers(0, 256, (ch, cw + pad), dtype=np.uint8)
         v = rng.integers(0, 256, (ch, cw + pad), dtype=np.uint8)
+    elif kind == "extremes":
+        # blocks of 0 / 255 stripes of period 2 and 3 across columns and across rows, flat 0 and flat 255 (each plane its own arrangement):
+        # the horizontal sums reach both ends of their range and, under sharpening filters, the clamp at 32767 and values below 0
+        def ext(hh, ww, shift):
+            yy, xx = np.mgrid[0:hh, 0:ww]
+            pat = np.stack([xx % 2 == 0, xx % 3 == 0, yy % 2 == 0, yy % 3 == 0, np.zeros_like(xx, bool), np.ones_like(xx, bool)])
+            blk = (xx // max(6, ww // 4 // 6 * 6) + yy // max(6, hh // 3 // 6 * 6) + shift) % 6
+            return np.where(np.take_along_axis(pat, blk[None], 0)[0], 255, 0).astype(np.uint8)
+        y, u, v = ext(h, w + pad, 0), ext(ch, cw + pad, 2), ext(ch, cw + pad, 4)
     elif kind == "limited":
         y = rng.integers(16, 236, (h, w + pad), dtype=np.uint8)
         u = rng.integers(16, 241, (ch, cw + pad), dtype=np.uint8)
@@ -318,13 +327,13 @@ PIX_FMT_YUV420P = 0
 
 
 def _sws_run_planar(lib, pre, w, h, dw, dh, flags, y, u, v, dst_pad=0, threads=1, src_fmt=0, ranges=(0, 0), details=None,
-                    dst_fmt=PIX_FMT_YUV420P, filters=None):
+                    dst_fmt=PIX_FMT_YUV420P, filters=None, param=None):
     """yuv420p / nv12 / nv21 -> yuv420p; returns (Y, U, V) destination planes (pad bytes stay 0xA5).
     ranges = (src_range, dst_range) given before initialisation; details = (src_cs, src_range, dst_cs, dst_range,
     brightness, contrast, saturation) for a sws_setColorspaceDetails() call after it.
-    dst_fmt nv12 / nv21: returns (Y, UV) with UV the interleaved plane."""
-    if filters is not None:
-        ctx = _open_filters(lib, pre, src_fmt, w, h, ranges[0], dst_fmt, dw, dh, ranges[1], flags, threads, filters, None)
+    dst_fmt nv12 / nv21: returns (Y, UV) with UV the interleaved plane.  param: sws_getContext's two scaler parameters"""
+    if filters is not None or param is not None:
+        ctx = _open_filters(lib, pre, src_fmt, w, h, ranges[0], dst_fmt, dw, dh, ranges[1], flags, threads, filters or (None, None), param)
     elif pre == "ffref":
         ctx = lib.ffref_sws_open_range(src_fmt, w, h, ranges[0], dst_fmt, dw, dh, ranges[1], flags, threads)
     else:

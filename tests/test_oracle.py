@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 import cpulibs as cl
-from cases import SWS_SMALL_CASES, SWS_HASH_CASES, FATE, idct_blocks
+from cases import SWS_SMALL_CASES, SWS_HASH_CASES, SWS_PATH_CASES, FATE, idct_blocks
 
 G = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
@@ -149,6 +149,29 @@ def test_sws_oracle_vs_reference_live(case):
             assert rc.same(b, lambda: cl.ref_sws(w, h, dw, dh, fl, y, u, v, dst_pad=5))
 
 
+@pytest.mark.parametrize("row", SWS_PATH_CASES, ids=lambda r: "x".join(map(str, r["geom"])) + f"-{r['flags']:x}-{r.get('src_fmt', 0)}")
+def test_sws_path_cases_oracle_vs_reference(row):
+    """the oracle the scaled-path GPU tests compare with (tests/test_sws_scaled_paths_gpu.py), against the reference on every row and
+    destination of SWS_PATH_CASES: nv12 / nv21 sources, `param` and `src_filter` included; one input kind for the 4K rows"""
+    w, h, dw, dh = row["geom"]
+    sf = row.get("src_fmt", 0)
+    kw = dict(src_fmt=sf, param=row.get("param"), filters=(row["src_filter"], None) if row.get("src_filter") else None)
+    kinds = ("extremes",) if max(w * h, dw * dh) >= 3840 * 2160 else ("random", "smooth", "limited", "extremes")
+    with cl.RefCheck() as rc:
+        for i, kind in enumerate(kinds):
+            y, u, v = cl.yuv_frame(w, h, 40 + i, kind, pad=7)
+            if sf:
+                u = v = cl.nv_interleave(u, v, sf, pad=5)
+            for dest in row["paths"]:
+                if dest == "yuv420p":
+                    b = cl.orc_sws_planar(w, h, dw, dh, row["flags"], y, u, v, dst_pad=3, **kw)
+                    assert rc.same(b, lambda: cl.ref_sws_planar(w, h, dw, dh, row["flags"], y, u, v, dst_pad=3, **kw)), (kind, dest)
+                else:
+                    f = cl.PACKED_RGB_FORMATS[dest]
+                    b = cl.orc_sws(w, h, dw, dh, row["flags"], y, u, v, dst_pad=5, fmt=f, **kw)
+                    assert rc.same(b, lambda: cl.ref_sws(w, h, dw, dh, row["flags"], y, u, v, dst_pad=5, fmt=f, **kw)), (kind, dest)
+
+
 def test_idct_oracle_vs_reference_live():
     O = cl.oracle()
     n = 4096
@@ -172,7 +195,8 @@ def test_host_filter_tables_match_oracle():
     """The product's host-side filter generation (sws_plan.cpp) against the oracle's, no GPU involved."""
     import ffmpeg_b200 as fb
     L, O = fb.lib(), cl.oracle()
-    for (w, h, dw, dh, fl, _k) in SWS_SMALL_CASES + SWS_HASH_CASES + [(3840, 2160, 3840, 2160, FATE, ""), (3840, 2160, 1920, 1080, FATE, "")]:
+    path_rows = [(*r["geom"], r["flags"], "") for r in SWS_PATH_CASES if not r.get("param") and not r.get("src_filter")]
+    for (w, h, dw, dh, fl, _k) in SWS_SMALL_CASES + SWS_HASH_CASES + [(3840, 2160, 3840, 2160, FATE, "")] + path_rows:
         ctx = O.orc_sws_open(w, h, dw, dh, fl)
         assert ctx
         oi = np.zeros(16, np.int32)

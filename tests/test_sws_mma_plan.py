@@ -6,6 +6,7 @@ import ctypes as C
 import numpy as np
 import pytest
 import cpulibs as cl
+from cases import SWS_PATH_CASES
 from ffmpeg_b200._lib import lib
 
 
@@ -90,6 +91,157 @@ def test_library_banks_replay(srcW, dstW, flags):
         coef = f[:n * size].reshape(n, size).copy(); pos = p[:n].copy()
         assert int(pos.min()) >= 0 and int((pos + size).max()) <= sw
         src = rng.integers(0, 256, (37, sw), dtype=np.uint8)
+        ref = hscale_direct(src, coef, pos)
+        for tg in (16, 8):
+            assert np.array_equal(replay_tiles(src, coef, pos, tg), ref), (which, tg)
+
+
+MT_W, MT_TPB, MT_CPB, MT_HDR = 128, 128 * 4 + 32, 128 * 2 + 32, 16      # sws_mma.cuh
+
+
+def case_banks(row, dest):
+    """info (as b200_sws_info) and the four filter banks {0: hLum, 1: hChr, 2: vLum, 3: vChr} as (coef, pos) of a SWS_PATH_CASES row, from the
+    oracle (whose tables test_host_filter_tables_match_oracle pins to the library's; this also covers `param` and `src_filter`)"""
+    w, h, dw, dh = row["geom"]
+    O = cl.oracle()
+    fmt = 0 if dest == "yuv420p" else cl.PACKED_RGB_FORMATS[dest]
+    ctx = cl._open_filters(O, "orc", row.get("src_fmt", 0), w, h, 0, fmt, dw, dh, 0, row["flags"], 1, (row.get("src_filter"), None), row.get("param"))
+    assert ctx
+    info = np.zeros(16, np.int32)
+    O.orc_sws_info(ctx, cl.ptr(info, cl.i32p))
+    banks = {}
+    for which in range(4):
+        size, n = int(info[which]), [dw, int(info[6]), dh, int(info[7])][which]
+        f, p = np.zeros(n * size, np.int16), np.zeros(n, np.int32)
+        O.orc_sws_get_filter(ctx, which, cl.ptr(f, cl.i16p), cl.ptr(p, cl.i32p), n)
+        banks[which] = (f.reshape(n, size), p)
+    O.orc_sws_close(ctx)
+    return info, banks
+
+
+def rows_needed(bank, srcH, dstH, TR):
+    """fused_rows_needed (csrc/sws.cu): staged lines of the tallest tile of TR output lines, -1 when a tile's windows are not nested"""
+    coef, pos = bank
+    size, mx = coef.shape[1], 0
+    win = [(min(max(max(1 - size, int(p)), 0), srcH - 1), min(max(max(1 - size, int(p)) + size - 1, 0), srcH - 1)) for p in pos]
+    for dy0 in range(0, dstH, TR):
+        ra, rb = win[dy0][0], win[min(dy0 + TR, dstH) - 1][1]
+        if rb < ra or any(a < ra or b > rb for a, b in win[dy0:dy0 + TR]):
+            return -1
+        mx = max(mx, rb - ra + 1)
+    return mx
+
+
+def mma_tiles(row, dest):
+    """The tile heights launch_batch / launch_planar3 pick for the tensor-core kernels at the row's geometry: [(TR, shared bytes)] for the
+    packed-RGB kernel or for the luma and chroma plane kernels; (None, None) where no height fits (the other kernels take over)"""
+    info, banks = case_banks(row, dest)
+    w, h, dw, dh = row["geom"]
+    csh = int(info[5])
+    pitch = {k: mma_tables(*banks[k])[2] for k in (0, 1)}
+    out = []
+    if dest == "yuv420p":
+        for k, sh, dhh in ((0, h, dh), (1, csh, int(info[7]))):
+            SP = int(pitch[k][0])
+            best, pick = 1e30, (None, None)
+            for TR in range(32, 7, -1):
+                r = rows_needed(banks[k + 2], sh, dhh, TR)
+                sm = MT_HDR + ((r + 15) & ~15) * (SP + MT_TPB)
+                if r <= 0 or sm > 112 * 1024:
+                    continue
+                cost = ((r + 15) >> 4) / TR * (1.0 + (0.15 if sm > 56 * 1024 else 0) + (0.15 if sm > 75 * 1024 else 0))
+                if cost < best - 1e-9:
+                    best, pick = cost, (TR, sm)
+            out.append(pick)
+        return out
+
+    def need(TR):
+        rl, rc = rows_needed(banks[2], h, dh, TR), rows_needed(banks[3], csh, dh, TR)
+        return (rl, rc), MT_HDR + ((rl + 15) & ~15) * (int(pitch[0][0]) + MT_TPB) + 2 * ((rc + 15) & ~15) * (int(pitch[1][1]) + MT_CPB)
+    (rl, rc), sm = need(16)
+    if rl > 0 and rc > 0 and sm <= 80 * 1024:
+        return [(16, sm)]
+    best, pick = 1e30, (None, None)
+    for TR in range(32, 7, -1):
+        (rl, rc), sm = need(TR)
+        if rl <= 0 or rc <= 0 or sm > 112 * 1024:
+            continue
+        cost = (((rl + 15) >> 4) + ((rc + 15) >> 4)) / TR * (1.0 + (0.15 if sm > 56 * 1024 else 0) + (0.15 if sm > 75 * 1024 else 0))
+        if cost < best - 1e-9:
+            best, pick = cost, (TR, sm)
+    return [pick]
+
+
+def _groups_nch(row):
+    ginfo = mma_tables(*case_banks(row, "yuv420p")[1][0])[0]
+    return np.diff(ginfo[:, 1])
+
+
+def _clamps(row):
+    """the luma horizontal pass over the `extremes` input, before hScale8To15_c's clamp, goes above 32767 and below 0"""
+    coef, pos = case_banks(row, "yuv420p")[1][0]
+    y = cl.yuv_frame(*row["geom"][:2], 0, "extremes")[0]
+    acc = (y[:, pos[:, None] + np.arange(coef.shape[1])[None, :]].astype(np.int64) * coef[None].astype(np.int64)).sum(axis=2) >> 7
+    return int(acc.max()) > 32767 and int(acc.min()) < 0
+
+
+def _tile(row, dest, plane=0):
+    return mma_tiles(row, dest)[plane][0] or 0
+
+
+# What a SWS_PATH_CASES row says it reaches, checked on the host tables (chunks and tiles as csrc/sws.cu and sws_mma.cuh derive them)
+REACHES = {
+    "nch=1": lambda r: _groups_nch(r).max() == 1,                                           # every group one 32-column chunk
+    "nch=2": lambda r: _groups_nch(r).max() == 2,                                           # the two-chunk instantiation
+    "nch>=3": lambda r: _groups_nch(r).max() >= 3,                                          # the general chunk loop (NCH == 0)
+    "up2x": lambda r: r["geom"][2] >= 2 * r["geom"][0],
+    "dstH%TR": lambda r: all(_tile(r, d) and r["geom"][3] % _tile(r, d) for d in ("rgb24", "yuv420p")),
+    "taps>16": lambda r: case_banks(r, "rgb24")[0][0] > 16,                                 # no CUDA-core fused kernel
+    "smem>75K": lambda r: (mma_tiles(r, "rgb24")[0][1] or 0) > 75 * 1024,
+    "no tile fits": lambda r: mma_tiles(r, "rgb24")[0][0] is None and mma_tiles(r, "yuv420p")[0][0] is None,
+    "vfs=1": lambda r: case_banks(r, "yuv420p")[0][2] == 1,
+    "hscaled": lambda r: case_banks(r, "yuv420p")[0][0] > 1,
+    "2-tap": lambda r: 2 in [int(x) for x in case_banks(r, "yuv420p")[0][:4]],
+    "srcW%16": lambda r: r["geom"][0] % 16 != 0,
+    "odd chroma": lambda r: case_banks(r, "yuv420p")[0][4] % 2 == 1 and case_banks(r, "yuv420p")[0][5] % 2 == 1,
+    "srcW<16": lambda r: r["geom"][0] < 16,
+    "bicublin": lambda r: case_banks(r, "yuv420p")[0][1] < case_banks(r, "yuv420p")[0][0],
+    "one tile of 2 groups": lambda r: (r["geom"][2] + 7) // 8 == 2,
+    "second tile of 2 groups": lambda r: (r["geom"][2] + 7) // 8 % 16 == 2 and r["geom"][2] > 128,
+    "partial column tile": lambda r: r["geom"][2] % 128 != 0,
+    "ngc<8": lambda r: (case_banks(r, "rgb24")[0][6] + 7) // 8 - 8 * ((r["geom"][2] + 127) // 128 - 1) < 8,    # chroma groups of the last RGB tile
+    "rgb row tile of 1": lambda r: _tile(r, "rgb24") and r["geom"][3] % _tile(r, "rgb24") == 1,
+    "luma row tile of 1": lambda r: _tile(r, "yuv420p") and r["geom"][3] % _tile(r, "yuv420p") == 1,
+    "chroma dstW%8": lambda r: r["geom"][2] % 8 == 0 and case_banks(r, "yuv420p")[0][6] % 8 != 0,                # plane kernels need dstW % 8
+    "coef>16384": lambda r: int(case_banks(r, "yuv420p")[1][0][0].max()) > 16384,          # high byte of the split above 63
+    "clamp": _clamps,
+    "nv": lambda r: r.get("src_fmt", 0) in (23, 24),
+}
+
+
+@pytest.mark.parametrize("row", SWS_PATH_CASES, ids=lambda r: "x".join(map(str, r["geom"])) + f"-{r['flags']:x}-{r.get('src_fmt', 0)}")
+def test_path_cases_reach_their_code(row):
+    for what in row["reaches"]:
+        assert REACHES[what](row), what
+
+
+def test_path_cases_cover_chunks_and_kernels():
+    """the rows between them take groups of one, two and three or more chunks, and expect each of the three kernels for every destination"""
+    top = {int(_groups_nch(r).max()) for r in SWS_PATH_CASES}
+    assert {1, 2} <= top and max(top) >= 3, top
+    for dest in ("rgb24", "bgra", "yuv420p"):
+        seen = {b for r in SWS_PATH_CASES for p in r["paths"].get(dest, ()) for b in (1, 2, 4) if p & b}
+        assert seen == {1, 2, 4}, (dest, seen)
+
+
+@pytest.mark.parametrize("row", SWS_PATH_CASES, ids=lambda r: "x".join(map(str, r["geom"])) + f"-{r['flags']:x}-{r.get('src_fmt', 0)}")
+def test_path_case_banks_replay(row):
+    """the library's operand tables of every SWS_PATH_CASES bank, through the lane-by-lane replay, against hScale8To15_c"""
+    info, banks = case_banks(row, "yuv420p")
+    rng = np.random.default_rng(sum(row["geom"]))
+    for which, sw in ((0, row["geom"][0]), (1, int(info[4]))):
+        coef, pos = banks[which]
+        src = rng.integers(0, 256, (17, sw), dtype=np.uint8)
         ref = hscale_direct(src, coef, pos)
         for tg in (16, 8):
             assert np.array_equal(replay_tiles(src, coef, pos, tg), ref), (which, tg)

@@ -23,6 +23,11 @@ def me_cmp_set_dct_algo(dct_algo):
     return check(lib().b200_me_cmp_set_dct_algo(dct_algo), "me_cmp_set_dct_algo")
 
 
+def me_cmp_set_nsse_weight(weight):
+    """nsse's noise weight (the reference reads avctx->nsse_weight, 8 for a NULL context); process-wide, default 8"""
+    lib().b200_me_cmp_set_nsse_weight(weight)
+
+
 def me_cmp_batch_device(device, fn, idx, frame1, frame2, stride, h, off1, off2, n, out):
     return check(lib().b200_me_cmp_batch_device(device.handle, fn, idx, vp(_dptr(frame1)), vp(_dptr(frame2)), stride, h,
                                                 vp(_dptr(off1)), vp(_dptr(off2)), n, vp(_dptr(out))), "me_cmp_batch_device")

@@ -614,7 +614,9 @@ int  b200_me_cmp_batch_device(B200Device *dev, int fn, int idx, const uint8_t *f
  * like vf_mestimate.c:85-127 — for every mb_size x mb_size block of every frame pair: cost of the zero vector first,
  * raster scan of the +-search_param window clipped to the frame, strict '<' (first minimum in raster order wins, the
  * zero vector wins ties against everything).  mb_size in {4, 8, 16}.  out_mv: 2 ints (absolute x, y of the best match)
- * per block in raster order per frame; out_cost: its SAD. */
+ * per block in raster order per frame; out_cost: its SAD.  The window is staged in shared memory at its unclipped size, so
+ * search_param >= 217 / 221 / 223 for mb_size 16 / 8 / 4 returns B200_ENOSYS and writes nothing, whatever the frame size
+ * (vf_mestimate accepts any search_param >= 4). */
 int  b200_me_esa_device(B200Device *dev, const uint8_t *cur, const uint8_t *ref, int linesize, int width, int height,
                         int64_t frame_stride, int nframes, int mb_size, int search_param, int32_t *out_mv, uint64_t *out_cost);
 /* same on HOST buffers (vf_mestimate's frames live in host memory): chunks of frame pairs rotate over three streams, H2D of both luma

@@ -276,6 +276,10 @@ int orc_sum_abs_dctelem(const int16_t *block)
     return sum;
 }
 
+/* nsse's weight: avctx->nsse_weight of the encoder context, 8 for a NULL context (me_cmp.c:407-410) */
+static int g_nsse_weight = 8;
+void orc_me_cmp_set_nsse_weight(int weight) { g_nsse_weight = weight; }
+
 int orc_me_cmp(int fn, int idx, const uint8_t *blk1, const uint8_t *blk2, ptrdiff_t stride, int h)
 {
     if (fn >= 8 && fn <= 10) {                                     /* dct_sad / dct_max / dct264_sad: [0] 16 wide, [1] 8x8 */
@@ -296,7 +300,7 @@ int orc_me_cmp(int fn, int idx, const uint8_t *blk1, const uint8_t *blk2, ptrdif
         if (idx != 0 && idx != 1 && idx != 4 && idx != 5) return -1;
         return vgrad_wh(blk1, blk2, stride, idx & 1 ? 8 : 16, h, idx >= 4, fn == 5);
     }
-    if (fn == 6) return idx == 0 || idx == 1 ? nsse_wh(blk1, blk2, stride, 16 >> idx, h, 8) : -1;     /* NULL context: weight 8 */
+    if (fn == 6) return idx == 0 || idx == 1 ? nsse_wh(blk1, blk2, stride, 16 >> idx, h, g_nsse_weight) : -1;
     if (fn == 7) return idx == 0 || idx == 1 ? median_sad_wh(blk1, blk2, stride, 16 >> idx, h) : -1;
     if (fn == 3) {
         if (idx == 1) return satd8x8(blk1, blk2, stride);
@@ -309,6 +313,13 @@ int orc_me_cmp(int fn, int idx, const uint8_t *blk1, const uint8_t *blk2, ptrdif
     if (fn == 1) return idx <= 2 ? sse_wh(blk1, blk2, stride, 16 >> idx, h) : -1;
     if (fn == 2) return idx < 8 ? sad_wh(blk1, blk2, stride, idx < 4 ? 16 : 8, h, idx & 3) : -1;
     return -1;
+}
+
+/* out[i] = orc_me_cmp(fn, idx, f1 + off1[i], f2 + off2[i], stride, h): one call for a whole batch */
+void orc_me_cmp_batch(int fn, int idx, const uint8_t *f1, const uint8_t *f2, ptrdiff_t stride, int h,
+                      const int64_t *off1, const int64_t *off2, int64_t n, int32_t *out)
+{
+    for (int64_t i = 0; i < n; i++) out[i] = orc_me_cmp(fn, idx, f1 + off1[i], f2 + off2[i], stride, h);
 }
 
 void orc_esa_frame(const uint8_t *cur, const uint8_t *ref, int linesize, int width, int height,

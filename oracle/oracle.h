@@ -150,6 +150,9 @@ int  orc_me_cmp(int fn, int idx, const uint8_t *blk1, const uint8_t *blk2, ptrdi
 int  orc_sum_abs_dctelem(const int16_t *block);
 void orc_fdct(int kind, int is248, int16_t *block);   /* FDCTDSPContext.fdct / fdct248: kind 0 islow_8, 1 ifast, 2 islow_10 */
 void orc_me_cmp_set_dct_algo(int algo);   /* fn 8 / 9 (dct_sad, dct_max): 0 = ff_jpeg_fdct_islow_8, 1 = ff_fdct_ifast */
+void orc_me_cmp_set_nsse_weight(int weight);   /* fn 6 (nsse): avctx->nsse_weight; 8 (the NULL-context weight) until set */
+void orc_me_cmp_batch(int fn, int idx, const uint8_t *f1, const uint8_t *f2, ptrdiff_t stride, int h,
+                      const int64_t *off1, const int64_t *off2, int64_t n, int32_t *out);
 int  orc_pixelutils_sad(int bits, const uint8_t *src1, ptrdiff_t stride1, const uint8_t *src2, ptrdiff_t stride2);
 void orc_esa_frame(const uint8_t *cur, const uint8_t *ref, int linesize, int width, int height,
                    int mb_size, int search_param, int mb_row0, int mb_row1, int32_t *out_mv, uint64_t *out_cost);

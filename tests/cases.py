@@ -250,3 +250,137 @@ SWS_PATH_CASES = [
          reaches=("nch=1",)),
     dict(geom=(704, 576, 1408, 1152), flags=SWS_BICUBIC, paths=_STD, reaches=("up2x",)),
 ]
+
+
+# ---------------------------------------------------------------- exhaustive motion search (csrc/mecmp.cu launch_esa)
+B200_ENOSYS = -38
+
+
+def esa_kernel_for(mb, search):
+    """Which kernel b200_me_esa_device runs for (mb, search), restating launch_esa<MB>'s shared-memory sizes: "esa2" while the four
+    byte-phase copies of a two-macroblock window fit in 100 KB, "esa" while one window fits in 200 KB, else B200_ENOSYS."""
+    wc = 2 * search + 2 * mb
+    pitch = (wc + 3) // 4 + 1
+    copy_words = (2 * search + mb + 7) * pitch + 1
+    copy_words += (8 - (copy_words & 31) + 32) & 31
+    if (2 * mb * (mb // 4) + 4 * copy_words) * 4 <= 100 * 1024:
+        return "esa2"
+    win_pitch = (2 * search + mb + 3) // 4 + 1
+    return "esa" if (mb * (mb // 4) + (2 * search + mb) * win_pitch) * 4 <= 200 * 1024 else B200_ENOSYS
+
+
+# Inputs of the search (esa_pictures): "flat" and the ties* kinds have several candidates of equal, minimal cost, spread over task groups of 8
+# rows, lanes, warps and both macroblocks of an esa2 CTA.  "ties_zero_min": the zero vector's cost equals the minimum and is not 0;
+# "ties_zero_0": it is 0 (the reference returns at once).  "extremes": inverse checkerboards (the zero vector costs 255 * mb^2, vectors of
+# odd parity 0); "saturated": every candidate costs 255 * mb^2.
+ESA_INPUTS_ALL = ("random", "shifted", "flat", "extremes", "saturated", "ties3", "ties8", "ties17", "ties_zero_min", "ties_zero_0")
+ESA_INPUTS = ("random", "shifted", "flat", "extremes", "ties8", "ties_zero_min")
+
+
+def _esa(w, h, mb, search, expect, note, nf=1, linesize=None, frame_stride=None, cur_off=0, ref_off=0, inputs=ESA_INPUTS, rows=None, group=None):
+    linesize = linesize or w
+    return dict(w=w, h=h, linesize=linesize, frame_stride=frame_stride or linesize * h, cur_off=cur_off, ref_off=ref_off, nf=nf, mb=mb,
+                search=search, expect=expect, note=note, inputs=inputs, rows=rows, group=group)
+
+
+def _boundary(mb, side, lo, last):
+    """the searches just below and above the esa2 / esa boundary and esa's last one on a frame whose window both cover whole (identical
+    outputs expected), and the first search that returns B200_ENOSYS"""
+    g = f"boundary{mb}"
+    return [_esa(side, side, mb, lo, "esa2", f"esa2_kernel<{mb}>, odd b_w, window = whole frame", inputs=ESA_INPUTS_ALL, group=g),
+            _esa(side, side, mb, lo + 1, "esa", f"esa_kernel<{mb}> on the same case", inputs=ESA_INPUTS_ALL, group=g),
+            _esa(side, side, mb, last, "esa", f"esa_kernel<{mb}>, its last search", inputs=ESA_INPUTS_ALL, group=g),
+            _esa(side, side, mb, last + 1, B200_ENOSYS, "first search without a kernel: outputs untouched", inputs=("random",))]
+
+
+_LS = 113                                                         # linesize = width + 13; frames at unaligned bases below
+ESA_CASES = _boundary(16, 80, 64, 216) + _boundary(8, 72, 70, 220) + _boundary(4, 76, 74, 222) + [
+    _esa(171, 107, 8, 75, "esa", "esa_kernel<8>, window inside the frame, size not a multiple of mb"),
+    _esa(174, 102, 4, 80, "esa", "esa_kernel<4>, window inside the frame, size not a multiple of mb"),
+    _esa(250, 170, 16, 70, "esa", "esa_kernel<16>, window inside the frame, size not a multiple of mb"),
+    _esa(336, 200, 16, 32, "esa2", "odd b_w (21) at an everyday search, 8-row partial bottom band"),
+    _esa(16, 200, 16, 32, "esa2", "b_w = 1"),
+    _esa(200, 16, 16, 32, "esa2", "b_h = 1"),
+    _esa(4, 4, 4, 3, "esa2", "one block"),
+    _esa(100, 60, 8, 0, "esa2", "search 0"),
+    _esa(37, 29, 4, 0, "esa2", "search 0, size not a multiple of mb"),
+    _esa(48, 48, 16, 32, "esa2", "search beyond the frame on all four sides"),
+    _esa(100, 70, 8, 12, "esa2", "linesize = width + 13, frame_stride odd, cur at base + 1, ref at base + 3: no word loads", nf=3,
+         linesize=_LS, frame_stride=_LS * 70 + 5, cur_off=1, ref_off=3),
+    _esa(100, 70, 16, 24, "esa2", "the same layout at mb 16", nf=3, linesize=_LS, frame_stride=_LS * 70 + 5, cur_off=1, ref_off=3),
+    _esa(100, 70, 4, 80, "esa", "the same layout through esa_kernel<4>", nf=3, linesize=_LS, frame_stride=_LS * 70 + 5, cur_off=1, ref_off=3),
+    _esa(101, 71, 16, 100, "esa", "the same layout through esa_kernel<16>", nf=2, linesize=_LS + 1, frame_stride=(_LS + 1) * 71 + 7,
+         cur_off=3, ref_off=1),
+    _esa(8, 8, 4, 4, "esa2", "65537 frames: the grid-z chunk loop, last chunk of two frames", nf=65537, linesize=9, frame_stride=75,
+         inputs=("random", "ties3")),
+    _esa(8, 8, 4, 75, "esa", "65537 frames through esa_kernel", nf=65537, linesize=9, frame_stride=75, inputs=("random", "ties3")),
+    _esa(3840, 2160, 16, 32, "esa2", "BASELINE config 4: 4K pairs, +-32", nf=3, inputs=("shifted", "ties8"), rows=(0, 67, 134)),
+    _esa(1920, 1080, 8, 16, "esa2", "1080p, mb 8", inputs=("shifted", "ties17"), rows=(0, 67, 134)),
+    _esa(1920, 1080, 4, 7, "esa2", "1080p, mb 4", inputs=("shifted", "ties3"), rows=(0, 135, 269)),
+]
+
+
+def esa_pictures(kind, nf, h, w, seed):
+    """(cur, ref): nf x h x w uint8 pictures of one input kind (see ESA_INPUTS_ALL)"""
+    rng = np.random.default_rng(seed)
+    yy, xx = np.mgrid[0:h, 0:w]
+    if kind == "random":
+        return rng.integers(0, 256, (nf, h, w), dtype=np.uint8), rng.integers(0, 256, (nf, h, w), dtype=np.uint8)
+    if kind == "shifted":                                        # a true vector exists, blurred by +-2 noise
+        cur = rng.integers(0, 256, (nf, h, w), dtype=np.uint8)
+        ref = np.stack([np.roll(cur[f], (int(rng.integers(-7, 8)), int(rng.integers(-7, 8))), (0, 1)) for f in range(nf)])
+        return cur, (ref.astype(np.int16) + rng.integers(-2, 3, ref.shape)).clip(0, 255).astype(np.uint8)
+    if kind == "flat":                                            # every candidate costs 2 * mb^2: the zero vector wins
+        return np.full((nf, h, w), 99, np.uint8), np.full((nf, h, w), 97, np.uint8)
+    if kind == "extremes":
+        chk = ((xx + yy) % 2 * 255).astype(np.uint8)
+        return np.broadcast_to(chk, (nf, h, w)).copy(), np.broadcast_to(255 - chk, (nf, h, w)).copy()
+    if kind == "saturated":
+        return np.full((nf, h, w), 255, np.uint8), np.zeros((nf, h, w), np.uint8)
+    p, (sy, sx), plus = {"ties3": (3, (1, 2), 0), "ties8": (8, (3, 5), 0), "ties17": (17, (5, 11), 0),
+                         "ties_zero_min": (5, (0, 0), 1), "ties_zero_0": (3, (0, 0), 0)}[kind]
+    t = rng.integers(0, 255, (nf, p, p), dtype=np.uint8)           # periodic tiles: exact minima at every vector of the shift's class
+    cur = t[:, yy % p, xx % p]
+    return cur, t[:, (yy - sy) % p, (xx - sx) % p] + np.uint8(plus)
+
+
+def esa_buffers(row, kind):
+    """(cur buffer, ref buffer, cur pictures, ref pictures): the row's layout (offset, linesize, frame_stride) with the pictures of one
+    input kind placed in it; padding bytes hold seeded noise, so a kernel that read them would change its result.  The seed depends on
+    the picture size and the kind only: the rows of a boundary group search the same pictures."""
+    w, h, ls, fs, nf = row["w"], row["h"], row["linesize"], row["frame_stride"], row["nf"]
+    seed = (w * 10000 + h) * 16 + ESA_INPUTS_ALL.index(kind)
+    cur, ref = esa_pictures(kind, nf, h, w, seed)
+    rng = np.random.default_rng(seed + 1)
+    bufs = []
+    for pics, off in ((cur, row["cur_off"]), (ref, row["ref_off"])):
+        b = rng.integers(0, 256, off + nf * fs + 64, dtype=np.uint8)
+        frames = np.lib.stride_tricks.as_strided(b[off:], (nf, h, w), (fs, ls, 1), writeable=True)
+        frames[...] = pics
+        bufs.append(b)
+    return bufs[0], bufs[1], cur, ref
+
+
+def esa_expected(lib_fn, row, curbuf, refbuf, workers=None):
+    """(mv [nf, blocks, 2] int32, cost [nf, blocks] uint64) of the CPU search `lib_fn` (orc_esa_frame / ffref_esa_frame) on the row's
+    buffers, frames and macroblock-row ranges spread over threads (the C calls release the GIL).  Rows the case does not check stay 0."""
+    import ctypes as C
+    import os
+    from concurrent.futures import ThreadPoolExecutor
+    w, h, ls, fs, nf, mb, sp = (row[k] for k in ("w", "h", "linesize", "frame_stride", "nf", "mb", "search"))
+    bw, bh = w // mb, h // mb
+    mv, cost = np.zeros((nf, bh * bw, 2), np.int32), np.zeros((nf, bh * bw), np.uint64)
+    spans = [(r, r + 1) for r in row["rows"]] if row["rows"] else [(r, min(r + 8, bh)) for r in range(0, bh, 8)]
+    u8p, i32p, u64p = C.POINTER(C.c_uint8), C.POINTER(C.c_int32), C.POINTER(C.c_uint64)
+    c0, r0 = curbuf.ctypes.data + row["cur_off"], refbuf.ctypes.data + row["ref_off"]
+
+    def run(task):
+        f0, f1, s = task
+        for f in range(f0, f1):
+            lib_fn(C.cast(c0 + f * fs, u8p), C.cast(r0 + f * fs, u8p), ls, w, h, mb, sp, s[0], s[1],
+                   C.cast(mv[f].ctypes.data, i32p), C.cast(cost[f].ctypes.data, u64p))
+    step = max(1, nf // 64)
+    tasks = [(f, min(f + step, nf), s) for f in range(0, nf, step) for s in spans]
+    with ThreadPoolExecutor(workers or os.cpu_count() or 1) as ex:
+        list(ex.map(run, tasks))
+    return mv, cost

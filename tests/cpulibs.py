@@ -56,6 +56,12 @@ def oracle():
         if hasattr(L, "orc_me_cmp"):
             L.orc_me_cmp.argtypes = [C.c_int, C.c_int, u8p, u8p, C.c_ssize_t, C.c_int]
             L.orc_esa_frame.argtypes = [u8p, u8p] + [C.c_int] * 7 + [i32p, u64p]
+            L.orc_esa_frame.restype = None
+            L.orc_me_cmp_set_nsse_weight.argtypes = [C.c_int]
+            L.orc_me_cmp_set_nsse_weight.restype = None
+            L.orc_me_cmp_batch.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_int, C.c_void_p, C.c_void_p,
+                                           C.c_int64, C.c_void_p]
+            L.orc_me_cmp_batch.restype = None
         if hasattr(L, "orc_h264qpel"):
             L.orc_h264qpel.argtypes = [C.c_int, C.c_int, C.c_int, u8p, u8p, C.c_ssize_t]
             L.orc_hpel.argtypes = [C.c_int, C.c_int, C.c_int, u8p, u8p, C.c_ssize_t, C.c_int]

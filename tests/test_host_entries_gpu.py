@@ -1,5 +1,6 @@
 """GPU tier: the pipelined HOST-buffer entry points (what bench.py's e2e legs time) against the oracle: b200_tx_batch_host,
-b200_h264qpel_frames_host, b200_me_esa_host.  Sizes are chosen so that a batch spans several chunks and every pipeline slot."""
+b200_h264qpel_frames_host, b200_me_esa_host.  The tx and qpel batches span several chunks and every pipeline slot; the 5 frames of
+the search fit in one chunk (several chunks and a reused slot: tests/test_me_search_gpu.py)."""
 import ctypes as C
 
 import numpy as np

@@ -32,35 +32,9 @@ def test_mecmp_pointer_table_golden(device):
         assert got == v, (fn, idx, h)
 
 
-def test_mecmp_batch_vs_oracle(device):
-    import torch
-    from ffmpeg_b200 import me_cmp
-    O = cl.oracle()
-    rng = np.random.default_rng(5)
-    W, H, n = 256, 128, 3000
-    f1 = rng.integers(0, 256, (H, W), dtype=np.uint8)
-    f2 = rng.integers(0, 256, (H, W), dtype=np.uint8)
-    xs1, ys1, xs2, ys2 = (rng.integers(0, d - 20, n) for d in (W, H, W, H))
-    off1 = (ys1 * W + xs1).astype(np.int64)
-    off2 = (ys2 * W + xs2).astype(np.int64)
-    with on_stream(device):
-        d1, d2 = torch.from_numpy(f1).cuda(), torch.from_numpy(f2).cuda()
-        o1, o2 = torch.from_numpy(off1).cuda(), torch.from_numpy(off2).cuda()
-        out = torch.zeros(n, dtype=torch.int32, device="cuda")
-        for fn, idxs in ((0, (0, 1)), (1, (0, 1, 2)), (2, range(8))):
-            for idx in idxs:
-                for h in (4, 8, 16):
-                    me_cmp.me_cmp_batch_device(device, fn, idx, d1, d2, W, h, o1, o2, n, out)
-                    device.sync()
-                    got = out.cpu().numpy()
-                    exp = np.array([O.orc_me_cmp(fn, idx, C.cast(f1.ctypes.data + int(a), cl.u8p), C.cast(f2.ctypes.data + int(b), cl.u8p), W, h)
-                                    for a, b in zip(off1[:400], off2[:400])])
-                    assert np.array_equal(got[:400], exp), (fn, idx, h)
-
-
 def test_mecmp_round2_families(device):
     """vsad / vsse (+ intra), nsse, median_sad, hadamard8_intra, sum_abs_dctelem: drop-in entries against the reference fixture
-    (NULL context like checkasm), batched entry against the oracle."""
+    (NULL context like checkasm), batched sum_abs_dctelem against it too (the batched compare entry: tests/test_me_search_gpu.py)."""
     import torch
     from ffmpeg_b200 import me_cmp
     from ffmpeg_b200._lib import u8p, i16p
@@ -75,27 +49,7 @@ def test_mecmp_round2_families(device):
         assert got == v, (fn, idx, h)
     for b, v in zip(g["blocks"][:8], g["sums"][:8]):
         assert c.sum_abs_dctelem(np.ascontiguousarray(b).ctypes.data_as(i16p)) == v
-    O = cl.oracle()
-    rng = np.random.default_rng(6)
-    W, H, n = 256, 128, 2000
-    f1 = rng.integers(0, 256, (H, W), dtype=np.uint8)
-    f2 = (f1.astype(int) + rng.integers(-9, 10, f1.shape)).clip(0, 255).astype(np.uint8)
-    xs1, ys1, xs2, ys2 = (rng.integers(1, d - 20, n) for d in (W, H, W, H))
-    off1 = (ys1 * W + xs1).astype(np.int64)
-    off2 = (ys2 * W + xs2).astype(np.int64)
     with on_stream(device):
-        d1, d2 = torch.from_numpy(f1).cuda(), torch.from_numpy(f2).cuda()
-        o1, o2 = torch.from_numpy(off1).cuda(), torch.from_numpy(off2).cuda()
-        out = torch.zeros(n, dtype=torch.int32, device="cuda")
-        for fn, idxs in ((3, (4, 5)), (4, (0, 1, 4, 5)), (5, (0, 1, 4, 5)), (6, (0, 1)), (7, (0, 1))):
-            for idx in idxs:
-                for h in (8, 16):
-                    me_cmp.me_cmp_batch_device(device, fn, idx, d1, d2, W, h, o1, o2, n, out)
-                    device.sync()
-                    got = out.cpu().numpy()
-                    exp = np.array([O.orc_me_cmp(fn, idx, C.cast(f1.ctypes.data + int(a), cl.u8p), C.cast(f2.ctypes.data + int(b), cl.u8p), W, h)
-                                    for a, b in zip(off1[:300], off2[:300])])
-                    assert np.array_equal(got[:300], exp), (fn, idx, h)
         blocks = torch.from_numpy(g["blocks"]).cuda()
         so = torch.zeros(blocks.shape[0], dtype=torch.int32, device="cuda")
         me_cmp.sum_abs_dctelem_batch_device(device, blocks, blocks.shape[0], so)
@@ -104,8 +58,7 @@ def test_mecmp_round2_families(device):
 
 
 def test_satd_pointer_table_and_batch(device):
-    """hadamard8_diff (SATD): drop-in entries against the reference fixture, batched entry against the oracle."""
-    import torch
+    """hadamard8_diff (SATD): drop-in entries against the reference fixture (the batched entry: tests/test_me_search_gpu.py)."""
     from ffmpeg_b200 import me_cmp
     from ffmpeg_b200._lib import u8p
     g, cases = np.load(os.path.join(G, "mecmp.npz")), np.load(os.path.join(G, "satd.npz"))["cases"]
@@ -114,25 +67,6 @@ def test_satd_pointer_table_and_batch(device):
     for fn, idx, x1, y1, x2, y2, h, v in cases[::3]:
         got = c.hadamard8_diff[idx](None, C.cast(img1.ctypes.data + int(y1) * 64 + int(x1), u8p), C.cast(img2.ctypes.data + int(y2) * 64 + int(x2), u8p), 64, int(h))
         assert got == v, (idx, h)
-    O = cl.oracle()
-    rng = np.random.default_rng(6)
-    W, H, n = 256, 128, 2000
-    f1 = rng.integers(0, 256, (H, W), dtype=np.uint8)
-    f2 = np.clip(f1.astype(np.int32) + rng.integers(-20, 21, (H, W)), 0, 255).astype(np.uint8)
-    off1 = (rng.integers(0, H - 20, n) * W + rng.integers(0, W - 20, n)).astype(np.int64)
-    off2 = (rng.integers(0, H - 20, n) * W + rng.integers(0, W - 20, n)).astype(np.int64)
-    with on_stream(device):
-        d1, d2 = torch.from_numpy(f1).cuda(), torch.from_numpy(f2).cuda()
-        o1, o2 = torch.from_numpy(off1).cuda(), torch.from_numpy(off2).cuda()
-        out = torch.zeros(n, dtype=torch.int32, device="cuda")
-        for idx in (0, 1):
-            for h in (8, 16):
-                me_cmp.me_cmp_batch_device(device, me_cmp.HADAMARD8, idx, d1, d2, W, h, o1, o2, n, out)
-                device.sync()
-                got = out.cpu().numpy()
-                exp = np.array([O.orc_me_cmp(3, idx, C.cast(f1.ctypes.data + int(a), cl.u8p), C.cast(f2.ctypes.data + int(b), cl.u8p), W, h)
-                                for a, b in zip(off1[:500], off2[:500])])
-                assert np.array_equal(got[:500], exp), (idx, h)
 
 
 def gpu_esa(device, cur, ref_, mb, sp):
@@ -162,9 +96,8 @@ def test_esa_golden(device):
 
 
 def test_esa_vs_oracle_multi_frame(device):
-    """720p-sized frame pairs, +-32 window (BASELINE config 4 geometry at a size the oracle finishes in seconds is too
-    slow; use 320x192 for the oracle and check 4K through the minimum-cost property).  A +-66 window on a small frame takes the
-    first kernel: the second one's window copies no longer fit in shared memory there."""
+    """Two 320x192 frame pairs at +-32, and a +-66 window on a small frame, which takes the first kernel: the second one's window
+    copies no longer fit in shared memory there (the full case matrix, 4K included: tests/test_me_search_gpu.py)."""
     O = cl.oracle()
     rng = np.random.default_rng(9)
     for nf, W, H, mb, sp in ((2, 320, 192, 16, 32), (1, 176, 112, 16, 66)):
@@ -177,27 +110,6 @@ def test_esa_vs_oracle_multi_frame(device):
             emv, ec = np.zeros((bh * bw, 2), np.int32), np.zeros(bh * bw, np.uint64)
             O.orc_esa_frame(cl.ptr(cur[i]), cl.ptr(ref_[i]), W, W, H, mb, sp, 0, bh, cl.ptr(emv, cl.i32p), cl.ptr(ec, cl.u64p))
             assert np.array_equal(mv[i], emv) and np.array_equal(cost[i], ec), (sp, i)
-
-
-def test_esa_4k_property(device):
-    """Full-size 4K pair: the returned cost must equal the SAD at the returned vector and be <= the zero-vector SAD and
-    the SAD at a few probe vectors (size-independent property; the oracle would need minutes here)."""
-    rng = np.random.default_rng(10)
-    W, H, mb, sp = 3840, 2160, 16, 32
-    cur = rng.integers(0, 256, (1, H, W), dtype=np.uint8)
-    ref_ = np.roll(cur, (0, 11, -6), (0, 1, 2)).copy()
-    mv, cost = gpu_esa(device, cur, ref_, mb, sp)
-    bw = W // mb
-    for b in rng.integers(0, mv.shape[1], 200):
-        by, bx = divmod(int(b), bw)
-        x_mb, y_mb = bx * mb, by * mb
-        blk = cur[0, y_mb:y_mb + mb, x_mb:x_mb + mb].astype(np.int32)
-        x, y = mv[0, b]
-        sad = lambda xx, yy: int(np.abs(ref_[0, yy:yy + mb, xx:xx + mb].astype(np.int32) - blk).sum())
-        assert sad(x, y) == int(cost[0, b])
-        assert int(cost[0, b]) <= sad(x_mb, y_mb)
-        if 32 <= y_mb <= H - 48 and 32 <= x_mb <= W - 48:
-            assert int(cost[0, b]) == 0 and (x, y) == (x_mb - 6, y_mb + 11)        # the true shift is found exactly
 
 
 # ---------------------------------------------------------------------------------------------- qpel / hpel

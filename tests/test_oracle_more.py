@@ -1173,3 +1173,56 @@ def test_fdct_oracle_vs_fixture_and_reference():
                     e = x[i].copy()
                     O.orc_fdct(kind, is248, cl.ptr(e, cl.i16p))
                     assert rc.same(e, lambda: ref_fdct(algo, bits, is248, x[i].copy())), (algo, bits, is248, i)
+
+
+def test_esa_kernel_mirror_boundaries():
+    """cases.esa_kernel_for (the restatement of launch_esa's kernel choice) has its boundaries where the header says, and every row of
+    ESA_CASES expects what it predicts."""
+    from cases import B200_ENOSYS, ESA_CASES, esa_kernel_for
+    for mb, last2, last in ((16, 64, 216), (8, 70, 220), (4, 74, 222)):
+        kinds = [esa_kernel_for(mb, s) for s in range(0, 400)]
+        assert kinds == ["esa2"] * (last2 + 1) + ["esa"] * (last - last2) + [B200_ENOSYS] * (400 - last - 1), mb
+    for row in ESA_CASES:
+        assert esa_kernel_for(row["mb"], row["search"]) == row["expect"], row["note"]
+
+
+def test_esa_cases_oracle_vs_reference():
+    """orc_esa_frame against the reference's ff_me_search_esa (driven like vf_mestimate) on every row and input of ESA_CASES that has a
+    kernel, in the row's layout; the 4K and 1080p rows on the macroblock rows the GPU test checks."""
+    from cases import B200_ENOSYS, ESA_CASES, esa_buffers, esa_expected
+    O = cl.oracle()
+    R = cl.ref() if cl.have_ref() else None
+    with cl.RefCheck() as rc:
+        for row in ESA_CASES:
+            if row["expect"] == B200_ENOSYS:
+                continue
+            for kind in row["inputs"]:
+                cb, rb, _, _ = esa_buffers(row, kind)
+                ours = list(esa_expected(O.orc_esa_frame, row, cb, rb))
+                assert rc.same(ours, lambda: list(esa_expected(R.ffref_esa_frame, row, cb, rb))), (row["note"], kind)
+
+
+def test_nsse_weight_oracle():
+    """nsse with a weight: at 8 (the NULL-context weight) against the reference; at any weight w the score is
+    sse + w * |noise|, so result(w) = result(0) + w * (result(1) - result(0))."""
+    O = cl.oracle()
+    R = cl.ref() if cl.have_ref() else None
+    rng = np.random.default_rng(41)
+    a = rng.integers(0, 256, (48, 96), dtype=np.uint8)
+    b = (a.astype(int) + rng.integers(-4, 5, a.shape)).clip(0, 255).astype(np.uint8)
+    c = rng.integers(0, 256, (48, 96), dtype=np.uint8)
+    cases = [(p, q, idx, h) for p, q in ((a, b), (a, c), (c, b)) for idx in (0, 1) for h in (1, 2, 7, 8, 16) + ((32,) if idx else ())]
+    ptrs = lambda p, q: (C.cast(p.ctypes.data + 96 * 3 + 5, cl.u8p), C.cast(q.ctypes.data + 96 * 2 + 9, cl.u8p))  # noqa: E731
+    try:
+        res = {}
+        for w in (0, 1, 8, 37, -5):
+            O.orc_me_cmp_set_nsse_weight(w)
+            res[w] = [O.orc_me_cmp(6, idx, *ptrs(p, q), 96, h) for p, q, idx, h in cases]
+        assert any(r1 != r0 for r0, r1 in zip(res[0], res[1]))
+        for w in (8, 37, -5):
+            assert res[w] == [r0 + w * (r1 - r0) for r0, r1 in zip(res[0], res[1])], w
+        with cl.RefCheck() as rc:
+            for (p, q, idx, h), v in zip(cases, res[8]):
+                assert rc.same(v, lambda: R.ffref_me_cmp(6, idx, *ptrs(p, q), 96, h)), (idx, h)
+    finally:
+        O.orc_me_cmp_set_nsse_weight(8)

@@ -164,6 +164,12 @@ class HevcMcOp(C.Structure):
                 ("wx1", C.c_int32), ("ox", C.c_int32), ("reserved", C.c_uint8 * 4)]
 
 
+class HevcTuOp(C.Structure):
+    """B200HevcTuOp (include/b200dsp.h), 32 bytes"""
+    _fields_ = [("dst_off", C.c_int64), ("coef_off", C.c_int64), ("log2_size", C.c_uint8), ("kind", C.c_uint8), ("flags", C.c_uint8),
+                ("reserved0", C.c_uint8), ("col_limit", C.c_int32), ("reserved", C.c_uint8 * 8)]
+
+
 class ProresDSPContext(C.Structure):
     """libavcodec/proresdsp.h:28-35"""
     _fields_ = [("idct_permutation_type", C.c_int), ("idct_permutation", C.c_uint8 * 64),
@@ -274,6 +280,8 @@ PROTOTYPES = {
     "b200_h264_pred_add_batch_device": (C.c_int, [vp, C.c_int, C.c_int64, vp, vp, vp, vp, C.c_ssize_t, vp, vp]),
     "b200_hevc_dsp_init": (C.c_int, [vp, C.c_int]),
     "b200_hevc_mc_batch_device": (C.c_int, [vp, C.c_int, C.c_int, C.c_int64, vp, vp, C.c_ssize_t, vp, C.c_ssize_t, C.c_int, C.c_int]),
+    "b200_hevc_dsp_init_transform": (C.c_int, [vp, C.c_int]),
+    "b200_hevc_transform_add_batch_device": (C.c_int, [vp, C.c_int, C.c_int64, vp, vp, vp, C.c_ssize_t]),
     "b200_proresdsp_init": (C.c_int, [vp, C.c_int]),
     "b200_prores_idct_put_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, vp, vp, vp, C.c_int]),
     "b200_float_dsp_init": (C.c_int, [vp]),

@@ -1,0 +1,462 @@
+// hevcidct.cu — HEVC residual reconstruction on sm_90a: the transform members of HEVCDSPContext (libavcodec/hevc/dsp.h:47-125:
+// add_residual[4], dequant, transform_rdpcm, transform_4x4_luma, idct[4], idct_dc[4]) as ff_hevc_dsp_init fills them for 8, 9, 10 and
+// 12 bit samples (hevc/dsp.c:198-215), and a batched device entry that runs the decoder's per-transform-unit sequence
+// (hevc/cabac.c:1550-1592) followed by add_residual.
+//
+// Reference semantics reproduced bit for bit (checker: oracle/hevcidct_oracle.c), hevc/dsp_template.c:46-309:
+//   idct N x N:  column pass then row pass, each clip16((sum + add) >> shift), shifts 7 and 20 - depth.  col_limit masks the odd inputs
+//                of the partial butterflies: column c of the first pass sums odd rows j < L(c), L(0) = L0 = min(col_limit + 4, N),
+//                L(c >= 1) = L0 - 4 ((c - 1) / 4) while below N (the reference's running limit2); every row of the second pass sums odd
+//                columns j < min(col_limit, N); at 32 points the inner 16-point butterfly gets end / 2, which also masks j = 2 (mod 4)
+//                by j / 2 < end / 2.  The 4x4 ignores col_limit.  Exact int32 sums, so the partial butterfly of the inputs with those
+//                terms zeroed is the reference's result.
+//   idct_dc:     every coefficient = (((c0 + 1) >> 1) + add) >> (14 - depth)
+//   4x4 luma:    the DST butterfly TR_4x4_LUMA with the idct's shifts and clips
+//   dequant:     (c + 2^(s - 1)) >> s, s = 15 - depth - log2; nothing for s == 0; (int16)((uint16)c << -s) for s < 0 (12 bit)
+//   rdpcm:       running sums along rows (mode 0) or down columns (mode != 0), int16 wrap at every step
+//   add:         dst = clip(dst + res, 0, 2^depth - 1)
+//
+// Kernel: a CTA of 256 threads takes a run of 1-256 ops (chosen from the batch size) and walks it in rounds of at most kCap
+// coefficients.  A round loads its ops' coefficients into shared memory as 16-byte vectors, then runs two line passes over all its
+// ops at once: pass 1 gives every thread one column of one op (the whole column transform in registers, clipped into a second shared
+// array whose rows are padded to an odd number of words), pass 2 one row of one op (the row transform in registers, fused with the
+// add, the clip and a store of whole 4-sample words of the destination).  A 32x32 TU is thus 32 threads' work per pass, a 4x4 TU four
+// threads', and a run of small TUs fills the CTA as well as a few large ones do.  Nothing goes to global memory between the passes.
+#include "common.h"
+#include <cstring>
+
+namespace {
+
+constexpr int kThreads = 256;
+constexpr int kMaxOps = 256;                                 // ops per CTA
+constexpr int kCap = 8192;                                   // coefficients per round
+constexpr int kBCap = kCap + kCap / 2;                       // pass-1 array: N x (N + 2) per op, at most 1.5 N^2 (N = 4)
+constexpr int kHead = 2 * (kMaxOps + 1) + 2 * kMaxOps + 2;  // ints in front of the coefficients (a multiple of 4: 16-byte aligned)
+constexpr size_t kSmem = 4 * kHead + 2 * (kCap + kBCap);
+enum { K_IDCT = B200_HEVC_TU_IDCT, K_DC = B200_HEVC_TU_IDCT_DC, K_DST4 = B200_HEVC_TU_DST4, K_SKIP = B200_HEVC_TU_SKIP,
+       K_BYPASS = B200_HEVC_TU_BYPASS };
+
+// The 32-point HEVC transform matrix (H.265 8.6.4.2): row k, column n is c(k (2n + 1) mod 128) with c(m) the scaled cos(pi m / 64)
+// of the standard's coefficient list, by the cosine's symmetries; row 0 is 64.
+struct Mat32 { int8_t v[32][32]; };
+constexpr int cosv(int m)
+{
+    constexpr int c[33] = { 64, 90, 90, 90, 89, 88, 87, 85, 83, 82, 80, 78, 75, 73, 70, 67, 64, 61, 57, 54, 50, 46, 43, 38, 36, 31, 25, 22,
+                            18, 13, 9, 4, 0 };
+    return m <= 32 ? c[m] : m <= 64 ? -c[64 - m] : m <= 96 ? -c[m - 64] : c[128 - m];
+}
+constexpr Mat32 make_t32()
+{
+    Mat32 t{};
+    for (int k = 0; k < 32; k++)
+        for (int n = 0; n < 32; n++) t.v[k][n] = (int8_t)(k ? cosv((k * (2 * n + 1)) & 127) : 64);
+    return t;
+}
+__constant__ Mat32 c_t32 = make_t32();
+
+struct TuArgs {
+    const B200HevcTuOp *ops;
+    long long nops;
+    const int16_t *coef;
+    uint8_t *dst;
+    long long dst_stride;
+    int16_t *res;                        // drop-in members: the int16 result goes here (at coef_off, N x N row-major) instead of dst
+    int depth, ops_per_cta;
+};
+
+// partial butterfly of N points, inputs x[k S], k < N (the reference's TR_4 .. TR_32 with every input taken)
+template <int N, int S>
+__device__ __forceinline__ void idct1d(const int *x, int *y)
+{
+    if constexpr (N == 4) {
+        const int e0 = 64 * x[0] + 64 * x[2 * S], e1 = 64 * x[0] - 64 * x[2 * S];
+        const int o0 = 83 * x[S] + 36 * x[3 * S], o1 = 36 * x[S] - 83 * x[3 * S];
+        y[0] = e0 + o0;
+        y[1] = e1 + o1;
+        y[2] = e1 - o1;
+        y[3] = e0 - o0;
+    } else {
+        int e[N / 2];
+        idct1d<N / 2, 2 * S>(x, e);
+#pragma unroll
+        for (int i = 0; i < N / 2; i++) {
+            int o = 0;
+#pragma unroll
+            for (int j = 1; j < N; j += 2) o += c_t32.v[j * (32 / N)][i] * x[j * S];
+            y[i] = e[i] + o;
+            y[N - 1 - i] = e[i] - o;
+        }
+    }
+}
+
+// the DST of transform_4x4_luma (TR_4x4_LUMA)
+__device__ __forceinline__ void dst4(const int *s, int *d)
+{
+    const int c0 = s[0] + s[2], c1 = s[2] + s[3], c2 = s[0] - s[3], c3 = 74 * s[1];
+    d[2] = 74 * (s[0] - s[2] + s[3]);
+    d[0] = 29 * c0 + 55 * c1 + c3;
+    d[1] = 55 * c2 - 29 * c1 + c3;
+    d[3] = 55 * c0 + 29 * c2 - c3;
+}
+
+__device__ __forceinline__ int clip16(int v) { return v < -32768 ? -32768 : v > 32767 ? 32767 : v; }
+
+// input j of an N-point butterfly that the reference sums with end E (odd j < E; j = 2 mod 4 at 32 points by j / 2 < E / 2)
+template <int N>
+__device__ __forceinline__ bool kept(int j, int E)
+{
+    if (N == 4 || (j & 1) == 0 && (N != 32 || (j & 3) == 0)) return true;
+    return (j & 1) ? j < E : (j >> 1) < (E >> 1);
+}
+
+// first-pass limit of column c: limit2 as the reference's loop leaves it (int arithmetic wrapping like the compiled reference's)
+template <int N>
+__device__ __forceinline__ int col_end(int col_limit, int c)
+{
+    const int l0 = (int)((unsigned)col_limit + 4u);
+    int l = l0 < N ? l0 : N;
+    for (int i = 4; i < c; i += 4)
+        if (l < N) l = (int)((unsigned)l - 4u);
+    return l;
+}
+
+template <int N>
+__device__ __forceinline__ void pass1(const B200HevcTuOp &op, int kind, int c, const int16_t *A, int16_t *B, int depth)
+{
+    if (kind == K_DC) return;
+    int x[N], y[N];
+#pragma unroll
+    for (int j = 0; j < N; j++) x[j] = A[j * N + c];
+    if (kind == K_IDCT || kind == K_DST4) {
+        if (kind == K_DST4) {
+            dst4(x, y);
+        } else {
+            const int E = col_end<N>(op.col_limit, c);
+#pragma unroll
+            for (int j = 0; j < N; j++) x[j] = kept<N>(j, E) ? x[j] : 0;
+            idct1d<N, 1>(x, y);
+        }
+#pragma unroll
+        for (int j = 0; j < N; j++) B[j * (N + 2) + c] = (int16_t)clip16((y[j] + 64) >> 7);
+        return;
+    }
+    if (kind == K_SKIP) {
+        if (N == 4 && (op.flags & B200_HEVC_TU_ROTATE)) {
+#pragma unroll
+            for (int j = 0; j < N; j++) x[j] = A[15 - (j * N + c)];
+        }
+        const int s = 15 - depth - (N == 4 ? 2 : N == 8 ? 3 : N == 16 ? 4 : 5);
+        if (s > 0) {
+#pragma unroll
+            for (int j = 0; j < N; j++) x[j] = (int16_t)((x[j] + (1 << (s - 1))) >> s);
+        } else if (s < 0) {
+#pragma unroll
+            for (int j = 0; j < N; j++) x[j] = (int16_t)(uint16_t)((unsigned)(uint16_t)x[j] << -s);
+        }
+    }
+    if ((op.flags & (B200_HEVC_TU_RDPCM | B200_HEVC_TU_RDPCM_VER)) == (B200_HEVC_TU_RDPCM | B200_HEVC_TU_RDPCM_VER)) {
+#pragma unroll
+        for (int j = 1; j < N; j++) x[j] = (int16_t)(x[j] + x[j - 1]);
+    }
+#pragma unroll
+    for (int j = 0; j < N; j++) B[j * (N + 2) + c] = (int16_t)x[j];
+}
+
+// one destination word of 4 samples: load, add, clip, store
+template <typename P>
+__device__ __forceinline__ void add4(P *d, const int *r, int maxv)
+{
+    if constexpr (sizeof(P) == 1) {
+        const unsigned w = *reinterpret_cast<const unsigned *>(d);
+        unsigned o = 0;
+#pragma unroll
+        for (int k = 0; k < 4; k++) o |= (unsigned)min(max((int)((w >> (8 * k)) & 0xFF) + r[k], 0), maxv) << (8 * k);
+        *reinterpret_cast<unsigned *>(d) = o;
+    } else {
+        const uint2 w = *reinterpret_cast<const uint2 *>(d);
+        const int s0 = w.x & 0xFFFF, s1 = w.x >> 16, s2 = w.y & 0xFFFF, s3 = w.y >> 16;
+        uint2 o;
+        o.x = (unsigned)min(max(s0 + r[0], 0), maxv) | (unsigned)min(max(s1 + r[1], 0), maxv) << 16;
+        o.y = (unsigned)min(max(s2 + r[2], 0), maxv) | (unsigned)min(max(s3 + r[3], 0), maxv) << 16;
+        *reinterpret_cast<uint2 *>(d) = o;
+    }
+}
+
+template <typename P, int N>
+__device__ __forceinline__ void pass2(const B200HevcTuOp &op, int kind, int r, const int16_t *A, const int16_t *B, const TuArgs &a)
+{
+    int x[N], y[N];
+    if (kind == K_DC) {
+        const int v = (((A[0] + 1) >> 1) + (1 << (13 - a.depth))) >> (14 - a.depth);
+#pragma unroll
+        for (int j = 0; j < N; j++) y[j] = v;
+    } else {
+#pragma unroll
+        for (int j = 0; j < N; j++) x[j] = B[r * (N + 2) + j];
+        const int sh = 20 - a.depth, add = 1 << (sh - 1);
+        if (kind == K_IDCT || kind == K_DST4) {
+            if (kind == K_DST4) {
+                dst4(x, y);
+            } else {
+                const int E = op.col_limit < N ? op.col_limit : N;
+#pragma unroll
+                for (int j = 0; j < N; j++) x[j] = kept<N>(j, E) ? x[j] : 0;
+                idct1d<N, 1>(x, y);
+            }
+#pragma unroll
+            for (int j = 0; j < N; j++) y[j] = clip16((y[j] + add) >> sh);
+        } else {
+            if ((op.flags & (B200_HEVC_TU_RDPCM | B200_HEVC_TU_RDPCM_VER)) == B200_HEVC_TU_RDPCM) {
+#pragma unroll
+                for (int j = 1; j < N; j++) x[j] = (int16_t)(x[j] + x[j - 1]);
+            }
+#pragma unroll
+            for (int j = 0; j < N; j++) y[j] = x[j];
+        }
+    }
+    if (a.res) {
+        int16_t *o = a.res + op.coef_off + r * N;
+#pragma unroll
+        for (int j = 0; j < N; j += 4)
+            *reinterpret_cast<uint2 *>(o + j) = make_uint2((unsigned)(uint16_t)y[j] | (unsigned)y[j + 1] << 16,
+                                                          (unsigned)(uint16_t)y[j + 2] | (unsigned)y[j + 3] << 16);
+        return;
+    }
+    P *d = reinterpret_cast<P *>(a.dst + op.dst_off + (long long)r * a.dst_stride);
+    const int maxv = (1 << a.depth) - 1;
+#pragma unroll
+    for (int j = 0; j < N; j += 4) add4<P>(d + j, y + j, maxv);
+}
+
+// the device-side guard: an op it refuses writes nothing
+template <typename P>
+__device__ __forceinline__ bool op_ok(const B200HevcTuOp &op, bool res_mode)
+{
+    if (op.log2_size < 2 || op.log2_size > 5 || op.kind > K_BYPASS || (op.kind == K_DST4 && op.log2_size != 2)) return false;
+    if (op.coef_off & 7) return false;
+    return res_mode || (op.dst_off & (4 * sizeof(P) - 1)) == 0;
+}
+
+// largest i in [lo, hi) with v[i] <= x (v non-decreasing, v[lo] <= x)
+__device__ __forceinline__ int find(const int *v, int lo, int hi, int x)
+{
+    while (hi - lo > 1) {
+        const int m = (lo + hi) >> 1;
+        if (v[m] <= x) lo = m;
+        else hi = m;
+    }
+    return lo;
+}
+
+template <typename P>
+__global__ void __launch_bounds__(kThreads) hevc_tu_kernel(TuArgs a)
+{
+    extern __shared__ int4 hevc_tu_smem[];
+    int *S = reinterpret_cast<int *>(hevc_tu_smem);          // [i] = first coefficient of op i in the CTA's run, [n] = total
+    int *L = S + kMaxOps + 1;                                // [i] = first line of op i
+    int *meta = L + kMaxOps + 1;                             // log2 | kind << 8, -1 for a refused op
+    int *boff = meta + kMaxOps;                              // first element of op i in Bs, relative to its round
+    int16_t *As = reinterpret_cast<int16_t *>(S + kHead), *Bs = As + kCap;
+    const int tid = threadIdx.x;
+    const long long o0 = (long long)blockIdx.x * a.ops_per_cta;
+    const int n = (int)(a.nops - o0 < a.ops_per_cta ? a.nops - o0 : a.ops_per_cta);
+    const B200HevcTuOp *ops = a.ops + o0;
+    if (tid < n) {
+        const B200HevcTuOp &op = ops[tid];
+        const bool ok = op_ok<P>(op, a.res != nullptr);
+        meta[tid] = ok ? op.log2_size | op.kind << 8 : -1;
+        S[tid + 1] = ok ? 1 << (2 * op.log2_size) : 0;
+        L[tid + 1] = ok ? 1 << op.log2_size : 0;
+    }
+    if (tid == 0) S[0] = L[0] = 0;
+    __syncthreads();
+    for (int d = 1; d < n; d <<= 1) {                        // inclusive scan of S[1..n], L[1..n]
+        int s = 0, l = 0;
+        if (tid < n && tid >= d) s = S[tid + 1 - d], l = L[tid + 1 - d];
+        __syncthreads();
+        if (tid < n && tid >= d) S[tid + 1] += s, L[tid + 1] += l;
+        __syncthreads();
+    }
+    for (int r0 = 0; r0 < n;) {
+        const int r1 = find(S, r0, n + 1, S[r0] + kCap);    // ops r0 .. r1 - 1 fit in a round (r1 > r0: an op is at most 1024)
+        const int sa = S[r0], la = L[r0];
+        for (int i = r0 + tid; i < r1; i += kThreads) boff[i] = S[i] - sa + 2 * (L[i] - la);
+        const int nv = (S[r1] - sa) >> 3;
+        for (int v = tid; v < nv; v += kThreads) {
+            const int s = sa + 8 * v, i = find(S, r0, r1, s);
+            const int4 q = *reinterpret_cast<const int4 *>(a.coef + ops[i].coef_off + (s - S[i]));
+            *reinterpret_cast<int4 *>(As + (s - sa)) = q;
+        }
+        __syncthreads();
+        const int nl = L[r1] - la;
+        for (int t = tid; t < nl; t += kThreads) {
+            const int i = find(L, r0, r1, la + t), m = meta[i], c = la + t - L[i];
+            const int16_t *A = As + (S[i] - sa);
+            int16_t *B = Bs + boff[i];
+            switch (m & 0xFF) {
+            case 2:  pass1<4>(ops[i], m >> 8, c, A, B, a.depth); break;
+            case 3:  pass1<8>(ops[i], m >> 8, c, A, B, a.depth); break;
+            case 4:  pass1<16>(ops[i], m >> 8, c, A, B, a.depth); break;
+            default: pass1<32>(ops[i], m >> 8, c, A, B, a.depth); break;
+            }
+        }
+        __syncthreads();
+        for (int t = tid; t < nl; t += kThreads) {
+            const int i = find(L, r0, r1, la + t), m = meta[i], r = la + t - L[i];
+            const int16_t *A = As + (S[i] - sa), *B = Bs + boff[i];
+            switch (m & 0xFF) {
+            case 2:  pass2<P, 4>(ops[i], m >> 8, r, A, B, a); break;
+            case 3:  pass2<P, 8>(ops[i], m >> 8, r, A, B, a); break;
+            case 4:  pass2<P, 16>(ops[i], m >> 8, r, A, B, a); break;
+            default: pass2<P, 32>(ops[i], m >> 8, r, A, B, a); break;
+            }
+        }
+        __syncthreads();
+        r0 = r1;
+    }
+}
+
+constexpr long long kChunkOps = 1LL << 20;                   // ops per launch
+
+bool depth_ok(int d) { return d == 8 || d == 9 || d == 10 || d == 12; }
+
+cudaError_t launch(TuArgs a, cudaStream_t st)
+{
+    const long long nops = a.nops;
+    const long long per = (nops + 1055) / 1056;             // about 8 CTAs per SM for a frame; 1 op per CTA for a few ops
+    a.ops_per_cta = (int)(per < 1 ? 1 : per > kMaxOps ? kMaxOps : per);
+    const B200HevcTuOp *ops = a.ops;
+    for (long long b = 0; b < nops; b += kChunkOps) {
+        a.ops = ops + b;
+        a.nops = nops - b < kChunkOps ? nops - b : kChunkOps;
+        const unsigned grid = (unsigned)((a.nops + a.ops_per_cta - 1) / a.ops_per_cta);
+        if (a.depth == 8) hevc_tu_kernel<uint8_t><<<grid, kThreads, kSmem, st>>>(a);
+        else hevc_tu_kernel<uint16_t><<<grid, kThreads, kSmem, st>>>(a);
+        B200_LAUNCHED();
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
+}
+
+void die(const char *what)
+{
+    fprintf(stderr, "libb200dsp: hevc transform failed: %s (%s)\n", what, b200_last_error());
+    abort();
+}
+
+// ---- drop-in members (host pointers): one op through the device scratch.  res != nullptr: the members that work in place on the
+// coefficients (the kernel's int16 result is copied back over them); else add_residual (the block of dst is staged and copied back).
+void member_host(int depth, int log2, int kind, int flags, int col_limit, int16_t *coeffs, const int16_t *res, uint8_t *dst, ptrdiff_t stride)
+{
+    const int N = 1 << log2, bps = depth > 8 ? 2 : 1;
+    const size_t cbytes = (size_t)N * N * sizeof(int16_t), dpitch = (size_t)N * bps;
+    B200Device *dev = b200_default_device();
+    if (!dev) die("no device");
+    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
+    B200_LOCK_DEVICE(dev);            // scratch + stream are per device: one host-pointer call at a time (released on return)
+    uint8_t *scr = (uint8_t *)b200_scratch(dev, 256 + 3 * 2048);
+    if (!scr) die("scratch");
+    cudaStream_t st = dev->stream;
+    uint8_t *dop = scr, *dcoef = scr + 256, *dres = dcoef + 2048, *ddst = dres + 2048;
+    B200HevcTuOp op;
+    memset(&op, 0, sizeof(op));
+    op.log2_size = (uint8_t)log2;
+    op.kind = (uint8_t)kind;
+    op.flags = (uint8_t)flags;
+    op.col_limit = col_limit;
+    if (cudaMemcpyAsync(dop, &op, sizeof(op), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d op");
+    if (cudaMemcpyAsync(dcoef, coeffs ? coeffs : res, cbytes, cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d coefficients");
+    if (!coeffs && b200_h2d_rows(ddst, dpitch, dst, stride, dpitch, (size_t)N, st) != cudaSuccess) die("h2d block");
+    TuArgs a = { (const B200HevcTuOp *)dop, 1, (const int16_t *)dcoef, ddst, (long long)dpitch, coeffs ? (int16_t *)dres : nullptr, depth, 1 };
+    if (launch(a, st) != cudaSuccess) die("launch");
+    if (coeffs) {
+        if (cudaMemcpyAsync(coeffs, dres, cbytes, cudaMemcpyDeviceToHost, st) != cudaSuccess) die("d2h coefficients");
+    } else if (b200_d2h_rows(dst, stride, ddst, dpitch, dpitch, (size_t)N, st) != cudaSuccess) {
+        die("d2h block");
+    }
+    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+}
+
+bool log2_ok(int log2, const char *who)
+{
+    if (log2 >= 2 && log2 <= 5) return true;
+    b200_set_error("hevc %s: log2_size %d outside 2..5, nothing written", who, log2);
+    return false;
+}
+
+template <int D, int LOG2>
+void m_add_residual(uint8_t *dst, const int16_t *res, ptrdiff_t stride) { member_host(D, LOG2, K_BYPASS, 0, 0, nullptr, res, dst, stride); }
+template <int D>
+void m_dequant(int16_t *coeffs, int16_t log2)
+{
+    if (log2_ok(log2, "dequant")) member_host(D, log2, K_SKIP, 0, 0, coeffs, nullptr, nullptr, 0);
+}
+template <int D>
+void m_rdpcm(int16_t *coeffs, int16_t log2, int mode)
+{
+    if (log2_ok(log2, "transform_rdpcm"))
+        member_host(D, log2, K_BYPASS, B200_HEVC_TU_RDPCM | (mode ? B200_HEVC_TU_RDPCM_VER : 0), 0, coeffs, nullptr, nullptr, 0);
+}
+template <int D>
+void m_dst4(int16_t *coeffs) { member_host(D, 2, K_DST4, 0, 0, coeffs, nullptr, nullptr, 0); }
+template <int D, int LOG2>
+void m_idct(int16_t *coeffs, int col_limit) { member_host(D, LOG2, K_IDCT, 0, col_limit, coeffs, nullptr, nullptr, 0); }
+template <int D, int LOG2>
+void m_idct_dc(int16_t *coeffs) { member_host(D, LOG2, K_DC, 0, 0, coeffs, nullptr, nullptr, 0); }
+
+template <int D, int LOG2>
+void fill_size(B200HEVCDSPContext *c)
+{
+    c->add_residual[LOG2 - 2] = m_add_residual<D, LOG2>;
+    c->idct[LOG2 - 2] = m_idct<D, LOG2>;
+    c->idct_dc[LOG2 - 2] = m_idct_dc<D, LOG2>;
+}
+// hevc/dsp.c:198-215
+template <int D>
+void fill(B200HEVCDSPContext *c)
+{
+    fill_size<D, 2>(c);
+    fill_size<D, 3>(c);
+    fill_size<D, 4>(c);
+    fill_size<D, 5>(c);
+    c->dequant = m_dequant<D>;
+    c->transform_rdpcm = m_rdpcm<D>;
+    c->transform_4x4_luma = m_dst4<D>;
+}
+
+} // namespace
+
+B200_API int b200_hevc_dsp_init_transform(B200HEVCDSPContext *c, int bit_depth)
+{
+    if (!c) return B200_EINVAL;
+    if (!depth_ok(bit_depth)) return B200_ENOSYS;
+    if (!b200_default_device()) return B200_ENODEV;
+    switch (bit_depth) {
+    case 8:  fill<8>(c); break;
+    case 9:  fill<9>(c); break;
+    case 10: fill<10>(c); break;
+    default: fill<12>(c); break;
+    }
+    return 0;
+}
+
+B200_API int b200_hevc_transform_add_batch_device(B200Device *dev, int bit_depth, int64_t nops, const B200HevcTuOp *ops, const int16_t *coef,
+                                                  uint8_t *dst, ptrdiff_t dst_stride)
+{
+    if (nops < 0) { b200_set_error("hevc transform batch: negative nops"); return B200_EINVAL; }
+    if (!depth_ok(bit_depth)) { b200_set_error("hevc transform batch: bit depth %d is not 8, 9, 10 or 12", bit_depth); return B200_EINVAL; }
+    const int bps = bit_depth > 8 ? 2 : 1;
+    if (dst_stride % (4 * bps)) { b200_set_error("hevc transform batch: dst_stride not a multiple of 4 samples"); return B200_EINVAL; }
+    if (nops == 0) return 0;
+    if (!ops || !coef || !dst || ((uintptr_t)ops & 15) || ((uintptr_t)coef & 15) || ((uintptr_t)dst % (4 * bps))) {
+        b200_set_error("hevc transform batch: NULL or misaligned pointer");
+        return B200_EINVAL;
+    }
+    if (!dev) dev = b200_default_device();
+    if (!dev) return B200_ENODEV;
+    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    TuArgs a = { ops, (long long)nops, coef, dst, (long long)dst_stride, nullptr, bit_depth, 1 };
+    B200_CUDA_OK(launch(a, dev->stream));
+    return 0;
+}

@@ -1,16 +1,31 @@
-"""Host-side mirror of libavcodec's HEVC motion compensation: the put_hevc_{q,e}pel tables of HEVCDSPContext as ff_hevc_dsp_init
-installs them (libavcodec/hevc/dsp.c:140-196), and the batched device entry b200_hevc_mc_batch_device."""
+"""Host-side mirror of libavcodec's HEVC DSP: the put_hevc_{q,e}pel tables of HEVCDSPContext as ff_hevc_dsp_init installs them
+(libavcodec/hevc/dsp.c:140-196) and the batched device entry b200_hevc_mc_batch_device; the residual members (hevc/dsp.c:198-215) and
+the batched device entry b200_hevc_transform_add_batch_device."""
 import ctypes as C
 
 import numpy as np
 
-from ._lib import lib, check, vp, HEVCDSPContext, HevcMcOp
+from ._lib import lib, check, vp, HEVCDSPContext, HevcMcOp, HevcTuOp
 
 UNI, UNI_W, BI, BI_W = range(4)                 # B200HevcMcOp.kind
 OP_DTYPE = np.dtype([("dst_off", "<i8"), ("ref_off", "<i8", 2), ("x", "<i4", 2), ("y", "<i4", 2), ("mx", "u1", 2), ("my", "u1", 2),
                      ("w", "u1"), ("h", "u1"), ("kind", "u1"), ("denom", "u1"), ("wx0", "<i4"), ("wx1", "<i4"), ("ox", "<i4"),
                      ("reserved", "u1", 4)])
 assert OP_DTYPE.itemsize == C.sizeof(HevcMcOp) == 64
+
+IDCT, IDCT_DC, DST4, SKIP, BYPASS = range(5)    # B200HevcTuOp.kind
+RDPCM, RDPCM_VER, ROTATE = 1, 2, 4              # B200HevcTuOp.flags
+TU_DTYPE = np.dtype([("dst_off", "<i8"), ("coef_off", "<i8"), ("log2_size", "u1"), ("kind", "u1"), ("flags", "u1"), ("reserved0", "u1"),
+                     ("col_limit", "<i4"), ("reserved", "u1", 8)])
+assert TU_DTYPE.itemsize == C.sizeof(HevcTuOp) == 32
+
+# the residual members' signatures (HEVCDSPContext keeps them as plain pointers; cast with these to call one)
+ADD_RESIDUAL = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t)
+DEQUANT = C.CFUNCTYPE(None, C.c_void_p, C.c_int16)
+TRANSFORM_RDPCM = C.CFUNCTYPE(None, C.c_void_p, C.c_int16, C.c_int)
+TRANSFORM_4X4_LUMA = C.CFUNCTYPE(None, C.c_void_p)
+IDCT_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_int)
+IDCT_DC_FN = C.CFUNCTYPE(None, C.c_void_p)
 
 
 def _dptr(x):
@@ -22,6 +37,20 @@ def ff_hevc_dsp_init(bit_depth=8):
     c = HEVCDSPContext()
     check(lib().b200_hevc_dsp_init(C.byref(c), bit_depth), "ff_hevc_dsp_init")
     return c
+
+
+def ff_hevc_dsp_init_transform(c, bit_depth=8):
+    """fills the residual members of the HEVCDSPContext `c` (HOST pointers: add_residual, dequant, transform_rdpcm,
+    transform_4x4_luma, idct, idct_dc), leaving every other member as it is; returns c"""
+    check(lib().b200_hevc_dsp_init_transform(C.byref(c), bit_depth), "ff_hevc_dsp_init_transform")
+    return c
+
+
+def hevc_transform_add_batch_device(device, bit_depth, nops, ops, coef, dst, dst_stride):
+    """one plane's transform units; ops = TU_DTYPE records (a uint8 tensor of nops * 32 bytes), coef an int16 tensor (not written),
+    dst a sample tensor, dst_stride in bytes (device)"""
+    return check(lib().b200_hevc_transform_add_batch_device(device.handle, bit_depth, nops, vp(_dptr(ops)), vp(_dptr(coef)), vp(_dptr(dst)),
+                                                            dst_stride), "hevc_transform_add_batch_device")
 
 
 def hevc_mc_batch_device(device, bit_depth, epel, nops, ops, dst, dst_stride, ref, ref_stride, pic_w, pic_h):

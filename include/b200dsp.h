@@ -420,6 +420,55 @@ _Static_assert(sizeof(B200HevcMcOp) == 64, "B200HevcMcOp is 64 bytes");
 int  b200_hevc_mc_batch_device(B200Device *dev, int bit_depth, int epel, int64_t nops, const B200HevcMcOp *ops,
                                uint8_t *dst, ptrdiff_t dst_stride, const uint8_t *ref, ptrdiff_t ref_stride, int pic_w, int pic_h);
 
+/* HEVC residual: fills the transform members of a B200HEVCDSPContext as ff_hevc_dsp_init does (hevc/dsp.c:198-215):
+ * add_residual[0..3], dequant, transform_rdpcm, transform_4x4_luma, idct[0..3], idct_dc[0..3] (hevc/dsp_template.c:46-309).  It does
+ * not clear the context and touches no other member: call b200_hevc_dsp_init() first, then this.  HOST pointers, the reference's
+ * signatures: the members that take `coeffs` work in place on the int16 coefficients; add_residual clips to the sample depth
+ * (samples uint8 at 8 bit, uint16 above, stride in bytes) and leaves `res` as it is.  idct[k](coeffs, col_limit) takes col_limit as
+ * the reference does, as part of the function: odd inputs at or beyond the limit are not summed (so a block with non-zero
+ * coefficients there does not get the full transform); any int value gives the reference's result.  dequant / transform_rdpcm with a
+ * log2_size outside 2..5 (outside the reference's contract) write nothing and record the reason (b200_last_error()).
+ * Returns 0; B200_EINVAL for c == NULL; B200_ENOSYS for depths other than 8, 9, 10 and 12; B200_ENODEV. */
+int  b200_hevc_dsp_init_transform(B200HEVCDSPContext *c, int bit_depth);
+
+/* One transform unit of b200_hevc_transform_add_batch_device: the (1 << log2_size)^2 coefficients at coef + coef_off (int16 elements,
+ * row-major, as the parser leaves them: already scaled) and the block of samples at dst + dst_off (bytes).  The op's result is the
+ * decoder's sequence (hevc/cabac.c:1550-1592) on a copy of the coefficients, then add_residual[log2_size - 2]:
+ *   B200_HEVC_TU_IDCT     idct[log2_size - 2](c, col_limit)
+ *   B200_HEVC_TU_IDCT_DC  idct_dc[log2_size - 2](c)
+ *   B200_HEVC_TU_DST4     transform_4x4_luma(c)                     (4x4 only)
+ *   B200_HEVC_TU_SKIP     the 180-degree swap of a 4x4 when B200_HEVC_TU_ROTATE is set, dequant(c, log2_size), then
+ *                         transform_rdpcm(c, log2_size, B200_HEVC_TU_RDPCM_VER set) when B200_HEVC_TU_RDPCM is set
+ *   B200_HEVC_TU_BYPASS   transform_rdpcm(c, log2_size, B200_HEVC_TU_RDPCM_VER set) when B200_HEVC_TU_RDPCM is set
+ * The decoder's choices (DC when max_xy == 0, the implicit rdpcm direction, rotation) stay with the caller. */
+enum { B200_HEVC_TU_IDCT = 0, B200_HEVC_TU_IDCT_DC = 1, B200_HEVC_TU_DST4 = 2, B200_HEVC_TU_SKIP = 3, B200_HEVC_TU_BYPASS = 4 };
+enum { B200_HEVC_TU_RDPCM = 1, B200_HEVC_TU_RDPCM_VER = 2, B200_HEVC_TU_ROTATE = 4 };
+typedef struct B200HevcTuOp {
+    int64_t dst_off;      /* bytes, into dst */
+    int64_t coef_off;     /* int16 elements, into coef */
+    uint8_t log2_size;    /* 2..5 */
+    uint8_t kind;         /* B200_HEVC_TU_* */
+    uint8_t flags;        /* B200_HEVC_TU_RDPCM, B200_HEVC_TU_RDPCM_VER, B200_HEVC_TU_ROTATE */
+    uint8_t reserved0;
+    int32_t col_limit;    /* IDCT only, as the idct member receives it (cabac.c:1258-1265) */
+    uint8_t reserved[8];
+} B200HevcTuOp;
+#ifdef __cplusplus
+static_assert(sizeof(B200HevcTuOp) == 32, "B200HevcTuOp is 32 bytes");
+#else
+_Static_assert(sizeof(B200HevcTuOp) == 32, "B200HevcTuOp is 32 bytes");
+#endif
+/* Batched HEVC residual reconstruction of one plane, DEVICE pointers, asynchronous on the device's stream: every op's residual is
+ * added to its block of dst, clipped to the sample depth.  Unlike the in-place members, `coef` is const: the batch never writes
+ * coefficients.  The ops of one call write disjoint blocks.  An op whose log2_size is outside 2..5 or whose kind is undefined, a DST4
+ * op on a block other than 4x4, and an op whose coef_off is not a multiple of 8 elements or whose dst_off is not a multiple of 4
+ * samples write nothing (transform unit positions in a stream always satisfy these alignments).  Offsets are 64-bit; a call may have
+ * more ops than one launch takes.
+ * Returns 0, or B200_EINVAL (launching nothing) for NULL pointers, ops or coef not 16-byte aligned, dst not aligned to 4 samples,
+ * nops < 0, a depth other than 8, 9, 10 or 12, or a dst_stride that is not a multiple of 4 samples; nops == 0 returns 0. */
+int  b200_hevc_transform_add_batch_device(B200Device *dev, int bit_depth, int64_t nops, const B200HevcTuOp *ops, const int16_t *coef,
+                                          uint8_t *dst, ptrdiff_t dst_stride);
+
 /* mpegvideo inverse quantisers: the members of MPVUnquantDSPContext (libavcodec/mpegvideo_unquantize.h:31-44) as
  * ff_mpv_unquantize_init() installs them (libavcodec/mpegvideo_unquantize.c:50-290), i.e. what runs in front of the IDCT in
  * mpv_reconstruct_mb's put_dct / add_dequant_dct (libavcodec/mpegvideo_dec.c).  The reference functions take the whole

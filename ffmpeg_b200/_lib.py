@@ -170,6 +170,11 @@ class HevcTuOp(C.Structure):
                 ("reserved0", C.c_uint8), ("col_limit", C.c_int32), ("reserved", C.c_uint8 * 8)]
 
 
+class HevcDbkSeg(C.Structure):
+    """B200HevcDbkSeg (include/b200dsp.h), 4 bytes"""
+    _fields_ = [("beta", C.c_uint8), ("tc", C.c_uint8), ("flags", C.c_uint8), ("reserved", C.c_uint8)]
+
+
 class ProresDSPContext(C.Structure):
     """libavcodec/proresdsp.h:28-35"""
     _fields_ = [("idct_permutation_type", C.c_int), ("idct_permutation", C.c_uint8 * 64),
@@ -282,6 +287,8 @@ PROTOTYPES = {
     "b200_hevc_mc_batch_device": (C.c_int, [vp, C.c_int, C.c_int, C.c_int64, vp, vp, C.c_ssize_t, vp, C.c_ssize_t, C.c_int, C.c_int]),
     "b200_hevc_dsp_init_transform": (C.c_int, [vp, C.c_int]),
     "b200_hevc_transform_add_batch_device": (C.c_int, [vp, C.c_int, C.c_int64, vp, vp, vp, C.c_ssize_t]),
+    "b200_hevc_dsp_init_deblock": (C.c_int, [vp, C.c_int]),
+    "b200_hevc_deblock_plane_device": (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_ssize_t, C.c_int, C.c_int, vp, C.c_int64, vp, C.c_int64]),
     "b200_proresdsp_init": (C.c_int, [vp, C.c_int]),
     "b200_prores_idct_put_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, vp, vp, vp, C.c_int]),
     "b200_float_dsp_init": (C.c_int, [vp]),

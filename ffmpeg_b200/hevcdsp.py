@@ -1,11 +1,12 @@
 """Host-side mirror of libavcodec's HEVC DSP: the put_hevc_{q,e}pel tables of HEVCDSPContext as ff_hevc_dsp_init installs them
 (libavcodec/hevc/dsp.c:140-196) and the batched device entry b200_hevc_mc_batch_device; the residual members (hevc/dsp.c:198-215) and
-the batched device entry b200_hevc_transform_add_batch_device."""
+the batched device entry b200_hevc_transform_add_batch_device; the loop-filter members (hevc/dsp.c:237-244) and the plane entry
+b200_hevc_deblock_plane_device."""
 import ctypes as C
 
 import numpy as np
 
-from ._lib import lib, check, vp, HEVCDSPContext, HevcMcOp, HevcTuOp
+from ._lib import lib, check, vp, HEVCDSPContext, HevcMcOp, HevcTuOp, HevcDbkSeg
 
 UNI, UNI_W, BI, BI_W = range(4)                 # B200HevcMcOp.kind
 OP_DTYPE = np.dtype([("dst_off", "<i8"), ("ref_off", "<i8", 2), ("x", "<i4", 2), ("y", "<i4", 2), ("mx", "u1", 2), ("my", "u1", 2),
@@ -26,6 +27,15 @@ TRANSFORM_RDPCM = C.CFUNCTYPE(None, C.c_void_p, C.c_int16, C.c_int)
 TRANSFORM_4X4_LUMA = C.CFUNCTYPE(None, C.c_void_p)
 IDCT_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_int)
 IDCT_DC_FN = C.CFUNCTYPE(None, C.c_void_p)
+
+NO_P, NO_Q = 1, 2                               # B200HevcDbkSeg.flags
+DBK_DTYPE = np.dtype([("beta", "u1"), ("tc", "u1"), ("flags", "u1"), ("reserved", "u1")])
+assert DBK_DTYPE.itemsize == C.sizeof(HevcDbkSeg) == 4
+
+# the loop-filter members' signatures: (pix, stride, beta, tc[2], no_p[2], no_q[2]) for luma, (pix, stride, tc[2], no_p[2], no_q[2]) for
+# chroma
+LOOP_FILTER_LUMA = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p)
+LOOP_FILTER_CHROMA = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_void_p, C.c_void_p)
 
 
 def _dptr(x):
@@ -51,6 +61,20 @@ def hevc_transform_add_batch_device(device, bit_depth, nops, ops, coef, dst, dst
     dst a sample tensor, dst_stride in bytes (device)"""
     return check(lib().b200_hevc_transform_add_batch_device(device.handle, bit_depth, nops, vp(_dptr(ops)), vp(_dptr(coef)), vp(_dptr(dst)),
                                                             dst_stride), "hevc_transform_add_batch_device")
+
+
+def ff_hevc_dsp_init_deblock(c, bit_depth=8):
+    """fills the eight loop-filter members of the HEVCDSPContext `c` (HOST pointers; each _c member equal to its plain twin), leaving
+    every other member as it is; returns c"""
+    check(lib().b200_hevc_dsp_init_deblock(C.byref(c), bit_depth), "ff_hevc_dsp_init_deblock")
+    return c
+
+
+def hevc_deblock_plane_device(device, bit_depth, chroma, pix, stride, width, height, vseg, vseg_stride, hseg, hseg_stride):
+    """deblocks one plane in place (device); pix a sample tensor, stride in bytes; vseg / hseg DBK_DTYPE grids (uint8 tensors of 4-byte
+    records) with their strides in records"""
+    return check(lib().b200_hevc_deblock_plane_device(device.handle, bit_depth, chroma, vp(_dptr(pix)), stride, width, height, vp(_dptr(vseg)),
+                                                      vseg_stride, vp(_dptr(hseg)), hseg_stride), "hevc_deblock_plane_device")
 
 
 def hevc_mc_batch_device(device, bit_depth, epel, nops, ops, dst, dst_stride, ref, ref_stride, pic_w, pic_h):

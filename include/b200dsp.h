@@ -469,6 +469,41 @@ _Static_assert(sizeof(B200HevcTuOp) == 32, "B200HevcTuOp is 32 bytes");
 int  b200_hevc_transform_add_batch_device(B200Device *dev, int bit_depth, int64_t nops, const B200HevcTuOp *ops, const int16_t *coef,
                                           uint8_t *dst, ptrdiff_t dst_stride);
 
+/* HEVC deblocking: fills the eight loop-filter members of a B200HEVCDSPContext as ff_hevc_dsp_init does (hevc/dsp.c:237-244):
+ * hevc_{h,v}_loop_filter_{luma,chroma} and their _c twins, each _c member the same function as its plain twin
+ * (hevc/dsp_template.c:834-928).  It does not clear the context and touches no other member.  HOST pointers, the reference's
+ * signatures: `pix` is Q0 of line 0, the stride in bytes, samples uint8 at 8 bit and uint16 above; two segments of 4 lines, tc[j],
+ * no_p[j] and no_q[j] for lines 4j..4j+3 (any non-zero byte counts).  Domain: beta 0..255 and tc[j] <= 255 (the decoder's tables give
+ * at most 64 and 24); a segment with tc[j] <= 0 is left as it is, as the reference leaves it.  A member reads only P3..Q3 (luma) or
+ * P1..Q1 (chroma) of the lines of segments with tc[j] > 0, and writes only P2..Q2 / P0..Q0 of those lines.
+ * Returns 0; B200_EINVAL for c == NULL; B200_ENOSYS for depths other than 8, 9, 10 and 12; B200_ENODEV. */
+int  b200_hevc_dsp_init_deblock(B200HEVCDSPContext *c, int bit_depth);
+
+/* One 4-sample edge segment of b200_hevc_deblock_plane_device: beta and tc as the members receive them (the 8-bit table values; the
+ * kernel shifts them by depth - 8), flags B200_HEVC_DBK_NO_P / B200_HEVC_DBK_NO_Q (pcm / transquant-bypass sides left as they are).
+ * Other flag bits and `reserved` are ignored. */
+enum { B200_HEVC_DBK_NO_P = 1, B200_HEVC_DBK_NO_Q = 2 };
+typedef struct B200HevcDbkSeg {
+    uint8_t beta, tc, flags, reserved;
+} B200HevcDbkSeg;
+#ifdef __cplusplus
+static_assert(sizeof(B200HevcDbkSeg) == 4, "B200HevcDbkSeg is 4 bytes");
+#else
+_Static_assert(sizeof(B200HevcDbkSeg) == 4, "B200HevcDbkSeg is 4 bytes");
+#endif
+/* Deblocks one width x height plane in place, DEVICE pointers, asynchronous on the device's stream.  chroma 0 selects the luma
+ * filter, 1 the chroma (weak) filter.  Grids, in plane sample coordinates:
+ *   vseg[(y / 4) * vseg_stride + x / 8]  rows y..y+3 of the vertical edge at column x   (x = 0, 8, ... < width; y = 0, 4, ... < height)
+ *   hseg[(y / 8) * hseg_stride + x / 4]  columns x..x+3 of the horizontal edge at row y (y = 0, 8, ... < height; x = 0, 4, ... < width)
+ * Entries at x = 0 (vertical) and y = 0 (horizontal) are picture edges and ignored.  The result is that of the member call for every
+ * vertical segment (its beta, tc and flags; tc 0 for the member's other segment), then for every horizontal segment: the decoder's
+ * CTB-by-CTB sequence of member calls (hevc/filter.c:501-676) gives the same picture.  64-bit offsets.
+ * Returns 0, or B200_EINVAL (launching nothing) for NULL pointers, a depth other than 8, 9, 10 or 12, chroma other than 0 / 1, width or
+ * height below 4 or not a multiple of 4, a stride shorter than a row or not a multiple of the sample size, pix not aligned to a sample,
+ * vseg_stride < ceil(width / 8) or hseg_stride < width / 4. */
+int  b200_hevc_deblock_plane_device(B200Device *dev, int bit_depth, int chroma, uint8_t *pix, ptrdiff_t stride, int width, int height,
+                                    const B200HevcDbkSeg *vseg, int64_t vseg_stride, const B200HevcDbkSeg *hseg, int64_t hseg_stride);
+
 /* mpegvideo inverse quantisers: the members of MPVUnquantDSPContext (libavcodec/mpegvideo_unquantize.h:31-44) as
  * ff_mpv_unquantize_init() installs them (libavcodec/mpegvideo_unquantize.c:50-290), i.e. what runs in front of the IDCT in
  * mpv_reconstruct_mb's put_dct / add_dequant_dct (libavcodec/mpegvideo_dec.c).  The reference functions take the whole

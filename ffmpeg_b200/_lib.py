@@ -175,6 +175,17 @@ class HevcDbkSeg(C.Structure):
     _fields_ = [("beta", C.c_uint8), ("tc", C.c_uint8), ("flags", C.c_uint8), ("reserved", C.c_uint8)]
 
 
+class HevcSaoCtb(C.Structure):
+    """B200HevcSaoCtb (include/b200dsp.h), 16 bytes"""
+    _fields_ = [("offset_val", C.c_int16 * 5), ("type", C.c_uint8), ("cls", C.c_uint8), ("flags", C.c_uint16), ("reserved", C.c_uint16)]
+
+
+class SAOParams(C.Structure):
+    """B200SAOParams = libavcodec/hevc/dsp.h:34-45 SAOParams, 148 bytes"""
+    _fields_ = [("offset_abs", (C.c_int32 * 4) * 3), ("offset_sign", (C.c_int32 * 4) * 3), ("band_position", C.c_uint8 * 3),
+                ("eo_class", C.c_int32 * 3), ("offset_val", (C.c_int16 * 5) * 3), ("type_idx", C.c_uint8 * 3)]
+
+
 class ProresDSPContext(C.Structure):
     """libavcodec/proresdsp.h:28-35"""
     _fields_ = [("idct_permutation_type", C.c_int), ("idct_permutation", C.c_uint8 * 64),
@@ -289,6 +300,9 @@ PROTOTYPES = {
     "b200_hevc_transform_add_batch_device": (C.c_int, [vp, C.c_int, C.c_int64, vp, vp, vp, C.c_ssize_t]),
     "b200_hevc_dsp_init_deblock": (C.c_int, [vp, C.c_int]),
     "b200_hevc_deblock_plane_device": (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_ssize_t, C.c_int, C.c_int, vp, C.c_int64, vp, C.c_int64]),
+    "b200_hevc_dsp_init_sao": (C.c_int, [vp, C.c_int]),
+    "b200_hevc_sao_plane_device": (C.c_int, [vp, C.c_int, vp, C.c_ssize_t, vp, C.c_ssize_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp,
+                                             C.c_int64, vp, C.c_int64, C.c_int]),
     "b200_proresdsp_init": (C.c_int, [vp, C.c_int]),
     "b200_prores_idct_put_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, vp, vp, vp, C.c_int]),
     "b200_float_dsp_init": (C.c_int, [vp]),

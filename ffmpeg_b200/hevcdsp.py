@@ -1,12 +1,13 @@
 """Host-side mirror of libavcodec's HEVC DSP: the put_hevc_{q,e}pel tables of HEVCDSPContext as ff_hevc_dsp_init installs them
 (libavcodec/hevc/dsp.c:140-196) and the batched device entry b200_hevc_mc_batch_device; the residual members (hevc/dsp.c:198-215) and
 the batched device entry b200_hevc_transform_add_batch_device; the loop-filter members (hevc/dsp.c:237-244) and the plane entry
-b200_hevc_deblock_plane_device."""
+b200_hevc_deblock_plane_device; the sample adaptive offset members (hevc/dsp.c:217-228) and the out-of-place plane entry
+b200_hevc_sao_plane_device."""
 import ctypes as C
 
 import numpy as np
 
-from ._lib import lib, check, vp, HEVCDSPContext, HevcMcOp, HevcTuOp, HevcDbkSeg
+from ._lib import lib, check, vp, HEVCDSPContext, HevcMcOp, HevcTuOp, HevcDbkSeg, HevcSaoCtb, SAOParams
 
 UNI, UNI_W, BI, BI_W = range(4)                 # B200HevcMcOp.kind
 OP_DTYPE = np.dtype([("dst_off", "<i8"), ("ref_off", "<i8", 2), ("x", "<i4", 2), ("y", "<i4", 2), ("mx", "u1", 2), ("my", "u1", 2),
@@ -36,6 +37,21 @@ assert DBK_DTYPE.itemsize == C.sizeof(HevcDbkSeg) == 4
 # chroma
 LOOP_FILTER_LUMA = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p)
 LOOP_FILTER_CHROMA = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_void_p, C.c_void_p)
+
+SAO_NONE, SAO_BAND, SAO_EDGE = range(3)         # B200HevcSaoCtb.type
+(SAO_RESTORE, SAO_VERT_L, SAO_VERT_R, SAO_HORIZ_T, SAO_HORIZ_B, SAO_DIAG_TL, SAO_DIAG_TR, SAO_DIAG_BR,
+ SAO_DIAG_BL) = (1 << k for k in range(9))      # B200HevcSaoCtb.flags
+SAO_DTYPE = np.dtype([("offset_val", "<i2", 5), ("type", "u1"), ("cls", "u1"), ("flags", "<u2"), ("reserved", "<u2")])
+assert SAO_DTYPE.itemsize == C.sizeof(HevcSaoCtb) == 16
+assert C.sizeof(SAOParams) == 148
+
+# the SAO members' signatures: band (dst, src, stride_dst, stride_src, offset_val, left_class, width, height); edge (dst, src at the
+# 192-byte stride, stride_dst, offset_val, eo_class, width, height); restore (dst, src, stride_dst, stride_src, sao, borders, width,
+# height, c_idx, vert_edge, horiz_edge, diag_edge)
+SAO_BAND_FILTER = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_ssize_t, C.c_void_p, C.c_int, C.c_int, C.c_int)
+SAO_EDGE_FILTER = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_int, C.c_int, C.c_int)
+SAO_EDGE_RESTORE = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_ssize_t, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                               C.c_void_p, C.c_void_p, C.c_void_p)
 
 
 def _dptr(x):
@@ -75,6 +91,23 @@ def hevc_deblock_plane_device(device, bit_depth, chroma, pix, stride, width, hei
     records) with their strides in records"""
     return check(lib().b200_hevc_deblock_plane_device(device.handle, bit_depth, chroma, vp(_dptr(pix)), stride, width, height, vp(_dptr(vseg)),
                                                       vseg_stride, vp(_dptr(hseg)), hseg_stride), "hevc_deblock_plane_device")
+
+
+def ff_hevc_dsp_init_sao(c, bit_depth=8):
+    """fills the SAO members of the HEVCDSPContext `c` (HOST pointers: sao_band_filter[5], sao_edge_filter[5], sao_edge_restore[2]),
+    leaving every other member as it is; returns c"""
+    check(lib().b200_hevc_dsp_init_sao(C.byref(c), bit_depth), "ff_hevc_dsp_init_sao")
+    return c
+
+
+def hevc_sao_plane_device(device, bit_depth, dst, dst_stride, src, src_stride, width, height, log2_ctb_size, hshift, vshift, ctb, ctb_stride,
+                          keep=None, keep_stride=0, log2_min_pu_size=0):
+    """applies SAO to one plane out of place (device): dst / src sample tensors (not overlapping), strides in bytes; ctb a SAO_DTYPE
+    grid (a uint8 tensor of 16-byte records) with its stride in records; keep None or the is_pcm map (uint8, one byte per luma min PU)"""
+    return check(lib().b200_hevc_sao_plane_device(device.handle, bit_depth, vp(_dptr(dst)), dst_stride, vp(_dptr(src)), src_stride, width,
+                                                  height, log2_ctb_size, hshift, vshift, vp(_dptr(ctb)), ctb_stride,
+                                                  None if keep is None else vp(_dptr(keep)), keep_stride, log2_min_pu_size),
+                 "hevc_sao_plane_device")
 
 
 def hevc_mc_batch_device(device, bit_depth, epel, nops, ops, dst, dst_stride, ref, ref_stride, pic_w, pic_h):

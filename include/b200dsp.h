@@ -504,6 +504,88 @@ _Static_assert(sizeof(B200HevcDbkSeg) == 4, "B200HevcDbkSeg is 4 bytes");
 int  b200_hevc_deblock_plane_device(B200Device *dev, int bit_depth, int chroma, uint8_t *pix, ptrdiff_t stride, int width, int height,
                                     const B200HevcDbkSeg *vseg, int64_t vseg_stride, const B200HevcDbkSeg *hseg, int64_t hseg_stride);
 
+/* HEVC sample adaptive offset: SAOParams (libavcodec/hevc/dsp.h:34-45) with the reference's layout, what sao_edge_restore[] reads
+ * through its `const struct SAOParams *` (only offset_val[c_idx][0] and eo_class[c_idx]). */
+typedef struct B200SAOParams {
+    int32_t offset_abs[3][4];
+    int32_t offset_sign[3][4];
+    uint8_t band_position[3];
+    int32_t eo_class[3];          /* 0 horizontal, 1 vertical, 2 = 135 degrees, 3 = 45 degrees */
+    int16_t offset_val[3][5];     /* SaoOffsetVal: offset_abs << log2_sao_offset_scale with its sign (up to +-124 at 12 bit) */
+    uint8_t type_idx[3];
+} B200SAOParams;
+#ifdef __cplusplus
+static_assert(sizeof(B200SAOParams) == 148, "B200SAOParams is 148 bytes");
+#else
+_Static_assert(sizeof(B200SAOParams) == 148, "B200SAOParams is 148 bytes");
+#endif
+
+/* Fills the SAO members of a B200HEVCDSPContext as ff_hevc_dsp_init does (hevc/dsp.c:217-228): sao_band_filter[0..4] (one
+ * function), sao_edge_filter[0..4] (one function), sao_edge_restore[0] and [1] (h26x/h2656_sao_template.c).  It does not clear the
+ * context and touches no other member.  HOST pointers, the reference's signatures, samples uint8 at 8 bit and uint16 above, strides
+ * in bytes:
+ *   sao_band_filter   dst[x] = clip(src[x] + table[(src[x] >> (depth - 5)) & 31]), table[(k + sao_left_class) & 31] = offset_val[k + 1]
+ *                     for k = 0..3 and 0 elsewhere, for any int sao_left_class.  Reads and writes exactly width x height; dst == src
+ *                     with equal strides (the decoder's in-place call) works, as do separate buffers.
+ *   sao_edge_filter   `src` at the implicit stride of 192 bytes (2 * MAX_PB_SIZE + AV_INPUT_BUFFER_PADDING_SIZE) at every depth;
+ *                     reads the width x height block and only the ring its class's neighbours use (no rows -1 / height for the
+ *                     horizontal class, no columns -1 / width for the vertical one); writes exactly width x height of dst.
+ *   Domain of both: 1 <= width, height <= 64, sao_eo_class 0..3; outside it a member writes nothing and records the reason in
+ *   b200_last_error().  Both run the plane kernel of b200_hevc_sao_plane_device on a scratch plane.
+ *   sao_edge_restore  [0] / [1]: the picture-border samples (borders[4] = left, top, right, bottom) become clip(src + offset_val[0]);
+ *                     [1] then puts back `src` where vert_edge[2], horiz_edge[2] and diag_edge[4] mark an edge that may not be
+ *                     filtered, with the reference's corner exceptions, in the reference's order of writes.  They read only
+ *                     sao->offset_val[c_idx][0] and sao->eo_class[c_idx] (any value, compared with the four classes as the
+ *                     reference does); c_idx outside 0..2 or a size outside 1..64 writes nothing and records the reason.  They launch nothing: at most four lines of at most 64
+ *                     samples are copied on the host, classified by the same per-sample function the kernel uses.  Where the
+ *                     reference would write outside the width x height block (a 1-sample-wide block with a picture border and an
+ *                     edge flag on the same side, which the decoder never passes), they do not.
+ * Returns 0; B200_EINVAL for c == NULL; B200_ENOSYS for depths other than 8, 9, 10 and 12; B200_ENODEV. */
+int  b200_hevc_dsp_init_sao(B200HEVCDSPContext *c, int bit_depth);
+
+/* One CTB of one component for b200_hevc_sao_plane_device: what hls_sao_param parsed for it (offset_val = SaoOffsetVal[0..4], type,
+ * band_position or eo_class) and what sao_filter_CTB computes from the slice and tile maps (hevc/filter.c:283-329): RESTORE = its
+ * `restore` (sao_edge_restore[1] is used), VERT_L / VERT_R = vert_edge[0 / 1], HORIZ_T / HORIZ_B = horiz_edge[0 / 1], DIAG_TL / TR /
+ * BR / BL = diag_edge[0..3].  The edge flags count only with RESTORE, and only where sao_filter_CTB can compute them: a flag on a side
+ * (or a corner touching a side) that is a picture border is ignored.  Unknown flag bits and `reserved` are ignored. */
+enum { B200_HEVC_SAO_NONE = 0, B200_HEVC_SAO_BAND = 1, B200_HEVC_SAO_EDGE = 2 };
+enum {
+    B200_HEVC_SAO_RESTORE = 1, B200_HEVC_SAO_VERT_L = 2, B200_HEVC_SAO_VERT_R = 4, B200_HEVC_SAO_HORIZ_T = 8, B200_HEVC_SAO_HORIZ_B = 16,
+    B200_HEVC_SAO_DIAG_TL = 32, B200_HEVC_SAO_DIAG_TR = 64, B200_HEVC_SAO_DIAG_BR = 128, B200_HEVC_SAO_DIAG_BL = 256
+};
+typedef struct B200HevcSaoCtb {
+    int16_t  offset_val[5];
+    uint8_t  type;                /* B200_HEVC_SAO_NONE / _BAND / _EDGE */
+    uint8_t  cls;                 /* band_position (BAND, used & 31) or eo_class (EDGE) */
+    uint16_t flags;
+    uint16_t reserved;
+} B200HevcSaoCtb;
+#ifdef __cplusplus
+static_assert(sizeof(B200HevcSaoCtb) == 16, "B200HevcSaoCtb is 16 bytes");
+#else
+_Static_assert(sizeof(B200HevcSaoCtb) == 16, "B200HevcSaoCtb is 16 bytes");
+#endif
+/* Applies SAO to one width x height plane out of place, DEVICE pointers, asynchronous on the device's stream: `src` is the deblocked
+ * plane and `dst` becomes what sao_filter_CTB (hevc/filter.c:269-478) makes of it for this component over every CTB, which depends
+ * only on the deblocked plane whatever order the CTBs run in (neighbours always come from deblocked samples).  CTB (i, j) is
+ * ctb[j * ctb_stride + i] and covers [i * cw, min((i + 1) * cw, width)) x [j * ch, min((j + 1) * ch, height)), cw = (1 << log2_ctb_size)
+ * >> hshift, ch = (1 << log2_ctb_size) >> vshift (log2_ctb_size is the luma CTB size); the picture borders are the grid's outer
+ * sides.  NONE CTBs, an unknown type and EDGE with cls > 3 are copied.
+ * keep: NULL when the decoder's `transquant_bypass_enable_flag || (pcm_enabled && pcm_loop_filter_disabled)` is false; else its
+ * is_pcm map (one byte per luma min PU, keep[py * keep_stride + px], 1 << log2_min_pu_size luma samples), and the samples
+ * restore_tqb_pixels (hevc/filter.c:228-265) puts back are taken from src.  Reference quirk reproduced: it is called with the luma
+ * CTB origin but the component's CTB width and height, so for 4:2:0 chroma only PCM / bypass blocks in the top-left quarter of a
+ * chroma CTB are restored, for 4:2:2 only those in the left half (luma and 4:4:4: the whole CTB).
+ * Reads nothing outside the src plane, writes nothing outside the dst plane; 64-bit offsets.
+ * Returns 0, or B200_EINVAL (launching nothing) for NULL dst / src / ctb, a depth other than 8, 9, 10 or 12, width or height below 1,
+ * log2_ctb_size outside 4..6, a shift outside {0, 1}, a stride shorter than a row or not a multiple of the sample size, dst / src
+ * not aligned to a sample or ctb not aligned to 16 bytes, ctb_stride < ceil(width / cw), with keep given log2_min_pu_size outside
+ * 2..log2_ctb_size - 1 or keep_stride < ((width << hshift) >> log2_min_pu_size), or dst and src byte ranges that overlap (the entry
+ * does not work in place). */
+int  b200_hevc_sao_plane_device(B200Device *dev, int bit_depth, uint8_t *dst, ptrdiff_t dst_stride, const uint8_t *src, ptrdiff_t src_stride,
+                                int width, int height, int log2_ctb_size, int hshift, int vshift, const B200HevcSaoCtb *ctb,
+                                int64_t ctb_stride, const uint8_t *keep, int64_t keep_stride, int log2_min_pu_size);
+
 /* mpegvideo inverse quantisers: the members of MPVUnquantDSPContext (libavcodec/mpegvideo_unquantize.h:31-44) as
  * ff_mpv_unquantize_init() installs them (libavcodec/mpegvideo_unquantize.c:50-290), i.e. what runs in front of the IDCT in
  * mpv_reconstruct_mb's put_dct / add_dequant_dct (libavcodec/mpegvideo_dec.c).  The reference functions take the whole

@@ -395,12 +395,22 @@ sws_vscale_rgb24_fast_kernel(SwsFrameArgs a, SwsDevTables t, SwsColorConst c, in
     store_out<KIND>(a.dst + f * a.dfs + (long long)dy * (int)a.ds + xg * (16 * OutWords<KIND>::bpp), m);
 }
 
-// ------------------------------------------------------------------------------------------------ kernel: two output lines per thread
-// Same arithmetic as sws_vscale_rgb24_fast_kernel<true, true, KIND, NV> (identity luma bank, 4 chroma taps), for a pair of output lines
+// ------------------------------------------------------------------------------------------------ kernel: line pairs, streamed down bands
+// Same arithmetic as sws_vscale_rgb24_fast_kernel<true, true, KIND, NV> (identity luma bank, 4 chroma taps), for pairs of output lines
 // whose chroma windows coincide.  With 2x vertical chroma up-sampling the bicubic window of output lines 2k+1 and 2k+2 starts at the same
-// chroma line (vChrFilterPos equal, only the coefficients differ; the host checks this for the whole bank), so one thread loads the four
-// chroma lines once, interleaves them once (PRMT) and evaluates both lines from the same registers: 16 px x 2 lines per thread,
-// half the chroma loads, interleaves, address arithmetic and set-up of the one-line kernel.
+// chroma line (vChrFilterPos equal, only the coefficients differ; the host checks this for the whole bank), so the four chroma lines are
+// interleaved once (PRMT) and both lines are evaluated from the same registers.
+// One thread = 16 px of a band of up to PairShape<KIND>::band consecutive pairs of one frame, walked top to bottom:
+//  - the raw chroma tap lines stay in registers as a sliding window: when the next pair's window starts one line lower (2x up-sampling)
+//    only the line it gains is loaded (one line per plane per pair instead of four); any other step reloads the window;
+//  - the next pair's luma rows, gained chroma line and coefficients are loaded before the current pair is computed, and the positions
+//    two pairs ahead, so that no load waits for another load issued in the same step.
+// Threads do not share data (no shared memory, no shuffles).  Grid: x over 16-px groups, y over bands, z over frames.
+// Band length and CTAs per SM as measured on the H100 (DESIGN.md §5).  24-bit rows: bands of 16 pairs at 6 CTAs per SM (80 registers).
+// 32-bit rows: one pair per thread at 5 CTAs per SM (96 registers): with their 64-byte stores, bands of 4 or 16 pairs were slower than
+// one pair, whatever the occupancy; with one pair the steps ahead reload the same pair's rows (L1 hits) and the window never slides.
+constexpr int PAIR_THREADS = 128;
+template <int KIND> struct PairShape { static constexpr int band = KIND <= SWS_OUT_BGR24 ? 16 : 1, ctas = KIND <= SWS_OUT_BGR24 ? 6 : 5; };
 __device__ __forceinline__ void interleave2(const uint2 &r0, const uint2 &r1, unsigned *w)
 {
     w[0] = __byte_perm(r0.x, r1.x, 0x5140); w[1] = __byte_perm(r0.x, r1.x, 0x7362);
@@ -415,61 +425,91 @@ __device__ __forceinline__ void interleave2_nv(const uint4 &r0, const uint4 &r1,
     wu[2] = __byte_perm(r0.z, r1.z, SU); wv[2] = __byte_perm(r0.z, r1.z, SV);
     wu[3] = __byte_perm(r0.w, r1.w, SU); wv[3] = __byte_perm(r0.w, r1.w, SV);
 }
-
-template <int KIND, int NV>
-__global__ void __launch_bounds__(128, 8)
-sws_vscale_rgb24_pair_kernel(SwsFrameArgs a, SwsDevTables t, SwsColorConst c, int ngroups)
+// one chroma tap line of a thread's 16 px: 8 U bytes in .x/.y and 8 V bytes in .z/.w (planar), or the 16 interleaved bytes (nv12 / nv21)
+template <int NV>
+__device__ __forceinline__ uint4 pair_chroma_line(const uint8_t *ub, const uint8_t *vb, int us, int vs, int l)
 {
-    constexpr int PW = OutWords<KIND>::per_pair;
+    if (NV) return __ldg(reinterpret_cast<const uint4 *>(ub + l * us));
+    const uint2 u = __ldg(reinterpret_cast<const uint2 *>(ub + l * us)), v = __ldg(reinterpret_cast<const uint2 *>(vb + l * vs));
+    return make_uint4(u.x, u.y, v.x, v.y);
+}
+// two tap lines -> two chroma samples x two lines per word, U in iu[0..3], V in iv[0..3]
+template <int NV>
+__device__ __forceinline__ void pair_interleave(const uint4 &r0, const uint4 &r1, unsigned *iu, unsigned *iv)
+{
+    if (NV) interleave2_nv<NV>(r0, r1, iu, iv);
+    else {
+        interleave2(make_uint2(r0.x, r0.y), make_uint2(r1.x, r1.y), iu);
+        interleave2(make_uint2(r0.z, r0.w), make_uint2(r1.z, r1.w), iv);
+    }
+}
+
+// pairs [0, npairs) of output lines (a.y0 + 2p, a.y0 + 2p + 1), a.y0 odd
+template <int KIND, int NV>
+__global__ void __launch_bounds__(PAIR_THREADS, PairShape<KIND>::ctas)
+sws_vscale_rgb24_pair_kernel(SwsFrameArgs a, SwsDevTables t, SwsColorConst c, int ngroups, int npairs)
+{
+    constexpr int PW = OutWords<KIND>::per_pair, BAND = PairShape<KIND>::band;
     const int xg = blockIdx.x * blockDim.x + threadIdx.x;
     if (xg >= ngroups) return;
-    const int dA = a.y0 + 2 * blockIdx.y;                                   // lines dA and dA + 1
+    const int dA0 = a.y0 + 2 * blockIdx.y * BAND, np = min(BAND, npairs - (int)blockIdx.y * BAND);
     const long long f = blockIdx.z;
-    const int firstChr = max(-3, __ldg(t.vChrPos + dA));                    // == vChrPos[dA + 1]
-    const int chmax = a.chrSrcH - 1;
-    const int l0 = min(max(firstChr, 0), chmax), l1 = min(max(firstChr + 1, 0), chmax);
-    const int l2 = min(max(firstChr + 2, 0), chmax), l3 = min(max(firstChr + 3, 0), chmax);
-    const int us = (int)a.us, vs = (int)a.vs, ys = (int)a.ys;
-    unsigned IU[2][4], IV[2][4];                                            // [tap pair][word]: two chroma samples x two lines each
-    if (NV) {
-        const uint8_t *uvb = a.u + f * a.ufs + xg * 16;
-        const uint4 q0 = __ldg(reinterpret_cast<const uint4 *>(uvb + l0 * us)), q1 = __ldg(reinterpret_cast<const uint4 *>(uvb + l1 * us));
-        const uint4 q2 = __ldg(reinterpret_cast<const uint4 *>(uvb + l2 * us)), q3 = __ldg(reinterpret_cast<const uint4 *>(uvb + l3 * us));
-        interleave2_nv<NV ? NV : 1>(q0, q1, IU[0], IV[0]);
-        interleave2_nv<NV ? NV : 1>(q2, q3, IU[1], IV[1]);
-    } else {
-        const uint8_t *ub = a.u + f * a.ufs + xg * 8, *vb = a.v + f * a.vfs + xg * 8;
-        const uint2 u0 = __ldg(reinterpret_cast<const uint2 *>(ub + l0 * us)), u1 = __ldg(reinterpret_cast<const uint2 *>(ub + l1 * us));
-        const uint2 u2 = __ldg(reinterpret_cast<const uint2 *>(ub + l2 * us)), u3 = __ldg(reinterpret_cast<const uint2 *>(ub + l3 * us));
-        const uint2 v0 = __ldg(reinterpret_cast<const uint2 *>(vb + l0 * vs)), v1 = __ldg(reinterpret_cast<const uint2 *>(vb + l1 * vs));
-        const uint2 v2 = __ldg(reinterpret_cast<const uint2 *>(vb + l2 * vs)), v3 = __ldg(reinterpret_cast<const uint2 *>(vb + l3 * vs));
-        interleave2(u0, u1, IU[0]); interleave2(u2, u3, IU[1]);
-        interleave2(v0, v1, IV[0]); interleave2(v2, v3, IV[1]);
-    }
+    const int ys = (int)a.ys, us = (int)a.us, vs = (int)a.vs, chmax = a.chrSrcH - 1, lmax = a.srcH - 1;
     const uint8_t *yb = a.y + f * a.yfs + xg * 16;
-    const int lyA = min(max(__ldg(t.vLumPos + dA), 0), a.srcH - 1), lyB = min(max(__ldg(t.vLumPos + dA + 1), 0), a.srcH - 1);
-    const uint4 qy[2] = { __ldg(reinterpret_cast<const uint4 *>(yb + lyA * ys)), __ldg(reinterpret_cast<const uint4 *>(yb + lyB * ys)) };
-    const int2 kA = __ldg(reinterpret_cast<const int2 *>(t.vChr2 + 2 * dA)), kB = __ldg(reinterpret_cast<const int2 *>(t.vChr2 + 2 * dA + 2));
-    uint8_t *drow = a.dst + f * a.dfs + (long long)dA * (int)a.ds + xg * (16 * OutWords<KIND>::bpp);
+    const uint8_t *ub = a.u + f * a.ufs + xg * (NV ? 16 : 8), *vb = NV ? nullptr : a.v + f * a.vfs + xg * 8;
+    uint8_t *drow = a.dst + f * a.dfs + (long long)dA0 * a.ds + xg * (16 * OutWords<KIND>::bpp);
+    auto line = [&](int l) { return pair_chroma_line<NV>(ub, vb, us, vs, min(max(l, 0), chmax)); };
+    auto luma = [&](int dy) { return __ldg(reinterpret_cast<const uint4 *>(yb + min(max(__ldg(t.vLumPos + dy), 0), lmax) * ys)); };
+    auto first_chr = [&](int p) { return max(-3, __ldg(t.vChrPos + dA0 + 2 * p)); };          // == vChrPos[dA + 1]
+
+    // pair 0: the whole window; pair 1: its positions
+    int fc = first_chr(0);
+    uint4 W0 = line(fc), W1 = line(fc + 1), W2 = line(fc + 2), W3 = line(fc + 3);
+    uint4 YA = luma(dA0), YB = luma(dA0 + 1);
+    int2 kA = __ldg(reinterpret_cast<const int2 *>(t.vChr2 + 2 * dA0)), kB = __ldg(reinterpret_cast<const int2 *>(t.vChr2 + 2 * dA0 + 2));
+    const int p1 = min(1, np - 1);
+    int fcN = first_chr(p1);
+    int lyNA = min(max(__ldg(t.vLumPos + dA0 + 2 * p1), 0), lmax) * ys, lyNB = min(max(__ldg(t.vLumPos + dA0 + 2 * p1 + 1), 0), lmax) * ys;
+    for (int i = 0; i < np; i++) {
+        // pair i + 1 (the last pair repeats itself): the line its window gains, its luma rows and coefficients; pair i + 2: positions
+        const int in = min(i + 1, np - 1), i2 = min(i + 2, np - 1), dN = dA0 + 2 * in, d2 = dA0 + 2 * i2;
+        const bool slide = fcN == fc + 1;
+        const uint4 G = slide ? line(fcN + 3) : W3;
+        const uint4 NA = __ldg(reinterpret_cast<const uint4 *>(yb + lyNA)), NB = __ldg(reinterpret_cast<const uint4 *>(yb + lyNB));
+        const int2 kNA = __ldg(reinterpret_cast<const int2 *>(t.vChr2 + 2 * dN)), kNB = __ldg(reinterpret_cast<const int2 *>(t.vChr2 + 2 * dN + 2));
+        const int fc2 = first_chr(i2);
+        const int ly2A = min(max(__ldg(t.vLumPos + d2), 0), lmax) * ys, ly2B = min(max(__ldg(t.vLumPos + d2 + 1), 0), lmax) * ys;
+
+        unsigned IU[2][4], IV[2][4];                                        // [tap pair][word]: two chroma samples x two lines each
+        pair_interleave<NV>(W0, W1, IU[0], IV[0]);
+        pair_interleave<NV>(W2, W3, IU[1], IV[1]);
+        uint8_t *d = drow + (long long)(2 * i) * a.ds;
+#pragma unroll 1
+        for (int L = 0; L < 2; L++) {
+            const int kx = L ? kB.x : kA.x, ky = L ? kB.y : kA.y;
+            int aU[8], aV[8];
 #pragma unroll
-    for (int L = 0; L < 2; L++) {
-        const int kx = L ? kB.x : kA.x, ky = L ? kB.y : kA.y;
-        int aU[8], aV[8];
+            for (int w = 0; w < 4; w++) {
+                aU[2 * w]     = dp2a_lo_su(ky, IU[1][w], dp2a_lo_su(kx, IU[0][w], 1 << 11));
+                aU[2 * w + 1] = dp2a_hi_su(ky, IU[1][w], dp2a_hi_su(kx, IU[0][w], 1 << 11));
+                aV[2 * w]     = dp2a_lo_su(ky, IV[1][w], dp2a_lo_su(kx, IV[0][w], 1 << 11));
+                aV[2 * w + 1] = dp2a_hi_su(ky, IV[1][w], dp2a_hi_su(kx, IV[0][w], 1 << 11));
+            }
+            const uint4 q = L ? YB : YA;
+            const unsigned yw[4] = { q.x, q.y, q.z, q.w };
+            unsigned m[8 * PW];
 #pragma unroll
-        for (int w = 0; w < 4; w++) {
-            aU[2 * w]     = dp2a_lo_su(ky, IU[1][w], dp2a_lo_su(kx, IU[0][w], 1 << 11));
-            aU[2 * w + 1] = dp2a_hi_su(ky, IU[1][w], dp2a_hi_su(kx, IU[0][w], 1 << 11));
-            aV[2 * w]     = dp2a_lo_su(ky, IV[1][w], dp2a_lo_su(kx, IV[0][w], 1 << 11));
-            aV[2 * w + 1] = dp2a_hi_su(ky, IV[1][w], dp2a_hi_su(kx, IV[0][w], 1 << 11));
+            for (int j = 0; j < 8; j++) {
+                const ChromaBase cb = chroma_base(c, aU[j] >> 12, aV[j] >> 12);
+                pair_out<KIND>(c.cy, cb, byte_of(yw[(2 * j) >> 2], (2 * j) & 3), byte_of(yw[(2 * j + 1) >> 2], (2 * j + 1) & 3), m + PW * j);
+            }
+            store_out<KIND>(L ? d + a.ds : d, m);
         }
-        const unsigned yw[4] = { qy[L].x, qy[L].y, qy[L].z, qy[L].w };
-        unsigned m[8 * PW];
-#pragma unroll
-        for (int i = 0; i < 8; i++) {
-            const ChromaBase cb = chroma_base(c, aU[i] >> 12, aV[i] >> 12);
-            pair_out<KIND>(c.cy, cb, byte_of(yw[(2 * i) >> 2], (2 * i) & 3), byte_of(yw[(2 * i + 1) >> 2], (2 * i + 1) & 3), m + PW * i);
-        }
-        store_out<KIND>(drow + (long long)L * (int)a.ds, m);
+
+        if (slide) { W0 = W1; W1 = W2; W2 = W3; W3 = G; }
+        else if (fcN != fc) { W0 = line(fcN); W1 = line(fcN + 1); W2 = line(fcN + 2); W3 = line(fcN + 3); }
+        YA = NA; YB = NB; kA = kNA; kB = kNB;
+        fc = fcN; fcN = fc2; lyNA = ly2A; lyNB = ly2B;
     }
 }
 
@@ -948,7 +988,8 @@ struct B200SwsContext {
     SwsDevTables dt{};
     void *mma_tables = nullptr;      // horizontal banks as tensor-core operands (sws_mma.cuh)
     SwsMmaBank mmaL{}, mmaC{};
-    int last_path = 0;               // kernels the last scaled-path launch used: 1 two passes, 2 fused CUDA-core, 4 fused tensor-core (b200_sws_last_path)
+    int last_path = 0;               // kernels the last launches used: 1 two passes, 2 fused CUDA-core, 4 fused tensor-core (scaled path),
+                                     // 8 same-size line-pair kernel (b200_sws_last_path)
     int mma_pitchL = 0, mma_pitchC = 0, mma_pitchC8 = 0;   // staged-line pitches: luma / chroma tiles of 16 groups, chroma tiles of 8 groups
     bool h_identity = false;         // both horizontal banks are the identity -> u8-source kernels
     bool fast_x = false;             // every line uses the _X writer and no 32-bit sum can wrap -> vector kernel
@@ -1626,18 +1667,20 @@ static void launch_vscale_fast_nv(int kind, int nv, dim3 grid, dim3 block, cudaS
 struct SwsRows { int dy0, ndy, ly0, nly, cy0, ncy; };
 
 
-// the two-line kernel over output lines [first, first + 2 * npairs), first odd
+// the line-pair kernel over output lines [b.y0, b.y0 + 2 * npairs), b.y0 odd, for ngroups 16-px groups of each line
 template <int NV>
-static void launch_vscale_pair(int kind, dim3 grid, dim3 block, cudaStream_t stream, const SwsFrameArgs &b, const SwsDevTables &dt,
-                               const SwsColorConst &col, int ngroups)
+static void launch_vscale_pair(int kind, int ngroups, int npairs, int nf, cudaStream_t stream, const SwsFrameArgs &b, const SwsDevTables &dt,
+                               const SwsColorConst &col)
 {
+    const dim3 block(PAIR_THREADS);
+    auto grid = [&](int band) { return dim3(b200_ceil_div(ngroups, PAIR_THREADS), b200_ceil_div(npairs, band), nf); };
     switch (kind) {
-    case SWS_OUT_RGB24: sws_vscale_rgb24_pair_kernel<SWS_OUT_RGB24, NV><<<grid, block, 0, stream>>>(b, dt, col, ngroups); break;
-    case SWS_OUT_BGR24: sws_vscale_rgb24_pair_kernel<SWS_OUT_BGR24, NV><<<grid, block, 0, stream>>>(b, dt, col, ngroups); break;
-    case SWS_OUT_RGBA:  sws_vscale_rgb24_pair_kernel<SWS_OUT_RGBA, NV><<<grid, block, 0, stream>>>(b, dt, col, ngroups); break;
-    case SWS_OUT_BGRA:  sws_vscale_rgb24_pair_kernel<SWS_OUT_BGRA, NV><<<grid, block, 0, stream>>>(b, dt, col, ngroups); break;
-    case SWS_OUT_ARGB:  sws_vscale_rgb24_pair_kernel<SWS_OUT_ARGB, NV><<<grid, block, 0, stream>>>(b, dt, col, ngroups); break;
-    default:            sws_vscale_rgb24_pair_kernel<SWS_OUT_ABGR, NV><<<grid, block, 0, stream>>>(b, dt, col, ngroups); break;
+    case SWS_OUT_RGB24: sws_vscale_rgb24_pair_kernel<SWS_OUT_RGB24, NV><<<grid(PairShape<SWS_OUT_RGB24>::band), block, 0, stream>>>(b, dt, col, ngroups, npairs); break;
+    case SWS_OUT_BGR24: sws_vscale_rgb24_pair_kernel<SWS_OUT_BGR24, NV><<<grid(PairShape<SWS_OUT_BGR24>::band), block, 0, stream>>>(b, dt, col, ngroups, npairs); break;
+    case SWS_OUT_RGBA:  sws_vscale_rgb24_pair_kernel<SWS_OUT_RGBA, NV><<<grid(PairShape<SWS_OUT_RGBA>::band), block, 0, stream>>>(b, dt, col, ngroups, npairs); break;
+    case SWS_OUT_BGRA:  sws_vscale_rgb24_pair_kernel<SWS_OUT_BGRA, NV><<<grid(PairShape<SWS_OUT_BGRA>::band), block, 0, stream>>>(b, dt, col, ngroups, npairs); break;
+    case SWS_OUT_ARGB:  sws_vscale_rgb24_pair_kernel<SWS_OUT_ARGB, NV><<<grid(PairShape<SWS_OUT_ARGB>::band), block, 0, stream>>>(b, dt, col, ngroups, npairs); break;
+    default:            sws_vscale_rgb24_pair_kernel<SWS_OUT_ABGR, NV><<<grid(PairShape<SWS_OUT_ABGR>::band), block, 0, stream>>>(b, dt, col, ngroups, npairs); break;
     }
 }
 
@@ -1708,11 +1751,11 @@ static int launch_batch(B200SwsContext *c, cudaStream_t stream, const uint8_t *c
                 const int ng = nv_direct ? p.dstW / 16 : ngroups;
                 SwsFrameArgs bp = b;
                 bp.y0 = pfirst;
-                dim3 block(128), grid(b200_ceil_div(ng, 128), npairs, nf);
-                if (!nv_direct) launch_vscale_pair<0>(p.out.kind, grid, block, stream, bp, c->dt, p.color, ng);
-                else if (p.src_nv == 1) launch_vscale_pair<1>(p.out.kind, grid, block, stream, bp, c->dt, p.color, ng);
-                else launch_vscale_pair<2>(p.out.kind, grid, block, stream, bp, c->dt, p.color, ng);
+                if (!nv_direct) launch_vscale_pair<0>(p.out.kind, ng, npairs, nf, stream, bp, c->dt, p.color);
+                else if (p.src_nv == 1) launch_vscale_pair<1>(p.out.kind, ng, npairs, nf, stream, bp, c->dt, p.color);
+                else launch_vscale_pair<2>(p.out.kind, ng, npairs, nf, stream, bp, c->dt, p.color);
                 B200_LAUNCHED();
+                c->last_path |= 8;
             }
             // the one-line kernel: everything when no pairs were formed, else the lines left over at either end
             const int seg0[2] = { R.dy0, pfirst + 2 * npairs }, segn[2] = { npairs > 0 ? pfirst - R.dy0 : R.ndy, npairs > 0 ? R.dy0 + R.ndy - (pfirst + 2 * npairs) : 0 };

@@ -81,7 +81,8 @@ class SwsContext:
         return list(o)
 
     def last_path(self):
-        """kernels used by the scaled-path launches since the previous call: 1 two passes, 2 fused, 4 fused with the tensor-core horizontal pass"""
+        """kernels used by the launches since the previous call: 1 two passes, 2 fused, 4 fused with the tensor-core horizontal pass (scaled
+        path); 8 the same-size line-pair kernel"""
         return lib().b200_sws_last_path(self._h)
 
     def get_filter(self, which):

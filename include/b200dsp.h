@@ -165,8 +165,9 @@ int  b200_sws_scale_batch_host(B200SwsContext *c, const uint8_t *const src[3], c
                                int64_t dstFrameStride, int nframes);
 /* introspection for tests: same layout as the shim used on the reference (16 ints) */
 int  b200_sws_info(const B200SwsContext *c, int *out16);
-/* diagnostics: which kernels the scaled-path launches since the previous call used (bit 0 two passes through 15-bit line planes,
- * bit 1 fused CUDA-core kernels, bit 2 fused kernels with the tensor-core horizontal pass); reading clears it. */
+/* diagnostics: which kernels the launches since the previous call used (scaled path: bit 0 two passes through 15-bit line planes,
+ * bit 1 fused CUDA-core kernels, bit 2 fused kernels with the tensor-core horizontal pass; same size: bit 3 the line-pair kernel);
+ * reading clears it. */
 int  b200_sws_last_path(B200SwsContext *c);
 /* which: 0 hLum 1 hChr 2 vLum 3 vChr — host copies of the generated filter tables */
 int  b200_sws_get_filter(const B200SwsContext *c, int which, int16_t *filter, int32_t *pos, int cap);

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Time one path quickly on the GPU box: python scripts/quick_bench.py qpel|idct|sws|lut|tx|esa [reps]"""
-import os, sys, time
+import json, os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch
@@ -12,6 +12,17 @@ reps = int(sys.argv[2]) if len(sys.argv) > 2 else 10
 stream = torch.cuda.Stream()
 dev = fb.Device(0, stream=stream.cuda_stream)
 g = torch.Generator(device="cuda"); g.manual_seed(1)
+
+
+def hbm_peak():
+    """the peak bench.py divides by: MEASURED_PEAKS.json hbm_gbs, else the H100 SXM data sheet (3.35 TB/s)"""
+    try:
+        return float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
+    except Exception:
+        return 3350.0
+
+
+PEAK_GBS = hbm_peak()
 
 
 def timed(call, n_units, unit, bytes_per_unit=None):
@@ -27,7 +38,7 @@ def timed(call, n_units, unit, bytes_per_unit=None):
     ms = e0.elapsed_time(e1) / reps
     line = f"{what}: {n_units / ms / 1e6:.3f} G{unit}/s  ({ms:.3f} ms)"
     if bytes_per_unit:
-        line += f"  {n_units * bytes_per_unit / ms / 1e6:.0f} GB/s = {n_units * bytes_per_unit / ms / 1e6 / 6571.9:.3f} of peak"
+        line += f"  {n_units * bytes_per_unit / ms / 1e6:.0f} GB/s = {n_units * bytes_per_unit / ms / 1e6 / PEAK_GBS:.3f} of peak"
     print(line)
 
 

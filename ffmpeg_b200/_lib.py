@@ -186,6 +186,18 @@ class SAOParams(C.Structure):
                 ("eo_class", C.c_int32 * 3), ("offset_val", (C.c_int16 * 5) * 3), ("type_idx", C.c_uint8 * 3)]
 
 
+class HevcIntraOp(C.Structure):
+    """B200HevcIntraOp (include/b200dsp.h), 16 bytes"""
+    _fields_ = [("x", C.c_int32), ("y", C.c_int32), ("log2_size", C.c_uint8), ("mode", C.c_uint8), ("flags", C.c_uint16),
+                ("reserved", C.c_uint8 * 4)]
+
+
+class HEVCPredContext(C.Structure):
+    """B200HEVCPredContext = libavcodec/hevc/pred.h HEVCPredContext"""
+    _fields_ = [("intra_pred", vp * 4), ("pred_planar", vp * 4), ("pred_dc", vp), ("pred_angular", vp * 4), ("ref_filter_3tap", vp * 3),
+                ("ref_filter_strong", vp)]
+
+
 class ProresDSPContext(C.Structure):
     """libavcodec/proresdsp.h:28-35"""
     _fields_ = [("idct_permutation_type", C.c_int), ("idct_permutation", C.c_uint8 * 64),
@@ -303,6 +315,9 @@ PROTOTYPES = {
     "b200_hevc_dsp_init_sao": (C.c_int, [vp, C.c_int]),
     "b200_hevc_sao_plane_device": (C.c_int, [vp, C.c_int, vp, C.c_ssize_t, vp, C.c_ssize_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp,
                                              C.c_int64, vp, C.c_int64, C.c_int]),
+    "b200_hevc_pred_init": (C.c_int, [vp, C.c_int]),
+    "b200_hevc_intra_pred_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_ssize_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64, vp, vp,
+                                                    C.c_ssize_t, C.c_int]),
     "b200_proresdsp_init": (C.c_int, [vp, C.c_int]),
     "b200_prores_idct_put_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, vp, vp, vp, C.c_int]),
     "b200_float_dsp_init": (C.c_int, [vp]),

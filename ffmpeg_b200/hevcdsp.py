@@ -2,12 +2,12 @@
 (libavcodec/hevc/dsp.c:140-196) and the batched device entry b200_hevc_mc_batch_device; the residual members (hevc/dsp.c:198-215) and
 the batched device entry b200_hevc_transform_add_batch_device; the loop-filter members (hevc/dsp.c:237-244) and the plane entry
 b200_hevc_deblock_plane_device; the sample adaptive offset members (hevc/dsp.c:217-228) and the out-of-place plane entry
-b200_hevc_sao_plane_device."""
+b200_hevc_sao_plane_device; HEVCPredContext (hevc/pred.c) and the batched intra prediction entry b200_hevc_intra_pred_batch_device."""
 import ctypes as C
 
 import numpy as np
 
-from ._lib import lib, check, vp, HEVCDSPContext, HevcMcOp, HevcTuOp, HevcDbkSeg, HevcSaoCtb, SAOParams
+from ._lib import lib, check, vp, HEVCDSPContext, HevcMcOp, HevcTuOp, HevcDbkSeg, HevcSaoCtb, SAOParams, HevcIntraOp, HEVCPredContext
 
 UNI, UNI_W, BI, BI_W = range(4)                 # B200HevcMcOp.kind
 OP_DTYPE = np.dtype([("dst_off", "<i8"), ("ref_off", "<i8", 2), ("x", "<i4", 2), ("y", "<i4", 2), ("mx", "u1", 2), ("my", "u1", 2),
@@ -52,6 +52,19 @@ SAO_BAND_FILTER = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_ssi
 SAO_EDGE_FILTER = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_int, C.c_int, C.c_int)
 SAO_EDGE_RESTORE = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_ssize_t, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                C.c_void_p, C.c_void_p, C.c_void_p)
+
+(INTRA_CAND_BL, INTRA_CAND_L, INTRA_CAND_UL, INTRA_CAND_U, INTRA_CAND_UR, INTRA_LUMA, INTRA_SMOOTH,
+ INTRA_STRONG) = (1 << k for k in range(8))     # B200HevcIntraOp.flags
+INTRA_DTYPE = np.dtype([("x", "<i4"), ("y", "<i4"), ("log2_size", "u1"), ("mode", "u1"), ("flags", "<u2"), ("reserved", "u1", 4)])
+assert INTRA_DTYPE.itemsize == C.sizeof(HevcIntraOp) == 16
+
+# HEVCPredContext's member signatures: planar (src, top, left, stride); dc (src, top, left, stride, log2_size, c_idx); angular (src,
+# top, left, stride, c_idx, mode); 3-tap (filtered_left, filtered_top, left, top, size); strong (filtered_top, left, top)
+PRED_PLANAR = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_void_p, C.c_ssize_t)
+PRED_DC = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_int, C.c_int)
+PRED_ANGULAR = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_int, C.c_int)
+REF_FILTER_3TAP = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int)
+REF_FILTER_STRONG = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_void_p)
 
 
 def _dptr(x):
@@ -108,6 +121,23 @@ def hevc_sao_plane_device(device, bit_depth, dst, dst_stride, src, src_stride, w
                                                   height, log2_ctb_size, hshift, vshift, vp(_dptr(ctb)), ctb_stride,
                                                   None if keep is None else vp(_dptr(keep)), keep_stride, log2_min_pu_size),
                  "hevc_sao_plane_device")
+
+
+def ff_hevc_pred_init(bit_depth=8):
+    """a HEVCPredContext with every member ff_hevc_pred_init fills except intra_pred[] (NULL): HOST pointers"""
+    c = HEVCPredContext()
+    check(lib().b200_hevc_pred_init(C.byref(c), bit_depth), "ff_hevc_pred_init")
+    return c
+
+
+def hevc_intra_pred_batch_device(device, bit_depth, pix, stride, width, height, hshift, vshift, nops, ops, intra_map=None, map_stride=0,
+                                 log2_min_pu_size=0):
+    """one call of independent intra TUs on one plane (device): pix a sample tensor, stride in bytes, width / height the LUMA picture
+    size; ops = INTRA_DTYPE records (a uint8 tensor of nops * 16 bytes); intra_map None (constrained_intra_pred_flag 0) or a uint8
+    tensor, one byte per luma min PU"""
+    return check(lib().b200_hevc_intra_pred_batch_device(device.handle, bit_depth, vp(_dptr(pix)), stride, width, height, hshift, vshift, nops,
+                                                         vp(_dptr(ops)), None if intra_map is None else vp(_dptr(intra_map)), map_stride,
+                                                         log2_min_pu_size), "hevc_intra_pred_batch_device")
 
 
 def hevc_mc_batch_device(device, bit_depth, epel, nops, ops, dst, dst_stride, ref, ref_stride, pic_w, pic_h):

@@ -587,6 +587,73 @@ int  b200_hevc_sao_plane_device(B200Device *dev, int bit_depth, uint8_t *dst, pt
                                 int width, int height, int log2_ctb_size, int hshift, int vshift, const B200HevcSaoCtb *ctb,
                                 int64_t ctb_stride, const uint8_t *keep, int64_t keep_stride, int log2_min_pu_size);
 
+/* HEVC intra prediction: HEVCPredContext (libavcodec/hevc/pred.h) with the reference's layout and function types. */
+struct HEVCLocalContext;
+struct HEVCPPS;
+typedef struct B200HEVCPredContext {
+    void (*intra_pred[4])(struct HEVCLocalContext *lc, const struct HEVCPPS *pps, int x0, int y0, int c_idx);
+    void (*pred_planar[4])(uint8_t *src, const uint8_t *top, const uint8_t *left, ptrdiff_t stride);
+    void (*pred_dc)(uint8_t *src, const uint8_t *top, const uint8_t *left, ptrdiff_t stride, int log2_size, int c_idx);
+    void (*pred_angular[4])(uint8_t *src, const uint8_t *top, const uint8_t *left, ptrdiff_t stride, int c_idx, int mode);
+    void (*ref_filter_3tap[3])(uint8_t *filtered_left, uint8_t *filtered_top, const uint8_t *left, const uint8_t *top, int size);
+    void (*ref_filter_strong)(uint8_t *filtered_top, uint8_t *left, const uint8_t *top);
+} B200HEVCPredContext;
+
+/* Fills every member of a B200HEVCPredContext that ff_hevc_pred_init fills (hevc/pred.c) except intra_pred[], which takes decoder
+ * structs and is left NULL: the reference's own intra_pred calls everything else through s->hpc, so a decoder copies these members
+ * over its HEVCPredContext.  HOST pointers, the reference's signatures, samples uint8 at 8 bit and uint16 above, and strides in SAMPLES
+ * (intra_pred passes linesize / sizeof(pixel)):
+ *   pred_planar[log2_size - 2], pred_dc, pred_angular[log2_size - 2]
+ *                     stage the samples the reference function reads (planar top[0..size], left[0..size]; DC top[0..size - 1],
+ *                     left[0..size - 1]; angular top[-1..2 * size - 1], left[-1..2 * size - 1]) onto the device, run the prediction stage
+ *                     of the batch kernel and copy the size x size block back.  An angular mode outside 2..34 or a pred_dc log2_size
+ *                     outside 2..5 writes nothing and records the reason (b200_last_error()).
+ *   ref_filter_3tap[0..2] (one function), ref_filter_strong
+ *                     run on the host (no launch) through the kernel's own filter functions, with the reference's writes:
+ *                     the 3-tap filter writes filtered_left / filtered_top [-1..2 * size - 1]; the strong filter writes
+ *                     filtered_top[-1..63] and left[0..62] in place.
+ * Returns 0; B200_EINVAL for hpc == NULL; B200_ENOSYS for depths other than 8, 9, 10 and 12 (the reference installs its 8-bit functions
+ * for them, but its decoder refuses such streams first); B200_ENODEV. */
+int  b200_hevc_pred_init(B200HEVCPredContext *hpc, int bit_depth);
+
+/* One transform block of b200_hevc_intra_pred_batch_device: what intra_pred (hevc/pred_template.c) reads for it at the call.
+ * CAND_* = the five cand_* values as intra_pred has them after its z-scan checks (pred_template.c:154-158), before constrained
+ * intra prediction; LUMA = (c_idx == 0); SMOOTH = !sps->intra_smoothing_disabled && (c_idx == 0 || chroma_format_idc == 3);
+ * STRONG = sps->strong_intra_smoothing_enabled.  Unknown flag bits and `reserved` are ignored. */
+enum {
+    B200_HEVC_INTRA_CAND_BL = 1, B200_HEVC_INTRA_CAND_L = 2, B200_HEVC_INTRA_CAND_UL = 4, B200_HEVC_INTRA_CAND_U = 8,
+    B200_HEVC_INTRA_CAND_UR = 16, B200_HEVC_INTRA_LUMA = 32, B200_HEVC_INTRA_SMOOTH = 64, B200_HEVC_INTRA_STRONG = 128
+};
+typedef struct B200HevcIntraOp {
+    int32_t  x, y;        /* the TU's top-left in plane samples (x0 >> hshift, y0 >> vshift) */
+    uint8_t  log2_size;   /* 2..5 */
+    uint8_t  mode;        /* 0 planar, 1 DC, 2..34 angular: the mode intra_pred reads (tu.intra_pred_mode / _c, after the 4:2:2 remap) */
+    uint16_t flags;       /* B200_HEVC_INTRA_* */
+    uint8_t  reserved[4];
+} B200HevcIntraOp;
+#ifdef __cplusplus
+static_assert(sizeof(B200HevcIntraOp) == 16, "B200HevcIntraOp is 16 bytes");
+#else
+_Static_assert(sizeof(B200HevcIntraOp) == 16, "B200HevcIntraOp is 16 bytes");
+#endif
+/* Batched HEVC intra prediction of one plane, DEVICE pointers, asynchronous on the device's stream: each op's block becomes what
+ * intra_pred writes for that TU given the plane as it is at the call.  pix / stride: the component plane (bytes); width / height the
+ * LUMA picture size (sps->width / height) and hshift / vshift the component's subsampling, so the plane is (width >> hshift) x
+ * (height >> vshift).  intra_map: NULL when constrained_intra_pred_flag is 0; else one byte per luma min PU (1 << log2_min_pu_size
+ * luma samples, (width >> log2_min_pu_size) x (height >> log2_min_pu_size) entries at map_stride bytes per row), non-zero where
+ * pred_flag == PF_INTRA, and the constrained-intra branch (pred_template.c:165-295) is reproduced with its quirks.  Where that branch
+ * reads a map entry outside the picture's map (the row above the picture, for a block on the top row whose left neighbours are all
+ * inter), the kernel reads "not intra" and never reads outside the map.
+ * The ops of one call must be independent: no op may write samples that another op of the call reads or writes; a decoder issues
+ * one call per dependency level.  An op whose log2_size or mode is out of range, or whose block or neighbours (the row above when a
+ * CAND_UL / U / UR flag is set, the column to the left when a CAND_BL / L / UL flag is set) fall outside the plane, writes nothing.
+ * Offsets are 64-bit.  Returns 0, or B200_EINVAL (launching nothing) for NULL pix or ops, pix not aligned to a sample or ops not aligned to 16 bytes, an intra_map with map_stride <
+ * (width >> log2_min_pu_size) or log2_min_pu_size outside 2..6, nops < 0, a depth other than 8, 9, 10 or 12, width or height below 1,
+ * a shift outside {0, 1}, a stride shorter than a plane row, or an odd stride or pix above 8 bit; nops == 0 returns 0. */
+int  b200_hevc_intra_pred_batch_device(B200Device *dev, int bit_depth, uint8_t *pix, ptrdiff_t stride, int width, int height, int hshift,
+                                       int vshift, int64_t nops, const B200HevcIntraOp *ops, const uint8_t *intra_map, ptrdiff_t map_stride,
+                                       int log2_min_pu_size);
+
 /* mpegvideo inverse quantisers: the members of MPVUnquantDSPContext (libavcodec/mpegvideo_unquantize.h:31-44) as
  * ff_mpv_unquantize_init() installs them (libavcodec/mpegvideo_unquantize.c:50-290), i.e. what runs in front of the IDCT in
  * mpv_reconstruct_mb's put_dct / add_dequant_dct (libavcodec/mpegvideo_dec.c).  The reference functions take the whole

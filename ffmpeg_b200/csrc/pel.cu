@@ -179,7 +179,7 @@ qpel_kernel(long long n, const uint8_t *op, uint8_t *dst, const int64_t *dst_off
             issue_window(ring0 + (ka & (QD - 1)) * RING_SLOT, srcb + (uintptr_t)sa, (16 >> ((oa >> 1) & 3)) + 5, lane, ka < QK && oa >= 0);
         }
 
-        const int avg = o & 1, size = 16 >> ((o >> 1) & 3), qx = (o >> 3) & 3, qy = (o >> 5) & 3;
+        const int avg = o & 1, sidx = (o >> 1) & 3, size = 16 >> sidx, qx = (o >> 3) & 3, qy = (o >> 5) & 3;
         uint8_t *dp = dst + doff0;
         const int wdim = size + 5;
         int npx = 8, segs = 2, y = lane >> 1, x0 = (lane & 1) << 3;
@@ -188,6 +188,9 @@ qpel_kernel(long long n, const uint8_t *op, uint8_t *dst, const int64_t *dst_off
             npx = size < 8 ? size : 8; segs = 1;
             mine = lane < size; y = lane; x0 = 0;
         }
+        // size index 3 names no table of the reference: the op writes nothing.  It still waits for its window (issued above like any
+        // other), so that the ring slot is free before the look-ahead of a later op is copied into it.
+        if (sidx == 3) mine = false;
         uint8_t *d = dp + (long long)y * stride + x0;
         const bool vec = npx == 8 && ((reinterpret_cast<uintptr_t>(d)) & 7) == 0;
         uint2 pv = make_uint2(0, 0);
@@ -280,6 +283,7 @@ hpel_kernel(long long n, const uint8_t *op, const uint8_t *hh, uint8_t *dst, con
     const int lane = threadIdx.x & 31;
     const int o = op[i], h = hh[i];
     const int tab = o & 3, sidx = (o >> 2) & 3, xy = (o >> 4) & 3, w = 16 >> sidx;
+    if ((tab == 2 && sidx >= 2) || (tab == 3 && sidx >= 1)) return;   // entries the reference leaves NULL (hpeldsp.c:337-352): write nothing
     const int no_rnd = tab >= 2;
     const int avg = (tab & 1) && !(sidx == 3 && xy == 3);        // avg_pixels2_xy2 stores without averaging (hpeldsp.c:134-166)
     const uint8_t *sp = src + src_off[i];
@@ -356,7 +360,8 @@ chroma_kernel(long long n, const uint8_t *op, const uint8_t *hh, const uint8_t *
     bool valid[CK];
 #pragma unroll
     for (int j = 0; j < CK; j++) {
-        o[j] = nmeta[j] & 255; h[j] = (nmeta[j] >> 8) & 255; pq[j] = (nmeta[j] >> 16) & 255; valid[j] = (nmeta[j] >> 24) & 1;
+        o[j] = nmeta[j] & 255; h[j] = (nmeta[j] >> 8) & 255; pq[j] = (nmeta[j] >> 16) & 255;
+        valid[j] = ((nmeta[j] >> 24) & 1) && ((o[j] >> 1) & 3) != 3;                  // width index 3 is the reference's NULL entry: write nothing
         so[j] = nso[j]; dof[j] = ndof[j];
     }
     fetch(b + nwarps);

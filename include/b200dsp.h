@@ -770,7 +770,8 @@ typedef struct B200H264WeightContext {
 int  b200_h264_weight_init(B200H264WeightContext *c, int bit_depth);            /* 8, or 9 / 10 / 12 / 14 (uint16 samples, stride in bytes) */
 /* batched, DEVICE pointers.  params: 4 int32 per block (16-byte aligned array): [0] = width index | height << 8 | log2_denom << 16,
  * [1] = weight (the destination weight for biweight), [2] = source weight (biweight), [3] = offset.  src == NULL: weight
- * (in place on dst + dst_off[i]); src != NULL: biweight of dst + dst_off[i] with src + src_off[i].  One stride for both. */
+ * (in place on dst + dst_off[i]); src != NULL: biweight of dst + dst_off[i] with src + src_off[i].  One stride for both.
+ * Destination blocks of one call must not overlap each other, and no op may read samples that another op of the same call writes. */
 int  b200_h264_weight_batch_device(B200Device *dev, int64_t n, const int32_t *params, uint8_t *dst, const int64_t *dst_off,
                                    const uint8_t *src, const int64_t *src_off, ptrdiff_t stride);
 /* the same for 9 / 10 / 12 / 14 bit samples (uint16): offsets and stride in BYTES (even) */
@@ -890,7 +891,12 @@ int  b200_hpeldsp_init(B200HpelDSPContext *c, int flags);
  * dst + dst_off[i] (same stride for both, like the reference's single stride argument).
  * qpel op byte: bit0 avg, bits1-2 size index (0:16,1:8,2:4), bits3-6 position x+4*y.
  * hpel op byte: bits0-1 table (0 put, 1 avg, 2 put_no_rnd, 3 avg_no_rnd), bits2-3 size index (0:16,1:8,2:4,3:2),
- * bits4-5 xy; h[i] = block height. Destination blocks of one call must not overlap each other.
+ * bits4-5 xy; h[i] = block height. Destination blocks of one call must not overlap each other, and no op may read samples that
+ * another op of the same call writes (ops run in any order, and the qpel kernel loads windows several ops ahead).
+ * An op code naming a table entry the reference leaves NULL writes nothing: qpel size index 3; hpel put_no_rnd (table 2) at size
+ * index 2 or 3, avg_no_rnd (table 3) at size index 1, 2 or 3.  n == 0 returns 0; NULL pointers or n < 0 return B200_EINVAL.
+ * hpel writes exactly h rows for every h; the reference's xy2 functions step two rows at a time, so at an odd h (outside the
+ * heights hpeldsp.h allows) they write one row more.
  * The qpel kernel may load the whole (size+5)^2 window of an operation whatever its position (unused taps never reach the
  * result): keep the planes edge-padded by 3 pixels / rows, as H.264 reference frames are (h264_mb.c mc_dir_part). */
 int  b200_h264qpel_batch_device(B200Device *dev, int64_t n, const uint8_t *op, uint8_t *dst, const int64_t *dst_off,
@@ -917,7 +923,9 @@ typedef struct B200H264ChromaContext {
 } B200H264ChromaContext;
 int  b200_h264chroma_init(B200H264ChromaContext *c, int bit_depth);   /* 9 ... 16: the uint16 tables (h264chroma.c:45-50); else 8 bit */
 /* batched, DEVICE pointers.  op byte: bit0 avg, bits1-2 width index (0:8,1:4,2:2); h[i] = rows; xy[i] = x | y << 3.
- * Like the reference, x == 0 never reads the column right of the block and y == 0 never reads the row below it. */
+ * Like the reference, x == 0 never reads the column right of the block and y == 0 never reads the row below it.  Destination blocks
+ * of one call must not overlap each other, and no op may read samples that another op of the same call writes.  Width index 3 (the
+ * reference's NULL entry) writes nothing.  n == 0 returns 0; NULL pointers or n < 0 return B200_EINVAL. */
 int  b200_h264chroma_batch_device(B200Device *dev, int64_t n, const uint8_t *op, const uint8_t *h, const uint8_t *xy,
                                   uint8_t *dst, const int64_t *dst_off, const uint8_t *src, const int64_t *src_off,
                                   ptrdiff_t stride);

@@ -270,6 +270,13 @@ int orc_h264chroma(int avg, int idx, uint8_t *dst, const uint8_t *src, ptrdiff_t
     return 0;
 }
 
+void orc_h264chroma_batch(int64_t n, const uint8_t *op, const uint8_t *h, const uint8_t *xy, uint8_t *dstbase, const int64_t *dst_off,
+                          const uint8_t *srcbase, const int64_t *src_off, ptrdiff_t stride)
+{
+    for (int64_t i = 0; i < n; i++)
+        orc_h264chroma(op[i] & 1, (op[i] >> 1) & 3, dstbase + dst_off[i], srcbase + src_off[i], stride, h[i], xy[i] & 7, (xy[i] >> 3) & 7);
+}
+
 void orc_emulated_edge_mc(uint8_t *buf, const uint8_t *src, ptrdiff_t buf_linesize, ptrdiff_t src_linesize,
                           int block_w, int block_h, int src_x, int src_y, int w, int h)
 {

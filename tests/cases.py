@@ -384,3 +384,103 @@ def esa_expected(lib_fn, row, curbuf, refbuf, workers=None):
     with ThreadPoolExecutor(workers or os.cpu_count() or 1) as ex:
         list(ex.map(run, tasks))
     return mv, cost
+
+
+# ---------------------------------------------------------------- 8-bit motion compensation (csrc/pel.cu, csrc/h264weight.cu)
+# Plane layouts of tests/test_pel_paths_gpu.py and tests/test_oracle_pel_layouts.py.  A case's source and destination pictures have
+# the same width and share one stride, like a decoder's reference and current pictures.  Each plane has an allocation of its own with
+# PEL_SLACK bytes before its first and after its last sample: the kernels load the aligned 16-byte (qpel) or 8-byte (chroma) words
+# around the bytes they need, so those words stay inside the allocation whatever the alignment of the base.
+#   A  stride a multiple of 64, plane bases 64-byte aligned, block offsets as a decoder makes them (x a multiple of the block width)
+#   B  odd stride (width + 37 or + 38): the rows of one block all have different alignments; source base at +3, destination base at
+#      +10, destination x jittered by 0..15, so that 8- and 16-wide qpel blocks take both the 8-byte and the byte store path
+#   C  the picture of A stored bottom-up: negative stride, the base (picture row 0) is the last row in memory and the offsets
+#      y * stride + x are negative
+PEL_SLACK = 64
+PEL_LAYOUTS = ("A", "B", "C")
+
+
+class PelPlane:
+    """One w x h picture in a layout.  buf: the whole allocation (uint8, seeded noise outside the picture); base: offset of sample
+    (0, 0) in buf; stride: bytes from one picture row to the next (negative in layout C).  Offsets handed to the kernels are relative
+    to base: off(x, y) = y * stride + x."""
+
+    def __init__(self, layout, w, h, role, seed):
+        if layout == "B":
+            pitch, mis = (w + 37 if (w + 37) % 2 else w + 38), (3 if role == "src" else 10)
+        else:
+            pitch, mis = (w + 63) // 64 * 64, 0
+        self.layout, self.w, self.h = layout, w, h
+        self.stride = -pitch if layout == "C" else pitch
+        self.base = PEL_SLACK + mis + ((h - 1) * pitch if layout == "C" else 0)
+        size = PEL_SLACK + mis + (h - 1) * pitch + w + PEL_SLACK
+        self.buf = np.random.default_rng(seed).integers(0, 256, (size + 15) // 16 * 16, dtype=np.uint8)
+
+    def off(self, x, y):
+        return y * self.stride + x
+
+    def fill(self, pic):
+        for y in range(self.h):
+            o = self.base + y * self.stride
+            self.buf[o:o + self.w] = pic[y]
+        return self
+
+    def picture(self):
+        return np.stack([self.buf[self.base + y * self.stride:][:self.w] for y in range(self.h)])
+
+
+def pel_picture(kind, h, w, seed):
+    """'random', or 'extremes': 0 / 255 patterns in 24 x 24 tiles, cycling through vertical and horizontal stripes of periods 2, 3
+    and 6, a checkerboard, flat 0 and flat 255 -- they drive the 6-tap sums, the centre sample and the weighted sums to both clip
+    limits"""
+    if kind == "random":
+        return np.random.default_rng(seed).integers(0, 256, (h, w), dtype=np.uint8)
+    yy, xx = np.mgrid[0:h, 0:w]
+    pats = [xx % p < p // 2 for p in (2, 3, 6)] + [yy % p < p // 2 for p in (2, 3, 6)] + [(xx + yy) % 2 == 0, xx < 0, xx >= 0]
+    tile = ((yy // 24) * 5 + xx // 24 + seed) % len(pats)
+    return (np.select([tile == i for i in range(len(pats))], pats) * 255).astype(np.uint8)
+
+
+def pel_layout_case(layout, kind, blocks, seed, src_h=96, margin=(0, 0), cell=(16, 16), phases=None, cols=64):
+    """Source and destination planes and per-op offsets for a list of (block width, block height).  Op i reads its block at a seeded
+    position of the source picture, `margin` = (samples before, samples after) it may read around the block staying inside the
+    picture; with `phases`, the address of its sample (0, 0) is phases[i] mod 16.  It writes a block of its own cell
+    (cell = (width, height)) of the destination picture, `cols` cells per row, at an x jitter the layout allows.
+    Returns dict(src=PelPlane, dst=PelPlane, soff=int64[n], doff=int64[n])."""
+    rng = np.random.default_rng(seed)
+    n = len(blocks)
+    bw, bh = (np.array([b[k] for b in blocks], np.int64).reshape(n) for k in (0, 1))
+    cw, ch = cell
+    w = cols * cw
+    rows = max(1, (n + cols - 1) // cols)
+    src = PelPlane(layout, w, src_h, "src", seed + 1).fill(pel_picture(kind, src_h, w, seed + 2))
+    dst = PelPlane(layout, w, rows * ch, "dst", seed + 3).fill(pel_picture("random", rows * ch, w, seed + 4))
+    lo, hi = margin
+    sy = rng.integers(lo, src_h - bh - hi + 1)
+    sx = rng.integers(lo, w - bw - hi - 15 + 1)
+    if phases is not None:
+        sx = sx + (np.asarray(phases, np.int64) - (src.base + src.off(sx, sy))) % 16
+    if layout == "B":
+        jx = rng.integers(0, np.minimum(15, cw - bw) + 1)
+    else:
+        jx = bw * rng.integers(0, (cw - bw) // bw + 1)
+    i = np.arange(n, dtype=np.int64)
+    return dict(src=src, dst=dst, soff=src.off(sx, sy).astype(np.int64), doff=dst.off((i % cols) * cw + jx, (i // cols) * ch).astype(np.int64))
+
+
+# the (table, size index) pairs of HpelDSPContext the reference fills (hpeldsp.c:337-352): put / avg at 16, 8, 4 and 2 wide,
+# put_no_rnd at 16 and 8, avg_no_rnd at 16; the other pairs are NULL there
+HPEL_DEFINED = [(0, s) for s in range(4)] + [(1, s) for s in range(4)] + [(2, 0), (2, 1), (3, 0)]
+HPEL_UNDEFINED = [(2, 2), (2, 3), (3, 1), (3, 2), (3, 3)]
+
+EDGE_SIZES = ((1, 1), (80, 80), (71, 71), (33, 5), (5, 33), (21, 21), (9, 9), (64, 17), (17, 64))
+
+
+def edge_windows(w, h):
+    """(block_w, block_h, src_x, src_y): windows wholly outside each side and corner, straddling each border, and inside"""
+    out = []
+    for bw, bh in EDGE_SIZES:
+        xs = sorted({-bw - 7, -bw, -bw + 1, -(bw // 2), 0, max(0, (w - bw) // 2), w - bw, w - 1, w, w + 9})
+        ys = sorted({-bh - 7, -bh, -bh + 1, -(bh // 2), 0, max(0, (h - bh) // 2), h - bh, h - 1, h, h + 9})
+        out += [(bw, bh, x, y) for x in xs for y in ys]
+    return out

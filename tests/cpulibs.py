@@ -77,6 +77,9 @@ def oracle():
             L.orc_h264_biweight.restype = None
         if hasattr(L, "orc_h264chroma"):
             L.orc_h264chroma.argtypes = [C.c_int, C.c_int, u8p, u8p, C.c_ssize_t, C.c_int, C.c_int, C.c_int]
+            L.orc_h264chroma_batch.argtypes = [C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_ssize_t]
+            L.orc_h264chroma_batch.restype = None
         if hasattr(L, "orc_tx_open"):
             L.orc_tx_open.restype = C.c_void_p
             L.orc_tx_open.argtypes = [C.c_int, C.c_int, C.c_int, C.c_float, C.c_uint]
@@ -94,14 +97,14 @@ def have_ref():
 # reference's results, keyed by the test's module file, name (with parameters) and the block's position in the test (the tests'
 # inputs are seeded, so the sequence is fixed).  With the reference built and FFDSP_RECORD_REF=1 in the environment, the digests are (re)written at exit.
 REF_DIGESTS = os.path.join(ROOT, "tests", "golden", "ref_digests.json")
-_digests = None
+_digests = {}                                                       # digest file -> its stored digests
 _blocks = {}
 
 
-def _write_digests():
+def _write_digests(path):
     import json
-    with open(REF_DIGESTS, "w") as f:
-        json.dump(_digests, f, indent=0, sort_keys=True)
+    with open(path, "w") as f:
+        json.dump(_digests[path], f, indent=0, sort_keys=True)
         f.write("\n")
 
 
@@ -109,10 +112,12 @@ class RefCheck:
     """with RefCheck() as rc: assert rc.same(ours, lambda: theirs) -- `ours` is an array, a number or a sequence of them.
     Where oracle/_ref/libffref.so is built, every same() compares with the reference's result at once and the block's end also
     checks the stored digest (so a stale file shows here too); elsewhere same() only accumulates `ours`, and the block's end
-    compares the accumulated digest with the stored one."""
+    compares the accumulated digest with the stored one.  `digests` names the file that keeps them (default REF_DIGESTS)."""
+
+    def __init__(self, digests=REF_DIGESTS):
+        self.path = digests
 
     def __enter__(self):
-        global _digests
         import hashlib
         import json
         nodeid = os.environ.get("PYTEST_CURRENT_TEST", "?").rsplit(" (", 1)[0]
@@ -121,12 +126,13 @@ class RefCheck:
         k = _blocks[test] = _blocks.get(test, -1) + 1
         self.key, self.h = f"{test}#{k}", hashlib.sha256()
         self.live, self.record = have_ref(), have_ref() and os.environ.get("FFDSP_RECORD_REF") == "1"
-        if _digests is None:
-            _digests = json.load(open(REF_DIGESTS)) if os.path.exists(REF_DIGESTS) else {}
+        if self.path not in _digests:
+            _digests[self.path] = json.load(open(self.path)) if os.path.exists(self.path) else {}
             if self.record:
                 import atexit
-                atexit.register(_write_digests)
-        assert self.live or self.key in _digests, f"no stored reference result for {self.key} ({REF_DIGESTS})"
+                atexit.register(_write_digests, self.path)
+        self.stored = _digests[self.path]
+        assert self.live or self.key in self.stored, f"no stored reference result for {self.key} ({self.path})"
         return self
 
     def _add(self, v):
@@ -151,10 +157,10 @@ class RefCheck:
         if typ is not None:
             return False
         if self.record:
-            _digests[self.key] = self.h.hexdigest()[:32]
+            self.stored[self.key] = self.h.hexdigest()[:32]
         else:
-            assert self.key in _digests, f"no stored reference result for {self.key} ({REF_DIGESTS})"
-            assert self.h.hexdigest()[:32] == _digests[self.key], f"differs from the stored reference results ({self.key})"
+            assert self.key in self.stored, f"no stored reference result for {self.key} ({self.path})"
+            assert self.h.hexdigest()[:32] == self.stored[self.key], f"differs from the stored reference results ({self.key})"
         return False
 
 

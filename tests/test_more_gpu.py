@@ -137,65 +137,6 @@ def test_pel_pointer_tables_golden(device):
     assert not hp.put_no_rnd_pixels_tab[2][0]                  # sizes the reference leaves empty stay NULL
 
 
-def test_qpel_batch_vs_oracle(device):
-    """A macroblock-stream like BASELINE config 3: random quarter-pel positions, put/avg and sizes over a frame."""
-    import torch
-    from ffmpeg_b200 import pel
-    O = cl.oracle()
-    rng = np.random.default_rng(12)
-    W, H = 640, 368
-    ref_ = rng.integers(0, 256, (H, W), dtype=np.uint8)
-    dst0 = rng.integers(0, 256, (H, W), dtype=np.uint8)
-    ops, doffs, soffs = [], [], []
-    for by in range(1, H // 16 - 1):
-        for bx in range(1, W // 16 - 1):
-            size_idx = int(rng.integers(0, 3))
-            op = pel.qpel_op(int(rng.integers(0, 2)), size_idx, int(rng.integers(0, 16)))
-            dx, dy = (int(v) for v in rng.integers(-10, 11, 2))
-            ops.append(op); doffs.append(by * 16 * W + bx * 16); soffs.append((by * 16 + dy) * W + bx * 16 + dx)
-    n = len(ops)
-    ops_a, do_a, so_a = np.array(ops, np.uint8), np.array(doffs, np.int64), np.array(soffs, np.int64)
-    exp = dst0.copy()
-    for op, do, so in zip(ops, doffs, soffs):
-        O.orc_h264qpel(op & 1, (op >> 1) & 3, (op >> 3) & 15, C.cast(exp.ctypes.data + do, cl.u8p), C.cast(ref_.ctypes.data + so, cl.u8p), W)
-    with on_stream(device):
-        d_ops, d_do, d_so = torch.from_numpy(ops_a).cuda(), torch.from_numpy(do_a).cuda(), torch.from_numpy(so_a).cuda()
-        d_dst, d_src = torch.from_numpy(dst0).cuda(), torch.from_numpy(ref_).cuda()
-        pel.h264qpel_batch_device(device, n, d_ops, d_dst, d_do, d_src, d_so, W)
-        device.sync()
-        got = d_dst.cpu().numpy()
-    assert np.array_equal(got, exp), int((got != exp).sum())
-
-
-def test_hpel_batch_vs_oracle(device):
-    import torch
-    from ffmpeg_b200 import pel
-    O = cl.oracle()
-    rng = np.random.default_rng(13)
-    W, H = 320, 192
-    ref_ = rng.integers(0, 256, (H, W), dtype=np.uint8)
-    dst0 = rng.integers(0, 256, (H, W), dtype=np.uint8)
-    ops, hs, doffs, soffs = [], [], [], []
-    for by in range(1, H // 16 - 1):
-        for bx in range(1, W // 16 - 1):
-            tab = int(rng.integers(0, 4))
-            sidx = 0 if tab == 3 else int(rng.integers(0, 2)) if tab == 2 else int(rng.integers(0, 4))
-            h = int(rng.choice([4, 8, 16] if sidx < 2 else [2, 4, 8]))
-            ops.append(pel.hpel_op(tab, sidx, int(rng.integers(0, 4)))); hs.append(h)
-            dx, dy = (int(v) for v in rng.integers(-8, 9, 2))
-            doffs.append(by * 16 * W + bx * 16); soffs.append((by * 16 + dy) * W + bx * 16 + dx)
-    exp = dst0.copy()
-    for op, h, do, so in zip(ops, hs, doffs, soffs):
-        assert O.orc_hpel(op & 3, (op >> 2) & 3, (op >> 4) & 3, C.cast(exp.ctypes.data + do, cl.u8p), C.cast(ref_.ctypes.data + so, cl.u8p), W, h) == 0
-    with on_stream(device):
-        t = lambda a, dt: torch.from_numpy(np.array(a, dt)).cuda()
-        d_dst, d_src = torch.from_numpy(dst0).cuda(), torch.from_numpy(ref_).cuda()
-        pel.hpel_batch_device(device, len(ops), t(ops, np.uint8), t(hs, np.uint8), d_dst, t(doffs, np.int64), d_src, t(soffs, np.int64), W)
-        device.sync()
-        got = d_dst.cpu().numpy()
-    assert np.array_equal(got, exp), int((got != exp).sum())
-
-
 def test_h264chroma_pointer_table_golden(device):
     """H264ChromaContext drop-in (host pointers): every phase / width / height of chroma.npz, guard pixels untouched."""
     from ffmpeg_b200 import pel
@@ -216,37 +157,6 @@ def test_h264chroma_pointer_table_golden(device):
             assert np.array_equal(o[8:24, 8:16], g[key][xy]), (key, xy)
             assert np.array_equal(o[:8], dst0[:8]) and np.array_equal(o[8 + h:], dst0[8 + h:]) and np.array_equal(o[:, 16:], dst0[:, 16:]), key
     assert pel.ff_h264chroma_init(10).put_h264_chroma_pixels_tab[0]        # the 16-bit tables (test_h264chroma_and_edge_hbd)
-
-
-def test_h264chroma_batch_vs_oracle(device):
-    """Chroma half of a 4:2:0 macroblock stream: random eighth-pel phases, widths, heights, unaligned offsets."""
-    import torch
-    from ffmpeg_b200 import pel
-    O = cl.oracle()
-    rng = np.random.default_rng(14)
-    W, H = 336, 208
-    ref_ = rng.integers(0, 256, (H, W), dtype=np.uint8)
-    dst0 = rng.integers(0, 256, (H, W), dtype=np.uint8)
-    ops, hs, xys, doffs, soffs = [], [], [], [], []
-    for by in range(1, H // 16 - 1):
-        for bx in range(1, W // 16 - 1):
-            idx = int(rng.integers(0, 3))
-            ops.append(pel.chroma_op(int(rng.integers(0, 2)), idx))
-            hs.append(int(rng.choice(((4, 8, 16), (2, 4, 8), (2, 4))[idx])))
-            xys.append(int(rng.integers(0, 64)))
-            dx, dy, jx = int(rng.integers(-8, 9)), int(rng.integers(-8, 9)), int(rng.integers(0, 8))
-            doffs.append(by * 16 * W + bx * 16 + jx); soffs.append((by * 16 + dy) * W + bx * 16 + dx)
-    exp = dst0.copy()
-    for op, h, xy, do, so in zip(ops, hs, xys, doffs, soffs):
-        assert O.orc_h264chroma(op & 1, op >> 1, C.cast(exp.ctypes.data + do, cl.u8p), C.cast(ref_.ctypes.data + so, cl.u8p), W, h, xy & 7, xy >> 3) == 0
-    with on_stream(device):
-        t = lambda a, dt: torch.from_numpy(np.array(a, dt)).cuda()
-        d_dst, d_src = torch.from_numpy(dst0).cuda(), torch.from_numpy(ref_).cuda()
-        pel.h264chroma_batch_device(device, len(ops), t(ops, np.uint8), t(hs, np.uint8), t(xys, np.uint8), d_dst, t(doffs, np.int64),
-                                    d_src, t(soffs, np.int64), W)
-        device.sync()
-        got = d_dst.cpu().numpy()
-    assert np.array_equal(got, exp), int((got != exp).sum())
 
 
 def test_h264chroma_no_reads_past_block_when_phase_zero(device):
@@ -294,35 +204,6 @@ def test_emulated_edge_mc_pointer_table_golden(device):
     assert pel.ff_videodsp_init(10).emulated_edge_mc                         # the 16-bit template (test_h264chroma_and_edge_hbd)
 
 
-def test_emulated_edge_mc_batch_vs_oracle(device):
-    """Windows hanging over every border of several frames in one call (the mc_dir_part case: 21x21 luma, 9x9 chroma)."""
-    import torch
-    from ffmpeg_b200 import pel
-    O = cl.oracle()
-    rng = np.random.default_rng(16)
-    NF, W, H, LS = 3, 100, 60, 112
-    pics = rng.integers(0, 256, (NF, H, LS), dtype=np.uint8)
-    n = 600
-    geom = np.zeros((n, 4), np.int32)
-    geom[:, 0] = rng.choice([9, 21, 5, 16], n); geom[:, 1] = rng.choice([9, 21, 5, 16], n)
-    geom[:, 2] = rng.integers(-30, W + 10, n); geom[:, 3] = rng.integers(-30, H + 10, n)
-    fr = rng.integers(0, NF, n)
-    origin = (fr * H * LS).astype(np.int64)
-    BLS = 32
-    boff = (np.arange(n) * 24 * BLS).astype(np.int64)
-    exp = np.full((n * 24, BLS), 0x33, np.uint8)
-    for i in range(n):
-        bw, bh, sx, sy = (int(v) for v in geom[i])
-        O.orc_emulated_edge_mc(C.cast(exp.ctypes.data + int(boff[i]), cl.u8p), pics[fr[i]].ctypes.data + sy * LS + sx, BLS, LS, bw, bh, sx, sy, W, H)
-    with on_stream(device):
-        d_buf = torch.full((n * 24, BLS), 0x33, dtype=torch.uint8, device="cuda")
-        pel.emulated_edge_mc_batch_device(device, n, d_buf, torch.from_numpy(boff).cuda(), BLS, torch.from_numpy(pics).cuda(),
-                                          torch.from_numpy(origin).cuda(), LS, torch.from_numpy(geom).cuda(), W, H)
-        device.sync()
-        got = d_buf.cpu().numpy()
-    assert np.array_equal(got, exp), int((got != exp).sum())
-
-
 def test_h264_weight_pointer_table_golden(device):
     from ffmpeg_b200 import pel
     g = np.load(os.path.join(G, "h264weight.npz"))
@@ -335,45 +216,6 @@ def test_h264_weight_pointer_table_golden(device):
         assert np.array_equal(a, g[f"w{k}"]), ("weight", k)
         assert np.array_equal(b, g[f"b{k}"]), ("biweight", k)
     assert pel.ff_h264dsp_weight_init(10).weight_pixels_tab[0]               # the 16-bit tables (test_h264_weight_hbd)
-
-
-def test_h264_weight_batch_vs_oracle(device):
-    """Weighted and bi-weighted prediction over a frame of partitions (all widths, heights, denominators, unaligned x)."""
-    import torch
-    from ffmpeg_b200 import pel
-    O = cl.oracle()
-    rng = np.random.default_rng(17)
-    W, H = 352, 208
-    src = rng.integers(0, 256, (H, W), dtype=np.uint8)
-    dst0 = rng.integers(0, 256, (H, W), dtype=np.uint8)
-    params, doffs, soffs = [], [], []
-    for by in range(H // 16):
-        for bx in range(W // 16 - 1):
-            idx = int(rng.integers(0, 4))
-            h = int(rng.choice([2, 4, 8, 16]))
-            ld = int(rng.integers(0, 8))
-            w1, w2, off = (int(v) for v in rng.integers(-128, 128, 3))
-            params.append(pel.weight_params(idx, h, ld, w1, w2, off))
-            jx = 0 if idx == 0 else int(rng.integers(0, 4)) * (1 if idx < 3 else 2)      # destinations of one call must not overlap
-            doffs.append(by * 16 * W + bx * 16 + jx); soffs.append(by * 16 * W + bx * 16 + int(rng.integers(0, 8)))
-    n = len(params)
-    pa = np.array(params, np.int32)
-    for bi in (False, True):
-        exp = dst0.copy()
-        for (p0, w1, w2, off), do, so in zip(params, doffs, soffs):
-            idx, h, ld = p0 & 3, (p0 >> 8) & 255, (p0 >> 16) & 31
-            if bi:
-                O.orc_h264_biweight(idx, C.cast(exp.ctypes.data + do, cl.u8p), C.cast(src.ctypes.data + so, cl.u8p), W, h, ld, w1, w2, off)
-            else:
-                O.orc_h264_weight(idx, C.cast(exp.ctypes.data + do, cl.u8p), W, h, ld, w1, off)
-        with on_stream(device):
-            t = lambda a, dt: torch.from_numpy(np.array(a, dt)).cuda()
-            d_dst, d_src = torch.from_numpy(dst0).cuda(), torch.from_numpy(src).cuda()
-            pel.h264_weight_batch_device(device, n, torch.from_numpy(pa).cuda(), d_dst, t(doffs, np.int64), d_src if bi else None,
-                                         t(soffs, np.int64) if bi else None, W)
-            device.sync()
-            got = d_dst.cpu().numpy()
-        assert np.array_equal(got, exp), (bi, int((got != exp).sum()))
 
 
 # ---------------------------------------------------------------------------------------------- tx

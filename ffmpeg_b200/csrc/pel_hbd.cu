@@ -146,49 +146,6 @@ int chroma_hbd_launch(cudaStream_t st, long long n, const uint8_t *op, const uin
     return 0;
 }
 
-// H.264 explicit weighted prediction for 9 / 10 / 12 / 14 bit samples (h264dsp_template.c:30-99 per depth; h264dsp.c:103-110):
-//   weight:   block = clip((block * w + o') >> d),               o'  = (o << (d + depth - 8)) + (d ? 1 << (d - 1) : 0)
-//   biweight: dst   = clip((src * ws + dst * wd + o'') >> (d + 1)), o'' = (((o << (depth - 8)) + 1) | 1) << d
-// params as in b200_h264_weight_batch_device: [0] = width index | height << 8 | log2_denom << 16, [1] weight (dst weight), [2] source
-// weight, [3] offset.  A warp per block, a lane per pixel; offsets and stride in BYTES.
-template <bool BI>
-__global__ void __launch_bounds__(32 * HB_WARPS)
-weight_hbd_kernel(long long n, const int32_t *__restrict__ params, uint8_t *dst, const long long *__restrict__ dst_off, const uint8_t *src,
-                  const long long *__restrict__ src_off, long long stride, int depth)
-{
-    const long long i = (long long)blockIdx.x * HB_WARPS + (threadIdx.x >> 5);
-    if (i >= n) return;
-    const int lane = threadIdx.x & 31;
-    const int p0 = params[4 * i], wd = params[4 * i + 1], ws = params[4 * i + 2], po = params[4 * i + 3];
-    const int lw = 4 - (p0 & 3), w = 1 << lw, h = (p0 >> 8) & 255, d = (p0 >> 16) & 31, maxv = (1 << depth) - 1;
-    int off;
-    if (BI) { off = (int)((unsigned)po << (depth - 8)); off = (int)((unsigned)((off + 1) | 1) << d); }
-    else    { off = (int)((unsigned)po << (d + depth - 8)); if (d) off += 1 << (d - 1); }
-    const int sh = BI ? d + 1 : d;
-    const long long st = stride / 2;
-    unsigned short *dp = reinterpret_cast<unsigned short *>(dst + dst_off[i]);
-    const unsigned short *sp = BI ? reinterpret_cast<const unsigned short *>(src + src_off[i]) : nullptr;
-    for (int k = lane; k < w * h; k += 32) {
-        const int y = k >> lw, x = k & (w - 1);
-        unsigned short *q = dp + y * st + x;
-        const int v = BI ? ((int)sp[y * st + x] * ws + (int)*q * wd + off) >> sh : ((int)*q * wd + off) >> sh;
-        *q = (unsigned short)min(max(v, 0), maxv);
-    }
-}
-
-int weight_hbd_launch(cudaStream_t st, int depth, long long n, const int32_t *params, uint8_t *dst, const long long *doff, const uint8_t *src,
-                      const long long *soff, long long stride)
-{
-    if (n <= 0) return 0;
-    const long long blocks = (n + HB_WARPS - 1) / HB_WARPS;
-    if (blocks > 0x7fffffffLL) return B200_EINVAL;
-    if (src) weight_hbd_kernel<true><<<(unsigned)blocks, 32 * HB_WARPS, 0, st>>>(n, params, dst, doff, src, soff, stride, depth);
-    else     weight_hbd_kernel<false><<<(unsigned)blocks, 32 * HB_WARPS, 0, st>>>(n, params, dst, doff, nullptr, nullptr, stride, depth);
-    B200_LAUNCHED();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
-}
-
 void hbd_die(const char *what)
 {
     fprintf(stderr, "libb200dsp: high-bit-depth motion compensation failed: %s (%s)\n", what, b200_last_error());
@@ -294,50 +251,6 @@ void edge_hbd_tab(uint8_t *buf, const uint8_t *src, ptrdiff_t buf_linesize, ptrd
     if (cudaStreamSynchronize(st) != cudaSuccess) hbd_die("sync");
 }
 
-// weight / biweight table functions for 16-bit samples: one block through the device (host pointers)
-template <int DEPTH>
-void weight_hbd_host(bool bi, int idx, uint8_t *dst, const uint8_t *src, ptrdiff_t stride, int height, int log2_denom, int wd, int ws, int offset)
-{
-    B200Device *dev = b200_default_device();
-    if (!dev) hbd_die("no device");
-    if (height < 0 || height > 255 || log2_denom < 0 || log2_denom > 7) hbd_die("unsupported height / log2_denom");
-    if (height == 0) return;
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) hbd_die("cudaSetDevice");
-    const int w = 16 >> idx;
-    const size_t pitch = 32;
-    B200_LOCK_DEVICE(dev);
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, 2 * pitch * 256 + 256);
-    if (!scr) hbd_die("scratch");
-    uint8_t *ddst = scr, *dsrc = scr + pitch * 256, *meta = scr + 2 * pitch * 256;
-    cudaStream_t st = dev->stream;
-    if (b200_h2d_rows(ddst, pitch, dst, stride, (size_t)w * 2, (size_t)height, st) != cudaSuccess) hbd_die("h2d dst");
-    if (bi && b200_h2d_rows(dsrc, pitch, src, stride, (size_t)w * 2, (size_t)height, st) != cudaSuccess) hbd_die("h2d src");
-    struct { int32_t p[4]; long long doff, soff; } m = { { idx | (height << 8) | (log2_denom << 16), wd, ws, offset }, 0, 0 };
-    if (cudaMemcpyAsync(meta, &m, sizeof(m), cudaMemcpyHostToDevice, st) != cudaSuccess) hbd_die("h2d meta");
-    if (weight_hbd_launch(st, DEPTH, 1, (const int32_t *)meta, ddst, (const long long *)(meta + 16), bi ? dsrc : nullptr, (const long long *)(meta + 24), (long long)pitch) < 0)
-        hbd_die("launch");
-    if (b200_d2h_rows(dst, stride, ddst, pitch, (size_t)w * 2, (size_t)height, st) != cudaSuccess) hbd_die("d2h");
-    if (cudaStreamSynchronize(st) != cudaSuccess) hbd_die("sync");
-}
-template <int DEPTH, int IDX>
-void weight_hbd_tab(uint8_t *block, ptrdiff_t stride, int height, int log2_denom, int weight, int offset)
-{
-    weight_hbd_host<DEPTH>(false, IDX, block, nullptr, stride, height, log2_denom, weight, 0, offset);
-}
-template <int DEPTH, int IDX>
-void biweight_hbd_tab(uint8_t *dst, uint8_t *src, ptrdiff_t stride, int height, int log2_denom, int weightd, int weights, int offset)
-{
-    weight_hbd_host<DEPTH>(true, IDX, dst, src, stride, height, log2_denom, weightd, weights, offset);
-}
-template <int DEPTH>
-void fill_weight(B200H264WeightContext *c)
-{
-    c->weight_pixels_tab[0] = weight_hbd_tab<DEPTH, 0>; c->weight_pixels_tab[1] = weight_hbd_tab<DEPTH, 1>;
-    c->weight_pixels_tab[2] = weight_hbd_tab<DEPTH, 2>; c->weight_pixels_tab[3] = weight_hbd_tab<DEPTH, 3>;
-    c->biweight_pixels_tab[0] = biweight_hbd_tab<DEPTH, 0>; c->biweight_pixels_tab[1] = biweight_hbd_tab<DEPTH, 1>;
-    c->biweight_pixels_tab[2] = biweight_hbd_tab<DEPTH, 2>; c->biweight_pixels_tab[3] = biweight_hbd_tab<DEPTH, 3>;
-}
-
 } // namespace
 
 bool pel_hbd_fill(B200H264QpelContext *c, int bit_depth)
@@ -395,26 +308,4 @@ B200_API int b200_emulated_edge_mc_hbd_batch_device(B200Device *dev, int64_t n, 
     B200_LAUNCHED();
     B200_CUDA_OK(cudaGetLastError());
     return 0;
-}
-
-bool pel_hbd_fill_weight(B200H264WeightContext *c, int bit_depth)
-{
-    switch (bit_depth) {
-    case 9:  fill_weight<9>(c);  return true;
-    case 10: fill_weight<10>(c); return true;
-    case 12: fill_weight<12>(c); return true;
-    case 14: fill_weight<14>(c); return true;
-    }
-    return false;
-}
-
-B200_API int b200_h264_weight_hbd_batch_device(B200Device *dev, int bit_depth, int64_t n, const int32_t *params, uint8_t *dst, const int64_t *dst_off,
-                                               const uint8_t *src, const int64_t *src_off, ptrdiff_t stride)
-{
-    if (!dev || n < 0 || !params || !dst || !dst_off || (src && !src_off)) return B200_EINVAL;
-    if (bit_depth != 9 && bit_depth != 10 && bit_depth != 12 && bit_depth != 14) return B200_ENOSYS;
-    if ((stride & 1) || ((reinterpret_cast<uintptr_t>(dst) | reinterpret_cast<uintptr_t>(src)) & 1)) return B200_EINVAL;
-    if (n == 0) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
-    return weight_hbd_launch(dev->stream, bit_depth, n, params, dst, (const long long *)dst_off, src, (const long long *)src_off, (long long)stride);
 }

@@ -7,5 +7,3 @@ bool pel_hbd_fill(B200H264QpelContext *c, int bit_depth);
 // the 16-bit tables of ff_h264chroma_init (h264chroma.c:45-50) and the 16-bit emulated_edge_mc of ff_videodsp_init (videodsp.c:41-45)
 void pel_hbd_fill_chroma(B200H264ChromaContext *c);
 void pel_hbd_fill_edge(B200VideoDSPContext *c);
-// weight_pixels_tab / biweight_pixels_tab of ff_h264dsp_init for 9 / 10 / 12 / 14 bit (h264dsp.c:103-110); false for other depths
-bool pel_hbd_fill_weight(B200H264WeightContext *c, int bit_depth);

@@ -30,6 +30,7 @@ static inline double2 make_double2(double a, double b) { double2 r = { a, b }; r
 static thread_local dim3 threadIdx, blockIdx, blockDim, gridDim;
 
 #define __global__
+#define __host__
 #define __device__
 #define __forceinline__ inline
 #define __launch_bounds__(...)

@@ -26,13 +26,3 @@ extern "C" void emu_host_edge_hbd_tab(uint8_t *buf, const uint8_t *src, long lon
     pel_hbd_fill_edge(&c);
     c.emulated_edge_mc(buf, src, (ptrdiff_t)buf_linesize, (ptrdiff_t)src_linesize, block_w, block_h, src_x, src_y, w, h);
 }
-extern "C" int emu_host_weight_hbd_tab(int depth, int bi, int idx, uint8_t *dst, uint8_t *src, long long stride, int height, int log2_denom,
-                                       int wd, int ws, int offset)
-{
-    B200H264WeightContext c;
-    memset(&c, 0, sizeof(c));
-    if (!pel_hbd_fill_weight(&c, depth)) return -38;
-    if (bi) c.biweight_pixels_tab[idx](dst, src, (ptrdiff_t)stride, height, log2_denom, wd, ws, offset);
-    else    c.weight_pixels_tab[idx](dst, (ptrdiff_t)stride, height, log2_denom, wd, offset);
-    return 0;
-}

@@ -78,13 +78,13 @@ def rewrite_launches(txt):
 
 @pytest.fixture(scope="module")
 def emuhost():
-    """libemuhost.so: the translation units without inline PTX (fdsp, unquant, idct_hbd, tx_pfa, h264lf, pixelutils), HOST CODE INCLUDED, compiled with
+    """libemuhost.so: the translation units without inline PTX (fdsp, unquant, idct_hbd, tx_pfa, h264lf, h264weight, pixelutils, ...), HOST CODE INCLUDED, compiled with
     g++ against a stand-in CUDA runtime (tests/cuda_emu/fake/cuda_runtime.h): the library's own entry points run on the CPU"""
     gen = os.path.join(EMU, "_gen")
     os.makedirs(gen, exist_ok=True)
     cs = os.path.join(ROOT, "ffmpeg_b200", "csrc")
     srcs = []
-    for f in ("fdsp.cu", "unquant.cu", "idct_hbd.cu", "tx_pfa.cu", "h264lf.cu", "pixelutils.cu", "pel_hbd.cu", "h264idct_hbd.cu", "h264lf_hbd.cu", "mecmp_dct.cu", "fdctdsp.cu"):
+    for f in ("fdsp.cu", "unquant.cu", "idct_hbd.cu", "tx_pfa.cu", "h264lf.cu", "h264weight.cu", "pixelutils.cu", "pel_hbd.cu", "h264idct_hbd.cu", "mecmp_dct.cu", "fdctdsp.cu"):
         t = rewrite_launches(open(os.path.join(cs, f)).read())
         t = t.replace("extern __shared__ float2 pfa_z[];", "float2 *pfa_z = (float2 *)emu_smem;")
         assert "<<<" not in t
@@ -1232,7 +1232,7 @@ def test_host_h264_loop_filter_entry_points(emuhost):
 
 
 def test_host_h264_loop_filter_hbd(emuhost):
-    """h264lf_hbd.cu (deblocking for 9 / 10 / 12 / 14 bit samples) with its host code on the stand-in runtime: the batched device entry against
+    """h264lf.cu (deblocking for 9 / 10 / 12 / 14 bit samples) with its host code on the stand-in runtime: the batched device entry against
     the hashes of the compiled reference's pictures, and the H264DSPContext members edge by edge against the checker"""
     import hashlib
     from ffmpeg_b200._lib import H264LoopFilterContext
@@ -1403,39 +1403,43 @@ def test_host_chroma_and_edge_hbd(emuhost):
 
 
 def test_host_h264_weight_hbd(emuhost):
-    """pel_hbd.cu: explicit weighted prediction for 9 / 10 / 12 / 14 bit samples, table functions and the batched device entry on the
-    stand-in runtime against the checker"""
+    """h264weight.cu: explicit weighted prediction for 9 / 10 / 12 / 14 bit samples, the tables b200_h264_weight_init installs and the
+    batched device entry on the stand-in runtime against the checker"""
+    from ffmpeg_b200._lib import H264WeightContext
     from test_oracle_more import run_weight_hbd_case
     L, O = emuhost, cl.oracle()
     O.orc_h264_weight_hbd.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_ssize_t] + [C.c_int] * 4
     O.orc_h264_biweight_hbd.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_ssize_t] + [C.c_int] * 5
-    L.emu_host_weight_hbd_tab.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_longlong] + [C.c_int] * 5
     L.b200_h264_weight_hbd_batch_device.argtypes = [C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_ssize_t]
     dev = C.c_void_p()
     assert L.b200_device_open(C.byref(dev), 0, None) == 0
     for depth in (9, 10, 12, 14):
+        t = H264WeightContext()
+        assert L.b200_h264_weight_init(C.byref(t), depth) == 0
+        wf = lambda dp, idx, blk, st, h, d, wd, off: t.weight_pixels_tab[idx](blk, st, h, d, wd, off)
+        bf = lambda dp, idx, blk, src, st, h, d, wd, ws, off: t.biweight_pixels_tab[idx](blk, src, st, h, d, wd, ws, off)
         cases = cl.hbd_weight_cases(depth)
         for case in cases[:25]:
             exp = run_weight_hbd_case(O.orc_h264_weight_hbd, O.orc_h264_biweight_hbd, depth, case)
-            wf = lambda dp, idx, blk, st, h, d, wd, off: L.emu_host_weight_hbd_tab(dp, 0, idx, blk, None, st, h, d, wd, 0, off)
-            bf = lambda dp, idx, blk, src, st, h, d, wd, ws, off: L.emu_host_weight_hbd_tab(dp, 1, idx, blk, src, st, h, d, wd, ws, off)
             assert np.array_equal(run_weight_hbd_case(wf, bf, depth, case), exp), (depth, case)
-        # batch: the weight cases in place, then the biweight cases, blocks on a 16 x 16 grid of a 64 x 48 picture (12 per call)
-        img, d0 = cl.hbd_picture(depth, 0)
+        # batch: the weight cases in place, then the biweight cases, blocks on a 16 x 16 grid of a 64 x 48 picture (12 per call), at
+        # 32-byte-aligned offsets and shifted by one sample (element accesses); the spare row takes the last sample of the shifted last block
+        img, d0 = (np.vstack([a, a[:1]]) for a in cl.hbd_picture(depth, 0))
         for bi in (0, 1):
             sel = [c for c in cases if c[0] == bi][:12]
             params = np.array([[c[1] | (c[2] << 8) | (c[3] << 16), c[4], c[5], c[6]] for c in sel], np.int32)
-            doff = np.array([((k // 4) * 16 * 64 + (k % 4) * 16) * 2 for k in range(len(sel))], np.int64)
-            got, exp = d0.copy(), d0.copy()
-            assert L.b200_h264_weight_hbd_batch_device(dev, depth, len(sel), params.ctypes.data, got.ctypes.data, doff.ctypes.data,
-                                                       img.ctypes.data if bi else None, doff.ctypes.data if bi else None, 128) == 0
-            for k, c in enumerate(sel):
-                if bi:
-                    O.orc_h264_biweight_hbd(depth, c[1], exp.ctypes.data + int(doff[k]), img.ctypes.data + int(doff[k]), 128, c[2], c[3], c[4], c[5], c[6])
-                else:
-                    O.orc_h264_weight_hbd(depth, c[1], exp.ctypes.data + int(doff[k]), 128, c[2], c[3], c[4], c[6])
-            assert np.array_equal(got, exp), (depth, bi)
-    assert L.emu_host_weight_hbd_tab(11, 0, 0, None, None, 0, 0, 0, 0, 0, 0) == -38
+            for shift in (0, 2):
+                doff = np.array([((k // 4) * 16 * 64 + (k % 4) * 16) * 2 + shift for k in range(len(sel))], np.int64)
+                got, exp = d0.copy(), d0.copy()
+                assert L.b200_h264_weight_hbd_batch_device(dev, depth, len(sel), params.ctypes.data, got.ctypes.data, doff.ctypes.data,
+                                                           img.ctypes.data if bi else None, doff.ctypes.data if bi else None, 128) == 0
+                for k, c in enumerate(sel):
+                    if bi:
+                        O.orc_h264_biweight_hbd(depth, c[1], exp.ctypes.data + int(doff[k]), img.ctypes.data + int(doff[k]), 128, c[2], c[3], c[4], c[5], c[6])
+                    else:
+                        O.orc_h264_weight_hbd(depth, c[1], exp.ctypes.data + int(doff[k]), 128, c[2], c[3], c[4], c[6])
+                assert np.array_equal(got, exp), (depth, bi, shift)
+    assert L.b200_h264_weight_init(C.byref(H264WeightContext()), 11) == -38
 
 
 def test_host_h264_idct_hbd(emuhost):

@@ -1057,8 +1057,9 @@ def test_h264_weight_hbd(device):
         pel.ff_h264dsp_weight_init(11)
     rng = np.random.default_rng(29)
     W, H, depth = 640, 368, 10
-    ref_ = rng.integers(0, 1 << depth, (H, W)).astype(np.uint16)
-    dst0 = rng.integers(0, 1 << depth, (H, W)).astype(np.uint16)
+    # one spare row: the last block shifted by a sample ends a sample into it
+    ref_ = rng.integers(0, 1 << depth, (H + 1, W)).astype(np.uint16)
+    dst0 = rng.integers(0, 1 << depth, (H + 1, W)).astype(np.uint16)
     for bi in (0, 1):
         prm, doffs = [], []
         for by in range(H // 16):
@@ -1066,20 +1067,21 @@ def test_h264_weight_hbd(device):
                 idx, h, d = int(rng.integers(0, 4)), int(rng.choice([2, 4, 8, 16])), int(rng.integers(0, 8))
                 prm.append([idx | (h << 8) | (d << 16), int(rng.integers(-128, 128)), int(rng.integers(-128, 128)), int(rng.integers(-128, 128))])
                 doffs.append((by * 16 * W + bx * 16) * 2)
-        prm_a, do_a = np.array(prm, np.int32), np.array(doffs, np.int64)
-        exp = dst0.copy()
-        for p_, o_ in zip(prm, doffs):
-            if bi:
-                O.orc_h264_biweight_hbd(depth, p_[0] & 3, exp.ctypes.data + o_, ref_.ctypes.data + o_, W * 2, (p_[0] >> 8) & 255, p_[0] >> 16, p_[1], p_[2], p_[3])
-            else:
-                O.orc_h264_weight_hbd(depth, p_[0] & 3, exp.ctypes.data + o_, W * 2, (p_[0] >> 8) & 255, p_[0] >> 16, p_[1], p_[3])
-        with on_stream(device):
-            d_p, d_o = torch.from_numpy(prm_a).cuda(), torch.from_numpy(do_a).cuda()
-            d_dst, d_src = torch.from_numpy(dst0.view(np.int16)).cuda(), torch.from_numpy(ref_.view(np.int16)).cuda()
-            pel.h264_weight_hbd_batch_device(device, depth, len(prm), d_p, d_dst, d_o, d_src if bi else None, d_o if bi else None, W * 2)
-            device.sync()
-            got = d_dst.cpu().numpy().view(np.uint16)
-        assert np.array_equal(got, exp), (bi, int((got != exp).sum()))
+        for shift in (0, 2):                                        # 32-byte-aligned blocks (word accesses), then one sample further
+            prm_a, do_a = np.array(prm, np.int32), np.array(doffs, np.int64) + shift
+            exp = dst0.copy()
+            for p_, o_ in zip(prm, do_a.tolist()):
+                if bi:
+                    O.orc_h264_biweight_hbd(depth, p_[0] & 3, exp.ctypes.data + o_, ref_.ctypes.data + o_, W * 2, (p_[0] >> 8) & 255, p_[0] >> 16, p_[1], p_[2], p_[3])
+                else:
+                    O.orc_h264_weight_hbd(depth, p_[0] & 3, exp.ctypes.data + o_, W * 2, (p_[0] >> 8) & 255, p_[0] >> 16, p_[1], p_[3])
+            with on_stream(device):
+                d_p, d_o = torch.from_numpy(prm_a).cuda(), torch.from_numpy(do_a).cuda()
+                d_dst, d_src = torch.from_numpy(dst0.view(np.int16)).cuda(), torch.from_numpy(ref_.view(np.int16)).cuda()
+                pel.h264_weight_hbd_batch_device(device, depth, len(prm), d_p, d_dst, d_o, d_src if bi else None, d_o if bi else None, W * 2)
+                device.sync()
+                got = d_dst.cpu().numpy().view(np.uint16)
+            assert np.array_equal(got, exp), (bi, shift, int((got != exp).sum()))
 
 
 # ---------------------------------------------------------------------------------------------- H.264 residual adds, 16-bit samples

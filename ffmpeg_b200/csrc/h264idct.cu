@@ -1,31 +1,46 @@
-// h264idct.cu — libavcodec H.264 residual transforms (8 bit) on sm_90a (C ABI: "h264 residual").
+// h264idct.cu — libavcodec H.264 residual transforms on sm_90a for 8, 9, 10, 12 and 14 bit samples: idct_add / idct8_add / idct_dc_add /
+// idct8_dc_add of H264DSPContext as ff_h264dsp_init(c, depth, ...) installs them (libavcodec/h264dsp.c:66-158) (C ABI: "h264 residual").
 //
 // Reference semantics reproduced bit-for-bit (checker: oracle/idct_oracle.c):
-//   ff_h264_idct_add_8_c      libavcodec/h264idct_template.c:33-70     4x4, result added to dst, coefficients cleared
-//   ff_h264_idct8_add_8_c     libavcodec/h264idct_template.c:72-145    8x8
-//   ff_h264_idct_dc_add_8_c / ff_h264_idct8_dc_add_8_c   :147-181      DC-only blocks
-// The first pass writes its results back as int16 (dctcoef), sums are mod 2^32 (SUINT): both are kept.
+//   ff_h264_idct_add_<depth>_c      libavcodec/h264idct_template.c:33-70     4x4, result added to dst, coefficients cleared
+//   ff_h264_idct8_add_<depth>_c     libavcodec/h264idct_template.c:72-145    8x8
+//   ff_h264_idct_dc_add_<depth>_c / ff_h264_idct8_dc_add_<depth>_c   :147-181   DC-only blocks
+// dctcoef is int16_t with uint8 samples at 8 bits, int32_t with uint16 samples above.  The first pass and the + 32 on the DC coefficient
+// write back into dctcoef (an int16 store wraps), sums are mod 2^32 (SUINT): both are kept.  The sum >> 6 is clipped to the sample depth.
 //
-// Batched kernel: one thread per block.  4x4: 32 bytes of coefficients in (two 16-byte loads), four 32-bit destination
-// words read-modify-written (the reference requires dst 4-aligned, h264dsp.h:81); 8x8: 128 bytes in, eight 8-byte rows.
-// Every consumed coefficient block is zeroed like the reference's memset (the decoder relies on it for the next macroblock).
+// Batched kernel: one thread per block.  Every consumed coefficient block is zeroed like the reference's memset (the decoder relies on
+// it for the next macroblock).  8 bit: 32 / 128 bytes of coefficients in 16-byte accesses, destination rows as 4- / 8-byte words (the
+// reference requires dst 4-aligned, h264dsp.h:81).  16 bit: coefficients one by one (the 16-bit entry takes 4-byte-aligned blocks), a
+// destination row in one 8- / 16-byte access where dst and stride allow it, else sample by sample.
 #include "common.h"
-#include "h264idct_hbd.h"
 #include <cstring>
+#include <type_traits>
 
 namespace {
 
-__device__ __forceinline__ int clip8(int v) { return __vimin_s32_relu(v, 255); }
-__device__ __forceinline__ int s16(unsigned v) { return (int)(short)v; }
+template <typename P> using dctcoef = std::conditional_t<sizeof(P) == 1, int16_t, int32_t>;
 
-// four clipped pixels dst + (v >> 6) packed into one word
-__device__ __forceinline__ unsigned add4(unsigned d, unsigned v0, unsigned v1, unsigned v2, unsigned v3)
+// a store into dctcoef, read back
+template <typename P> __device__ __forceinline__ int coef(unsigned v) { return (int)(dctcoef<P>)v; }
+
+// a destination row of N samples: 4-byte words, accessed as one unsigned / uint2 / uint4
+template <int WORDS> struct RowVec;
+template <> struct RowVec<1> { using T = unsigned; };
+template <> struct RowVec<2> { using T = uint2; };
+template <> struct RowVec<4> { using T = uint4; };
+
+// clipped samples of the word d plus the residuals v[] (four uint8 or two uint16 samples)
+__device__ __forceinline__ unsigned add_word(unsigned d, const int *v, int, uint8_t)
 {
-    const unsigned p0 = (unsigned)clip8((int)__byte_perm(d, 0, 0x4440) + ((int)v0 >> 6));
-    const unsigned p1 = (unsigned)clip8((int)__byte_perm(d, 0, 0x4441) + ((int)v1 >> 6));
-    const unsigned p2 = (unsigned)clip8((int)__byte_perm(d, 0, 0x4442) + ((int)v2 >> 6));
-    const unsigned p3 = (unsigned)clip8((int)(d >> 24) + ((int)v3 >> 6));
+    const unsigned p0 = (unsigned)__vimin_s32_relu((int)__byte_perm(d, 0, 0x4440) + v[0], 255);
+    const unsigned p1 = (unsigned)__vimin_s32_relu((int)__byte_perm(d, 0, 0x4441) + v[1], 255);
+    const unsigned p2 = (unsigned)__vimin_s32_relu((int)__byte_perm(d, 0, 0x4442) + v[2], 255);
+    const unsigned p3 = (unsigned)__vimin_s32_relu((int)(d >> 24) + v[3], 255);
     return __byte_perm(__byte_perm(p0, p1, 0x1140), __byte_perm(p2, p3, 0x1140), 0x5410);
+}
+__device__ __forceinline__ unsigned add_word(unsigned d, const int *v, int maxv, uint16_t)
+{
+    return (unsigned)__vimin_s32_relu((int)(d & 0xffff) + v[0], maxv) | (unsigned)__vimin_s32_relu((int)(d >> 16) + v[1], maxv) << 16;
 }
 
 __device__ __forceinline__ void idct8_1d(const int *in, unsigned *out)
@@ -43,112 +58,122 @@ __device__ __forceinline__ void idct8_1d(const int *in, unsigned *out)
     out[2] = b4 + b3; out[5] = b4 - b3; out[3] = b6 + b1; out[4] = b6 - b1;
 }
 
-// kind 0: 4x4, 1: 8x8, 2: 4x4 DC only, 3: 8x8 DC only.  blk_off in int16 elements (multiples of 8: blocks are 16-byte aligned)
-template <int KIND>
+// kind 0: 4x4, 1: 8x8, 2: 4x4 DC only, 3: 8x8 DC only.  P = uint8_t (depth 8) or uint16_t (9 / 10 / 12 / 14).  blk_off in coefficients
+// (multiples of 8 at 8 bits: blocks are 16-byte aligned), dst_off and stride in bytes.
+template <typename P, int KIND>
 __global__ void __launch_bounds__(128)
-h264_idct_kernel(long long n, int16_t *blocks, const int64_t *blk_off, uint8_t *dst, const int64_t *dst_off, long long stride)
+h264_idct_kernel(long long n, dctcoef<P> *blocks, const int64_t *blk_off, uint8_t *dst, const int64_t *dst_off, long long stride, int depth)
 {
+    constexpr int N = (KIND & 1) ? 8 : 4, NC = N * N, SPW = 4 / sizeof(P), WORDS = N / SPW;     // samples per word, words per row
+    using Row = typename RowVec<WORDS>::T;
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    int16_t *b = blocks + __ldg(blk_off + i);
+    dctcoef<P> *b = blocks + __ldg(blk_off + i);
     uint8_t *d = dst + __ldg(dst_off + i);
+    const int maxv = sizeof(P) == 1 ? 255 : (1 << depth) - 1;
+    // a row in one access; the 8-bit entry guarantees the alignment, at 16 bits a misaligned row goes sample by sample
+    const bool vec = sizeof(P) == 1 || ((reinterpret_cast<uintptr_t>(d) | (uintptr_t)stride) % sizeof(Row)) == 0;
+    // every destination row is requested before the first store: written row by row (load, add, store) each row's load would sit
+    // behind the previous row's store in program order and the thread would make one trip to memory per row (ncu: 138 warps stalled
+    // on the long scoreboard per issue with the memory system at 15 %)
+    unsigned dv[N][WORDS];
+    auto load_rows = [&] {
+#pragma unroll
+        for (int r = 0; r < N; r++) {
+            if (vec) {
+                const Row v = *reinterpret_cast<const Row *>(d + r * stride);
+                memcpy(dv[r], &v, sizeof(Row));
+            } else {
+                const P *p = reinterpret_cast<const P *>(d + r * stride);
+#pragma unroll
+                for (int k = 0; k < WORDS; k++) dv[r][k] = p[2 * k] | (unsigned)p[2 * k + 1] << 16;
+            }
+        }
+    };
+    auto store_rows = [&](const int (*res)[N]) {
+#pragma unroll
+        for (int r = 0; r < N; r++) {
+#pragma unroll
+            for (int k = 0; k < WORDS; k++) dv[r][k] = add_word(dv[r][k], res[r] + SPW * k, maxv, P());
+            if (vec) {
+                Row v;
+                memcpy(&v, dv[r], sizeof(Row));
+                *reinterpret_cast<Row *>(d + r * stride) = v;
+            } else {
+                P *p = reinterpret_cast<P *>(d + r * stride);
+#pragma unroll
+                for (int k = 0; k < WORDS; k++) { p[2 * k] = (P)dv[r][k]; p[2 * k + 1] = (P)(dv[r][k] >> 16); }
+            }
+        }
+    };
+    int res[N][N];                                              // res[row][column]: what is added to the sample
     if (KIND >= 2) {
-        constexpr int N = KIND == 2 ? 4 : 8;
-        const int dc = ((int)b[0] + 32) >> 6;
+        const int dc = (int)((unsigned)b[0] + 32u) >> 6;
+        load_rows();
         b[0] = 0;
-        const unsigned z = (unsigned)dc << 6;                  // add4 shifts it back
-        unsigned dv[N][2];
 #pragma unroll
-        for (int r = 0; r < N; r++) {
-            const unsigned *p = reinterpret_cast<const unsigned *>(d + r * stride);
-            dv[r][0] = p[0]; dv[r][1] = N == 8 ? p[1] : 0u;
-        }
+        for (int r = 0; r < N; r++)
 #pragma unroll
-        for (int r = 0; r < N; r++) {
-            unsigned *p = reinterpret_cast<unsigned *>(d + r * stride);
-            p[0] = add4(dv[r][0], z, z, z, z);
-            if (N == 8) p[1] = add4(dv[r][1], z, z, z, z);
-        }
+            for (int x = 0; x < N; x++) res[r][x] = dc;
+        store_rows(res);
         return;
     }
-    if (KIND == 0) {
+    int c[NC];
+    if (sizeof(P) == 1) {
+        uint4 q[NC / 8];
         uint4 *bp = reinterpret_cast<uint4 *>(b);
-        const uint4 q0 = bp[0], q1 = bp[1];
-        // every destination row is requested before the first store: written row by row (load, add, store) each row's load would sit
-        // behind the previous row's store in program order and the thread would make one trip to memory per row (ncu: 138 warps stalled
-        // on the long scoreboard per issue with the memory system at 15 %)
-        unsigned dv[4];
 #pragma unroll
-        for (int r = 0; r < 4; r++) dv[r] = *reinterpret_cast<const unsigned *>(d + r * stride);
-        bp[0] = make_uint4(0, 0, 0, 0); bp[1] = make_uint4(0, 0, 0, 0);
-        const unsigned w[8] = { q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w };
-        int c[16];
+        for (int k = 0; k < NC / 8; k++) q[k] = bp[k];
+        load_rows();
 #pragma unroll
-        for (int k = 0; k < 8; k++) { c[2 * k] = s16(w[k]); c[2 * k + 1] = (int)w[k] >> 16; }
-        c[0] = s16((unsigned)(c[0] + 32));                      // block[0] += 1 << 5 wraps in int16 storage
-        int t[16];
+        for (int k = 0; k < NC / 8; k++) {
+            bp[k] = make_uint4(0, 0, 0, 0);
+            const unsigned w[4] = { q[k].x, q[k].y, q[k].z, q[k].w };
+#pragma unroll
+            for (int j = 0; j < 4; j++) { c[8 * k + 2 * j] = coef<P>(w[j]); c[8 * k + 2 * j + 1] = (int)w[j] >> 16; }
+        }
+    } else {
+#pragma unroll
+        for (int k = 0; k < NC; k++) c[k] = b[k];
+        load_rows();
+#pragma unroll
+        for (int k = 0; k < NC; k++) b[k] = 0;
+    }
+    c[0] = coef<P>((unsigned)(c[0] + 32));                      // block[0] += 1 << 5
+    if (KIND == 0) {
 #pragma unroll
         for (int x = 0; x < 4; x++) {
             const unsigned z0 = c[x] + (unsigned)c[x + 8], z1 = c[x] - (unsigned)c[x + 8];
             const unsigned z2 = (c[x + 4] >> 1) - (unsigned)c[x + 12], z3 = c[x + 4] + (unsigned)(c[x + 12] >> 1);
-            t[x] = s16(z0 + z3); t[x + 4] = s16(z1 + z2); t[x + 8] = s16(z1 - z2); t[x + 12] = s16(z0 - z3);
+            c[x] = coef<P>(z0 + z3); c[x + 4] = coef<P>(z1 + z2); c[x + 8] = coef<P>(z1 - z2); c[x + 12] = coef<P>(z0 - z3);
         }
-        unsigned o[4][4];                                       // o[row][column]
 #pragma unroll
         for (int x = 0; x < 4; x++) {
-            const unsigned z0 = t[4 * x] + (unsigned)t[2 + 4 * x], z1 = t[4 * x] - (unsigned)t[2 + 4 * x];
-            const unsigned z2 = (t[1 + 4 * x] >> 1) - (unsigned)t[3 + 4 * x], z3 = t[1 + 4 * x] + (unsigned)(t[3 + 4 * x] >> 1);
-            o[0][x] = z0 + z3; o[1][x] = z1 + z2; o[2][x] = z1 - z2; o[3][x] = z0 - z3;
+            const unsigned z0 = c[4 * x] + (unsigned)c[2 + 4 * x], z1 = c[4 * x] - (unsigned)c[2 + 4 * x];
+            const unsigned z2 = (c[1 + 4 * x] >> 1) - (unsigned)c[3 + 4 * x], z3 = c[1 + 4 * x] + (unsigned)(c[3 + 4 * x] >> 1);
+            res[0][x] = (int)(z0 + z3) >> 6; res[1][x] = (int)(z1 + z2) >> 6; res[2][x] = (int)(z1 - z2) >> 6; res[3][x] = (int)(z0 - z3) >> 6;
+        }
+    } else {
+#pragma unroll
+        for (int x = 0; x < 8; x++) {
+            int in[8]; unsigned out[8];
+#pragma unroll
+            for (int k = 0; k < 8; k++) in[k] = c[x + 8 * k];
+            idct8_1d(in, out);
+#pragma unroll
+            for (int k = 0; k < 8; k++) c[x + 8 * k] = coef<P>(out[k]);
         }
 #pragma unroll
-        for (int r = 0; r < 4; r++)
-            *reinterpret_cast<unsigned *>(d + r * stride) = add4(dv[r], o[r][0], o[r][1], o[r][2], o[r][3]);
-        return;
+        for (int x = 0; x < 8; x++) {
+            int in[8]; unsigned out[8];
+#pragma unroll
+            for (int k = 0; k < 8; k++) in[k] = c[k + 8 * x];
+            idct8_1d(in, out);
+#pragma unroll
+            for (int k = 0; k < 8; k++) res[k][x] = (int)out[k] >> 6;
+        }
     }
-    // 8x8
-    uint4 *bp = reinterpret_cast<uint4 *>(b);
-    int c[64];
-    uint4 qq[8];
-    uint2 dv[8];                                                // all loads first (see the 4x4 case)
-#pragma unroll
-    for (int r = 0; r < 8; r++) qq[r] = bp[r];
-#pragma unroll
-    for (int r = 0; r < 8; r++) dv[r] = *reinterpret_cast<const uint2 *>(d + r * stride);
-#pragma unroll
-    for (int r = 0; r < 8; r++) {
-        const uint4 q = qq[r];
-        bp[r] = make_uint4(0, 0, 0, 0);
-        const unsigned w[4] = { q.x, q.y, q.z, q.w };
-#pragma unroll
-        for (int k = 0; k < 4; k++) { c[8 * r + 2 * k] = s16(w[k]); c[8 * r + 2 * k + 1] = (int)w[k] >> 16; }
-    }
-    c[0] = s16((unsigned)(c[0] + 32));
-#pragma unroll
-    for (int x = 0; x < 8; x++) {
-        int in[8]; unsigned out[8];
-#pragma unroll
-        for (int k = 0; k < 8; k++) in[k] = c[x + 8 * k];
-        idct8_1d(in, out);
-#pragma unroll
-        for (int k = 0; k < 8; k++) c[x + 8 * k] = s16(out[k]);
-    }
-    unsigned o[8][8];                                           // o[row][column]
-#pragma unroll
-    for (int x = 0; x < 8; x++) {
-        int in[8]; unsigned out[8];
-#pragma unroll
-        for (int k = 0; k < 8; k++) in[k] = c[k + 8 * x];
-        idct8_1d(in, out);
-#pragma unroll
-        for (int k = 0; k < 8; k++) o[k][x] = out[k];
-    }
-#pragma unroll
-    for (int r = 0; r < 8; r++) {
-        uint2 v = dv[r];
-        v.x = add4(v.x, o[r][0], o[r][1], o[r][2], o[r][3]);
-        v.y = add4(v.y, o[r][4], o[r][5], o[r][6], o[r][7]);
-        *reinterpret_cast<uint2 *>(d + r * stride) = v;
-    }
+    store_rows(res);
 }
 
 void die(const char *what)
@@ -157,37 +182,56 @@ void die(const char *what)
     abort();
 }
 
-template <int KIND>
-void launch(cudaStream_t st, long long n, int16_t *blocks, const int64_t *blk_off, uint8_t *dst, const int64_t *dst_off, long long stride)
+template <typename P>
+int launch(cudaStream_t st, int kind, int depth, long long n, dctcoef<P> *blocks, const int64_t *blk_off, uint8_t *dst, const int64_t *dst_off,
+           long long stride)
 {
     const long long ctas = (n + 127) / 128;
-    h264_idct_kernel<KIND><<<(unsigned)ctas, 128, 0, st>>>(n, blocks, blk_off, dst, dst_off, stride);
+    if (ctas > 0x7fffffffLL) return B200_EINVAL;
+    const unsigned g = (unsigned)ctas;
+    switch (kind) {
+    case 0: h264_idct_kernel<P, 0><<<g, 128, 0, st>>>(n, blocks, blk_off, dst, dst_off, stride, depth); break;
+    case 1: h264_idct_kernel<P, 1><<<g, 128, 0, st>>>(n, blocks, blk_off, dst, dst_off, stride, depth); break;
+    case 2: h264_idct_kernel<P, 2><<<g, 128, 0, st>>>(n, blocks, blk_off, dst, dst_off, stride, depth); break;
+    default: h264_idct_kernel<P, 3><<<g, 128, 0, st>>>(n, blocks, blk_off, dst, dst_off, stride, depth); break;
+    }
+    B200_LAUNCHED();
+    B200_CUDA_OK(cudaGetLastError());
+    return 0;
 }
 
-// drop-in: one block through the device (host pointers)
-template <int KIND>
-void host_fn(uint8_t *dst, int16_t *block, ptrdiff_t stride)
+// drop-in: one block through the device (host pointers; above 8 bits `block` holds int32 coefficients behind the reference's int16_t * type)
+template <int DEPTH, int KIND>
+void host_fn(uint8_t *dst, int16_t *block16, ptrdiff_t stride)
 {
+    using P = std::conditional_t<DEPTH == 8, uint8_t, uint16_t>;
     constexpr int N = (KIND & 1) ? 8 : 4, NC = N * N;
+    dctcoef<P> *block = reinterpret_cast<dctcoef<P> *>(block16);
     B200Device *dev = b200_default_device();
     if (!dev) die("no device");
     if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
     B200_LOCK_DEVICE(dev);      // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, 512);
+    constexpr size_t CB = 64 * sizeof(dctcoef<P>);                // coefficients of an 8x8 block
+    uint8_t *scr = (uint8_t *)b200_scratch(dev, CB + 256);
     if (!scr) die("scratch");
-    int16_t *dblk = (int16_t *)scr;                       // 128 B
-    uint8_t *dpix = scr + 128;                            // N rows, pitch 16
-    int64_t *meta = (int64_t *)(scr + 256);
+    dctcoef<P> *dblk = (dctcoef<P> *)scr;
+    uint8_t *dpix = scr + CB;                                      // N rows, pitch 16 bytes
+    int64_t *meta = (int64_t *)(scr + CB + 128);
     cudaStream_t st = dev->stream;
     const int64_t m[2] = { 0, 0 };
-    if (cudaMemcpyAsync(dblk, block, NC * sizeof(int16_t), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d block");
-    if (b200_h2d_rows(dpix, 16, dst, stride, N, N, st) != cudaSuccess) die("h2d dst");
+    if (cudaMemcpyAsync(dblk, block, (KIND >= 2 ? 1 : NC) * sizeof(dctcoef<P>), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d block");
+    if (b200_h2d_rows(dpix, 16, dst, stride, N * sizeof(P), N, st) != cudaSuccess) die("h2d dst");
     if (cudaMemcpyAsync(meta, m, sizeof(m), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d meta");
-    h264_idct_kernel<KIND><<<1, 128, 0, st>>>(1, dblk, meta, dpix, meta + 1, 16);
-    B200_LAUNCHED();
-    if (b200_d2h_rows(dst, stride, dpix, 16, N, N, st) != cudaSuccess) die("d2h");
+    if (launch<P>(st, KIND, DEPTH, 1, dblk, meta, dpix, meta + 1, 16) < 0) die("launch");
+    if (b200_d2h_rows(dst, stride, dpix, 16, N * sizeof(P), N, st) != cudaSuccess) die("d2h");
     if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
-    if (KIND >= 2) block[0] = 0; else memset(block, 0, NC * sizeof(int16_t));     // what the reference leaves behind
+    if (KIND >= 2) block[0] = 0; else memset(block, 0, NC * sizeof(dctcoef<P>));     // what the reference leaves behind
+}
+
+template <int DEPTH>
+void fill(B200H264IDCTContext *c)
+{
+    c->idct_add = host_fn<DEPTH, 0>; c->idct8_add = host_fn<DEPTH, 1>; c->idct_dc_add = host_fn<DEPTH, 2>; c->idct8_dc_add = host_fn<DEPTH, 3>;
 }
 
 } // namespace
@@ -197,9 +241,14 @@ B200_API int b200_h264_idct_init(B200H264IDCTContext *c, int bit_depth, int chro
     (void)chroma_format_idc;
     if (!c) return B200_EINVAL;
     if (!b200_default_device()) return B200_ENODEV;
-    if (bit_depth != 8) return h264idct_hbd_fill(c, bit_depth) ? 0 : B200_ENOSYS;      // h264dsp.c:139-158: 9 / 10 / 12 / 14 (h264idct_hbd.cu)
-    c->idct_add = host_fn<0>; c->idct8_add = host_fn<1>; c->idct_dc_add = host_fn<2>; c->idct8_dc_add = host_fn<3>;
-    return 0;
+    switch (bit_depth) {                                           // h264dsp.c:139-158
+    case 8:  fill<8>(c);  return 0;
+    case 9:  fill<9>(c);  return 0;
+    case 10: fill<10>(c); return 0;
+    case 12: fill<12>(c); return 0;
+    case 14: fill<14>(c); return 0;
+    }
+    return B200_ENOSYS;
 }
 
 B200_API int b200_h264_idct_batch_device(B200Device *dev, int kind, int64_t n, int16_t *blocks, const int64_t *blk_off,
@@ -208,15 +257,17 @@ B200_API int b200_h264_idct_batch_device(B200Device *dev, int kind, int64_t n, i
     if (!dev || n < 0 || !blocks || !blk_off || !dst || !dst_off || kind < 0 || kind > 3) return B200_EINVAL;
     if (((uintptr_t)blocks & 15) || ((uintptr_t)dst & ((kind & 1) ? 7 : 3)) || (stride & ((kind & 1) ? 7 : 3))) return B200_EINVAL;
     if (n == 0) return 0;
-    if ((n + 127) / 128 > 0x7fffffffLL) return B200_EINVAL;
     B200_CUDA_OK(cudaSetDevice(dev->ordinal));
-    switch (kind) {
-    case 0: launch<0>(dev->stream, n, blocks, blk_off, dst, dst_off, stride); break;
-    case 1: launch<1>(dev->stream, n, blocks, blk_off, dst, dst_off, stride); break;
-    case 2: launch<2>(dev->stream, n, blocks, blk_off, dst, dst_off, stride); break;
-    default: launch<3>(dev->stream, n, blocks, blk_off, dst, dst_off, stride); break;
-    }
-    B200_LAUNCHED();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
+    return launch<uint8_t>(dev->stream, kind, 8, n, blocks, blk_off, dst, dst_off, (long long)stride);
+}
+
+B200_API int b200_h264_idct_hbd_batch_device(B200Device *dev, int bit_depth, int kind, int64_t n, int32_t *blocks, const int64_t *blk_off,
+                                             uint8_t *dst, const int64_t *dst_off, ptrdiff_t stride)
+{
+    if (!dev || n < 0 || !blocks || !blk_off || !dst || !dst_off || kind < 0 || kind > 3) return B200_EINVAL;
+    if (bit_depth != 9 && bit_depth != 10 && bit_depth != 12 && bit_depth != 14) return B200_ENOSYS;
+    if (((uintptr_t)blocks & 3) || ((uintptr_t)dst & 1) || (stride & 1)) return B200_EINVAL;
+    if (n == 0) return 0;
+    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    return launch<uint16_t>(dev->stream, kind, bit_depth, n, blocks, blk_off, dst, dst_off, (long long)stride);
 }

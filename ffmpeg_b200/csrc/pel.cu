@@ -428,28 +428,6 @@ chroma_kernel(long long n, const uint8_t *op, const uint8_t *hh, const uint8_t *
     }
 }
 
-// emulated_edge_mc (videodsp_template.c:24-101) as a clamped gather: one warp per window, lanes across columns.
-// geom[4*i..] = block_w, block_h, src_x, src_y; origin[i] = offset of that picture's sample (0, 0) from `src`.
-__global__ void __launch_bounds__(32 * WARPS)
-edge_kernel(long long n, uint8_t *buf, const int64_t *buf_off, long long buf_ls, const uint8_t *src, const int64_t *origin,
-            long long src_ls, const int32_t *geom, int w, int h)
-{
-    const long long i = (long long)blockIdx.x * WARPS + (threadIdx.x >> 5);
-    if (i >= n) return;
-    const int lane = threadIdx.x & 31;
-    const int4 gm = __ldg((const int4 *)geom + i);
-    const int bw = gm.x, bh = gm.y, sx = gm.z, sy = gm.w;
-    const uint8_t *pic = src + origin[i];
-    uint8_t *out = buf + buf_off[i];
-    for (int x = lane; x < bw; x += 32) {
-        const int px = min(max(sx + x, 0), w - 1);
-        for (int y = 0; y < bh; y++) {
-            const int py = min(max(sy + y, 0), h - 1);
-            out[(long long)y * buf_ls + x] = __ldg(pic + (long long)py * src_ls + px);
-        }
-    }
-}
-
 // The dot-product form is the one qpel path: the filter arithmetic is a minority of the instructions per block, the rest is per-block
 // scaffolding (descriptor shuffles, window re-alignment, destination addressing, stores), so moving the filters to the tensor cores
 // does not pay.  Windows arrive by cp.async rather than TMA: small 2-D boxes (one 48 x 21-byte box per operation) are bound by the
@@ -573,65 +551,6 @@ B200_API int b200_hpeldsp_init(B200HpelDSPContext *c, int flags)
     fill_hpel<1, 0>(c->avg_pixels_tab[0]); fill_hpel<1, 1>(c->avg_pixels_tab[1]); fill_hpel<1, 2>(c->avg_pixels_tab[2]); fill_hpel<1, 3>(c->avg_pixels_tab[3]);
     fill_hpel<2, 0>(c->put_no_rnd_pixels_tab[0]); fill_hpel<2, 1>(c->put_no_rnd_pixels_tab[1]);
     fill_hpel<3, 0>(c->avg_no_rnd_pixels_tab);
-    return 0;
-}
-
-namespace {
-void edge_tab(uint8_t *buf, const uint8_t *src, ptrdiff_t buf_linesize, ptrdiff_t src_linesize, int block_w, int block_h,
-              int src_x, int src_y, int w, int h)
-{
-    if (!w || !h) return;                                          // videodsp_template.c:33-34
-    if (block_w <= 0 || block_h <= 0) return;
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
-    // the part of the picture the window can reach after clamping
-    const int x0 = std::min(std::max(src_x, 0), w - 1), x1 = std::min(std::max(src_x + block_w - 1, 0), w - 1);
-    const int y0 = std::min(std::max(src_y, 0), h - 1), y1 = std::min(std::max(src_y + block_h - 1, 0), h - 1);
-    const size_t rw = (size_t)(x1 - x0 + 1), rh = (size_t)(y1 - y0 + 1);
-    const size_t rp = (rw + 15) & ~(size_t)15, bp = ((size_t)block_w + 15) & ~(size_t)15;
-    B200_LOCK_DEVICE(dev);      // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, rp * rh + bp * block_h + 256);
-    if (!scr) die("scratch");
-    uint8_t *drect = scr, *dbuf = scr + rp * rh, *meta = dbuf + bp * block_h;
-    meta += (16 - ((uintptr_t)meta & 15)) & 15;
-    cudaStream_t st = dev->stream;
-    const uint8_t *pic = src - (ptrdiff_t)src_y * src_linesize - src_x;
-    if (b200_h2d_rows(drect, rp, pic + (ptrdiff_t)y0 * src_linesize + x0, src_linesize, rw, rh, st) != cudaSuccess) die("h2d");
-    struct { int32_t g[4]; int64_t boff, origin; } m = { { block_w, block_h, src_x, src_y }, 0, -((int64_t)y0 * (int64_t)rp + x0) };
-    if (cudaMemcpyAsync(meta, &m, sizeof(m), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d meta");
-    edge_kernel<<<1, 32 * WARPS, 0, st>>>(1, dbuf, (const int64_t *)(meta + 16), (long long)bp, drect, (const int64_t *)(meta + 24),
-                                          (long long)rp, (const int32_t *)meta, w, h);
-    B200_LAUNCHED();
-    if (b200_d2h_rows(buf, buf_linesize, dbuf, bp, (size_t)block_w, (size_t)block_h, st) != cudaSuccess) die("d2h");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
-}
-void prefetch_nop(const uint8_t *, ptrdiff_t, int) {}
-} // namespace
-
-B200_API int b200_videodsp_init(B200VideoDSPContext *c, int bpc)
-{
-    if (!c) return B200_EINVAL;
-    if (!b200_default_device()) return B200_ENODEV;
-    c->emulated_edge_mc = edge_tab;
-    if (bpc > 8) pel_hbd_fill_edge(c);                             // videodsp.c:41-45: the 16 bit template above 8
-    c->prefetch = prefetch_nop;                                    // videodsp.c:34-36: the C prefetch is an empty function
-    return 0;
-}
-
-B200_API int b200_emulated_edge_mc_batch_device(B200Device *dev, int64_t n, uint8_t *buf, const int64_t *buf_off,
-                                                ptrdiff_t buf_linesize, const uint8_t *src, const int64_t *origin,
-                                                ptrdiff_t src_linesize, const int32_t *geom, int w, int h)
-{
-    if (!dev || n < 0 || !buf || !buf_off || !src || !origin || !geom || w < 0 || h < 0) return B200_EINVAL;
-    if (((uintptr_t)geom & 15) != 0) return B200_EINVAL;
-    if (n == 0 || !w || !h) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
-    const long long blocks = (n + WARPS - 1) / WARPS;
-    if (blocks > 0x7fffffffLL) return B200_EINVAL;
-    edge_kernel<<<(unsigned)blocks, 32 * WARPS, 0, dev->stream>>>(n, buf, buf_off, buf_linesize, src, origin, src_linesize, geom, w, h);
-    B200_LAUNCHED();
-    B200_CUDA_OK(cudaGetLastError());
     return 0;
 }
 

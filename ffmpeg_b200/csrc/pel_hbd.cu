@@ -10,7 +10,6 @@
 // This is the plain version (the 8-bit path in pel.cu carries the tuned kernels): 16-bit content is a small share of H.264 streams.
 #include "common.h"
 #include "pel_hbd.h"
-#include <algorithm>
 #include <cstring>
 
 namespace {
@@ -113,27 +112,6 @@ chroma_hbd_kernel(long long n, const uint8_t *__restrict__ op, const uint8_t *__
     }
 }
 
-// emulated_edge_mc for 16-bit samples (videodsp_template.c:24-101 with BIT_DEPTH 16, videodsp.c:41-45): geom[4i..4i+3] = {block_w, block_h,
-// src_x, src_y} in PIXELS, line sizes / offsets in BYTES; samples outside the w x h picture replicate the nearest border sample
-__global__ void __launch_bounds__(32 * HB_WARPS)
-edge_hbd_kernel(long long n, uint8_t *buf, const long long *buf_off, long long buf_ls, const uint8_t *src, const long long *origin,
-                long long src_ls, const int32_t *geom, int w, int h)
-{
-    const long long i = (long long)blockIdx.x * HB_WARPS + (threadIdx.x >> 5);
-    if (i >= n) return;
-    const int lane = threadIdx.x & 31;
-    const int bw = geom[4 * i], bh = geom[4 * i + 1], sx = geom[4 * i + 2], sy = geom[4 * i + 3];
-    const uint8_t *pic = src + origin[i];
-    uint8_t *out = buf + buf_off[i];
-    for (int x = lane; x < bw; x += 32) {
-        const int px = min(max(sx + x, 0), w - 1);
-        for (int y = 0; y < bh; y++) {
-            const int py = min(max(sy + y, 0), h - 1);
-            *reinterpret_cast<unsigned short *>(out + (long long)y * buf_ls + 2 * x) = *reinterpret_cast<const unsigned short *>(pic + (long long)py * src_ls + 2 * px);
-        }
-    }
-}
-
 int chroma_hbd_launch(cudaStream_t st, long long n, const uint8_t *op, const uint8_t *h, const uint8_t *xy, uint8_t *dst, const long long *doff,
                       const uint8_t *src, const long long *soff, long long stride)
 {
@@ -221,36 +199,6 @@ void chroma_hbd_tab(uint8_t *dst, const uint8_t *src, ptrdiff_t stride, int h, i
     if (cudaStreamSynchronize(st) != cudaSuccess) hbd_die("sync");
 }
 
-// VideoDSPContext.emulated_edge_mc for 16-bit samples (host pointers): only the part of the picture the window reaches is copied
-void edge_hbd_tab(uint8_t *buf, const uint8_t *src, ptrdiff_t buf_linesize, ptrdiff_t src_linesize, int block_w, int block_h,
-                  int src_x, int src_y, int w, int h)
-{
-    if (!w || !h) return;                                          // videodsp_template.c:33-34
-    if (block_w <= 0 || block_h <= 0) return;
-    B200Device *dev = b200_default_device();
-    if (!dev) hbd_die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) hbd_die("cudaSetDevice");
-    const int x0 = std::min(std::max(src_x, 0), w - 1), x1 = std::min(std::max(src_x + block_w - 1, 0), w - 1);
-    const int y0 = std::min(std::max(src_y, 0), h - 1), y1 = std::min(std::max(src_y + block_h - 1, 0), h - 1);
-    const size_t rw = (size_t)(x1 - x0 + 1) * 2, rh = (size_t)(y1 - y0 + 1);
-    const size_t rp = (rw + 15) & ~(size_t)15, bp = ((size_t)block_w * 2 + 15) & ~(size_t)15;
-    B200_LOCK_DEVICE(dev);
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, rp * rh + bp * block_h + 256);
-    if (!scr) hbd_die("scratch");
-    uint8_t *drect = scr, *dbuf = scr + rp * rh, *meta = dbuf + bp * block_h;
-    meta += (16 - ((uintptr_t)meta & 15)) & 15;
-    cudaStream_t st = dev->stream;
-    const uint8_t *pic = src - (ptrdiff_t)src_y * src_linesize - (ptrdiff_t)src_x * 2;
-    if (b200_h2d_rows(drect, rp, pic + (ptrdiff_t)y0 * src_linesize + (ptrdiff_t)x0 * 2, src_linesize, rw, rh, st) != cudaSuccess) hbd_die("h2d");
-    struct { int32_t g[4]; long long boff, origin; } m = { { block_w, block_h, src_x, src_y }, 0, -((long long)y0 * (long long)rp + 2LL * x0) };
-    if (cudaMemcpyAsync(meta, &m, sizeof(m), cudaMemcpyHostToDevice, st) != cudaSuccess) hbd_die("h2d meta");
-    edge_hbd_kernel<<<1, 32 * HB_WARPS, 0, st>>>(1, dbuf, (const long long *)(meta + 16), (long long)bp, drect, (const long long *)(meta + 24),
-                                                 (long long)rp, (const int32_t *)meta, w, h);
-    B200_LAUNCHED();
-    if (b200_d2h_rows(buf, buf_linesize, dbuf, bp, (size_t)block_w * 2, (size_t)block_h, st) != cudaSuccess) hbd_die("d2h");
-    if (cudaStreamSynchronize(st) != cudaSuccess) hbd_die("sync");
-}
-
 } // namespace
 
 bool pel_hbd_fill(B200H264QpelContext *c, int bit_depth)
@@ -282,8 +230,6 @@ void pel_hbd_fill_chroma(B200H264ChromaContext *c)
     c->avg_h264_chroma_pixels_tab[0] = chroma_hbd_tab<1, 0>; c->avg_h264_chroma_pixels_tab[1] = chroma_hbd_tab<1, 1>; c->avg_h264_chroma_pixels_tab[2] = chroma_hbd_tab<1, 2>;
 }
 
-void pel_hbd_fill_edge(B200VideoDSPContext *c) { c->emulated_edge_mc = edge_hbd_tab; }
-
 B200_API int b200_h264chroma_hbd_batch_device(B200Device *dev, int64_t n, const uint8_t *op, const uint8_t *h, const uint8_t *xy, uint8_t *dst,
                                               const int64_t *dst_off, const uint8_t *src, const int64_t *src_off, ptrdiff_t stride)
 {
@@ -292,20 +238,4 @@ B200_API int b200_h264chroma_hbd_batch_device(B200Device *dev, int64_t n, const 
     if (n == 0) return 0;
     B200_CUDA_OK(cudaSetDevice(dev->ordinal));
     return chroma_hbd_launch(dev->stream, n, op, h, xy, dst, (const long long *)dst_off, src, (const long long *)src_off, (long long)stride);
-}
-
-B200_API int b200_emulated_edge_mc_hbd_batch_device(B200Device *dev, int64_t n, uint8_t *buf, const int64_t *buf_off, ptrdiff_t buf_linesize,
-                                                    const uint8_t *src, const int64_t *origin, ptrdiff_t src_linesize, const int32_t *geom, int w, int h)
-{
-    if (!dev || n < 0 || !buf || !buf_off || !src || !origin || !geom || w < 0 || h < 0) return B200_EINVAL;
-    if (((buf_linesize | src_linesize) & 1) || ((reinterpret_cast<uintptr_t>(buf) | reinterpret_cast<uintptr_t>(src)) & 1)) return B200_EINVAL;
-    if (n == 0 || !w || !h) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
-    const long long blocks = (n + HB_WARPS - 1) / HB_WARPS;
-    if (blocks > 0x7fffffffLL) return B200_EINVAL;
-    edge_hbd_kernel<<<(unsigned)blocks, 32 * HB_WARPS, 0, dev->stream>>>(n, buf, (const long long *)buf_off, (long long)buf_linesize, src, (const long long *)origin,
-                                                                          (long long)src_linesize, geom, w, h);
-    B200_LAUNCHED();
-    B200_CUDA_OK(cudaGetLastError());
-    return 0;
 }

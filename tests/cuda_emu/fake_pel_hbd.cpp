@@ -18,11 +18,3 @@ extern "C" int emu_host_chroma_hbd_tab(int avg, int idx, uint8_t *dst, const uin
     (avg ? c.avg_h264_chroma_pixels_tab : c.put_h264_chroma_pixels_tab)[idx](dst, src, (ptrdiff_t)stride, h, x, y);
     return 0;
 }
-extern "C" void emu_host_edge_hbd_tab(uint8_t *buf, const uint8_t *src, long long buf_linesize, long long src_linesize, int block_w, int block_h,
-                                      int src_x, int src_y, int w, int h)
-{
-    B200VideoDSPContext c;
-    memset(&c, 0, sizeof(c));
-    pel_hbd_fill_edge(&c);
-    c.emulated_edge_mc(buf, src, (ptrdiff_t)buf_linesize, (ptrdiff_t)src_linesize, block_w, block_h, src_x, src_y, w, h);
-}

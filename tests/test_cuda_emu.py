@@ -78,13 +78,13 @@ def rewrite_launches(txt):
 
 @pytest.fixture(scope="module")
 def emuhost():
-    """libemuhost.so: the translation units without inline PTX (fdsp, unquant, idct_hbd, tx_pfa, h264lf, h264weight, pixelutils, ...), HOST CODE INCLUDED, compiled with
+    """libemuhost.so: the translation units without inline PTX (fdsp, unquant, idct_hbd, tx_pfa, h264lf, h264weight, h264idct, videodsp, ...), HOST CODE INCLUDED, compiled with
     g++ against a stand-in CUDA runtime (tests/cuda_emu/fake/cuda_runtime.h): the library's own entry points run on the CPU"""
     gen = os.path.join(EMU, "_gen")
     os.makedirs(gen, exist_ok=True)
     cs = os.path.join(ROOT, "ffmpeg_b200", "csrc")
     srcs = []
-    for f in ("fdsp.cu", "unquant.cu", "idct_hbd.cu", "tx_pfa.cu", "h264lf.cu", "h264weight.cu", "pixelutils.cu", "pel_hbd.cu", "h264idct_hbd.cu", "mecmp_dct.cu", "fdctdsp.cu"):
+    for f in ("fdsp.cu", "unquant.cu", "idct_hbd.cu", "tx_pfa.cu", "h264lf.cu", "h264weight.cu", "pixelutils.cu", "pel_hbd.cu", "h264idct.cu", "videodsp.cu", "mecmp_dct.cu", "fdctdsp.cu"):
         t = rewrite_launches(open(os.path.join(cs, f)).read())
         t = t.replace("extern __shared__ float2 pfa_z[];", "float2 *pfa_z = (float2 *)emu_smem;")
         assert "<<<" not in t
@@ -94,7 +94,7 @@ def emuhost():
     so = os.path.join(gen, "libemuhost.so")
     cxx = "/opt/gcc/bin/g++" if os.path.exists("/opt/gcc/bin/g++") else "g++"
     r = subprocess.run([cxx, "-std=c++20", "-O1", "-fPIC", "-shared", "-pthread", "-ffp-contract=off", "-w", "-I" + os.path.join(EMU, "fake"), "-I" + cs,
-                        "-I" + os.path.join(ROOT, "include"), "-I" + EMU] + srcs + [os.path.join(EMU, "fake_device.cpp"), os.path.join(EMU, "fake_pel_hbd.cpp"), os.path.join(EMU, "fake_h264idct_hbd.cpp"), os.path.join(EMU, "fake_mecmp_dct.cpp"), "-o", so],
+                        "-I" + os.path.join(ROOT, "include"), "-I" + EMU] + srcs + [os.path.join(EMU, "fake_device.cpp"), os.path.join(EMU, "fake_pel_hbd.cpp"), os.path.join(EMU, "fake_mecmp_dct.cpp"), "-o", so],
                        capture_output=True, text=True)
     assert r.returncode == 0, r.stderr[-3000:]
     return C.CDLL(so)
@@ -1336,13 +1336,13 @@ def test_host_h264qpel_hbd(emuhost):
 
 
 def test_host_chroma_and_edge_hbd(emuhost):
-    """pel_hbd.cu: h264chroma and emulated_edge_mc for 16-bit samples, batched device entries and drop-in table functions on the stand-in
-    runtime against the checker (every eighth-pel phase, put / avg, widths 8 / 4 / 2; windows on and beyond every picture border)"""
+    """pel_hbd.cu: h264chroma for 16-bit samples, and videodsp.cu: emulated_edge_mc for 16-bit and 8-bit samples; batched device entries and
+    drop-in table functions on the stand-in runtime against the checker (every eighth-pel phase, put / avg, widths 8 / 4 / 2; windows on and
+    beyond every picture border)"""
     L, O = emuhost, cl.oracle()
     L.b200_h264chroma_hbd_batch_device.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 7 + [C.c_ssize_t]
     L.b200_emulated_edge_mc_hbd_batch_device.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_int, C.c_int]
     L.emu_host_chroma_hbd_tab.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_int, C.c_int]
-    L.emu_host_edge_hbd_tab.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong, C.c_longlong] + [C.c_int] * 6
     O.orc_h264chroma_hbd.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_int, C.c_int, C.c_int]
     O.orc_emulated_edge_mc_hbd.argtypes = [C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_ssize_t] + [C.c_int] * 6
     dev = C.c_void_p()
@@ -1381,25 +1381,36 @@ def test_host_chroma_and_edge_hbd(emuhost):
             assert L.emu_host_chroma_hbd_tab(*args, got.ctypes.data + off, img.ctypes.data + off, Wd * 2, hs[j], xys[j] & 7, xys[j] >> 3) == 0
             O.orc_h264chroma_hbd(*args, exp.ctypes.data + off, img.ctypes.data + off, Wd * 2, hs[j], xys[j] & 7, xys[j] >> 3)
             assert np.array_equal(got, exp), (depth, "tab", j)
-    pic = rng.integers(0, 1024, (30, 41)).astype(np.uint16)
-    geoms, origins, boffs = [], [], []
-    BW = 32
-    for it in range(60):
-        bw, bh = int(rng.integers(1, 25)), int(rng.integers(1, 25))
-        sx, sy = int(rng.integers(-30, 60)), int(rng.integers(-30, 50))
-        geoms.append((bw, bh, sx, sy)); origins.append(0); boffs.append(it * 25 * BW * 2)
-        got, exp = np.zeros((bh, bw + 3), np.uint16), np.zeros((bh, bw + 3), np.uint16)
-        src = pic.ctypes.data + sy * pic.strides[0] + sx * 2
-        L.emu_host_edge_hbd_tab(got.ctypes.data, src, got.strides[0], pic.strides[0], bw, bh, sx, sy, 41, 30)
-        O.orc_emulated_edge_mc_hbd(exp.ctypes.data, src, exp.strides[0], pic.strides[0], bw, bh, sx, sy, 41, 30)
-        assert np.array_equal(got, exp), ("edge tab", bw, bh, sx, sy)
-    g = np.array(geoms, np.int32); og = np.array(origins, np.int64); bo = np.array(boffs, np.int64)
-    buf = np.zeros((60 * 25, BW), np.uint16)
-    assert L.b200_emulated_edge_mc_hbd_batch_device(dev, 60, buf.ctypes.data, bo.ctypes.data, BW * 2, pic.ctypes.data, og.ctypes.data, pic.strides[0], g.ctypes.data, 41, 30) == 0
-    for it, (bw, bh, sx, sy) in enumerate(geoms):
-        exp = np.zeros((bh, bw), np.uint16)
-        O.orc_emulated_edge_mc_hbd(exp.ctypes.data, pic.ctypes.data + sy * pic.strides[0] + sx * 2, exp.strides[0], pic.strides[0], bw, bh, sx, sy, 41, 30)
-        assert np.array_equal(buf[it * 25:it * 25 + bh, :bw], exp), ("edge batch", it)
+    # emulated_edge_mc: the member b200_videodsp_init installs and the batched entry, 16-bit samples (bpc 10), then 8-bit
+    from ffmpeg_b200._lib import VideoDSPContext
+    L.b200_emulated_edge_mc_batch_device.argtypes = L.b200_emulated_edge_mc_hbd_batch_device.argtypes
+    orc8 = lambda b, *a: O.orc_emulated_edge_mc(C.cast(b, cl.u8p), *a)
+    for bpc, dt, orc, batch in ((10, np.uint16, O.orc_emulated_edge_mc_hbd, L.b200_emulated_edge_mc_hbd_batch_device),
+                                (8, np.uint8, orc8, L.b200_emulated_edge_mc_batch_device)):
+        vd = VideoDSPContext()
+        assert L.b200_videodsp_init(C.byref(vd), bpc) == 0
+        bps = np.dtype(dt).itemsize
+        pic = rng.integers(0, 1 << bpc, (30, 41)).astype(dt)
+        geoms, origins, boffs = [], [], []
+        BW = 32
+        for it in range(60):
+            bw, bh = int(rng.integers(1, 25)), int(rng.integers(1, 25))
+            sx, sy = int(rng.integers(-30, 60)), int(rng.integers(-30, 50))
+            geoms.append((bw, bh, sx, sy)); origins.append(0); boffs.append(it * 25 * BW * bps)
+            got, exp = np.zeros((bh, bw + 3), dt), np.zeros((bh, bw + 3), dt)
+            src = pic.ctypes.data + sy * pic.strides[0] + sx * bps
+            vd.emulated_edge_mc(got.ctypes.data, src, got.strides[0], pic.strides[0], bw, bh, sx, sy, 41, 30)
+            orc(exp.ctypes.data, src, exp.strides[0], pic.strides[0], bw, bh, sx, sy, 41, 30)
+            assert np.array_equal(got, exp), ("edge tab", bpc, bw, bh, sx, sy)
+        g = _aligned((60 * 16,)).view(np.int32).reshape(60, 4)     # the 8-bit entry wants 16-byte-aligned geom
+        g[...] = geoms
+        og, bo = np.array(origins, np.int64), np.array(boffs, np.int64)
+        buf = np.zeros((60 * 25, BW), dt)
+        assert batch(dev, 60, buf.ctypes.data, bo.ctypes.data, BW * bps, pic.ctypes.data, og.ctypes.data, pic.strides[0], g.ctypes.data, 41, 30) == 0
+        for it, (bw, bh, sx, sy) in enumerate(geoms):
+            exp = np.zeros((bh, bw), dt)
+            orc(exp.ctypes.data, pic.ctypes.data + sy * pic.strides[0] + sx * bps, exp.strides[0], pic.strides[0], bw, bh, sx, sy, 41, 30)
+            assert np.array_equal(buf[it * 25:it * 25 + bh, :bw], exp), ("edge batch", bpc, it)
 
 
 def test_host_h264_weight_hbd(emuhost):
@@ -1443,33 +1454,70 @@ def test_host_h264_weight_hbd(emuhost):
 
 
 def test_host_h264_idct_hbd(emuhost):
-    """h264idct_hbd.cu (residual adds for 9 / 10 / 12 / 14 bit samples, int32 coefficients) with its host code on the stand-in runtime: the member
-    functions and the batched device entry against the hashes of the compiled reference's outputs and the checker"""
+    """h264idct.cu (H.264 residual adds) with its host code on the stand-in runtime: the members b200_h264_idct_init installs and the batched
+    device entries.  9 / 10 / 12 / 14 bit (int32 coefficients) against the hashes of the compiled reference's outputs and the checker, 8 bit
+    (int16 coefficients) against the checker"""
+    from ffmpeg_b200._lib import H264IDCTContext
     from test_oracle_more import h264_idct_hbd_hashes, run_h264_idct_hbd_case
     L, O = emuhost, cl.oracle()
-    L.emu_host_h264_idct_hbd.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_longlong]
     L.b200_h264_idct_hbd_batch_device.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_ssize_t]
+    L.b200_h264_idct_batch_device.argtypes = [C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_ssize_t]
     O.orc_h264_idct_hbd.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_ssize_t]
     dev = C.c_void_p()
     assert L.b200_device_open(C.byref(dev), 0, None) == 0
+
+    def members(depth):
+        c = H264IDCTContext()
+        assert L.b200_h264_idct_init(C.byref(c), depth, 1) == 0
+        m = [c.idct_add, c.idct8_add, c.idct_dc_add, c.idct8_dc_add]
+        return lambda dp, kind, d, b, st: m[kind](C.cast(d, cl.u8p), C.cast(b, cl.i16p), st)
+
+    def aligned(a):
+        out = _aligned((a.nbytes,)).view(a.dtype).reshape(a.shape)
+        out[...] = a
+        return out
     hs = h264_idct_hbd_hashes()
     for depth in (9, 10, 12, 14):
+        fn = members(depth)
         for kind in range(4):
             cases = cl.h264_idct_hbd_cases(depth, kind)
             for k, case in enumerate(cases[:10]):
-                assert run_h264_idct_hbd_case(L.emu_host_h264_idct_hbd, depth, kind, case) == hs[(depth, kind, k)], (depth, kind, k)
-            # batch: all 24 blocks into one 48 x 64 picture (8 x 8 grid cells), coefficient blocks back to back
+                assert run_h264_idct_hbd_case(fn, depth, kind, case) == hs[(depth, kind, k)], (depth, kind, k)
+            # batch: all 24 blocks into one 48 x 64 picture (8 x 8 grid cells), coefficient blocks back to back; at 16-byte-aligned
+            # destinations (row accesses), then shifted by one sample (sample accesses)
             N = 64 if kind & 1 else 16
             blocks = np.concatenate([c[0] for c in cases]).astype(np.int32)
             boff = np.arange(len(cases), dtype=np.int64) * N
-            doff = np.array([((k // 6) * 8 * 64 + (k % 6) * 8) * 2 for k in range(len(cases))], np.int64)
-            pic = np.random.default_rng(depth * 10 + kind).integers(0, 1 << depth, (48, 64)).astype(np.uint16)
-            got, exp, gb, eb = pic.copy(), pic.copy(), blocks.copy(), blocks.copy()
-            assert L.b200_h264_idct_hbd_batch_device(dev, depth, kind, len(cases), gb.ctypes.data, boff.ctypes.data, got.ctypes.data, doff.ctypes.data, 128) == 0
-            for k in range(len(cases)):
-                O.orc_h264_idct_hbd(depth, kind, exp.ctypes.data + int(doff[k]), eb.ctypes.data + 4 * int(boff[k]), 128)
-            assert np.array_equal(got, exp) and np.array_equal(gb, eb), (depth, kind)
-    assert L.emu_host_h264_idct_hbd(11, 0, None, None, 0) == -38
+            pic = aligned(np.random.default_rng(depth * 10 + kind).integers(0, 1 << depth, (48, 64)).astype(np.uint16))
+            for shift in (0, 2):
+                doff = np.array([((k // 6) * 8 * 64 + (k % 6) * 8) * 2 + shift for k in range(len(cases))], np.int64)
+                got, exp, gb, eb = pic.copy(), pic.copy(), blocks.copy(), blocks.copy()
+                assert L.b200_h264_idct_hbd_batch_device(dev, depth, kind, len(cases), gb.ctypes.data, boff.ctypes.data, got.ctypes.data, doff.ctypes.data, 128) == 0
+                for k in range(len(cases)):
+                    O.orc_h264_idct_hbd(depth, kind, exp.ctypes.data + int(doff[k]), eb.ctypes.data + 4 * int(boff[k]), 128)
+                assert np.array_equal(got, exp) and np.array_equal(gb, eb), (depth, kind, shift)
+    # 8 bit: int16 coefficients up to the full range (the stores into dctcoef wrap), the same 12 x 16 pictures and 48 x 64 batch layout
+    fn = members(8)
+    for kind in range(4):
+        rng = np.random.default_rng(70 + kind)
+        N = 64 if kind & 1 else 16
+        blocks = np.stack([rng.integers(-amp, amp, N) for amp in [300, 4000, 32768] * 8]).astype(np.int16)
+        blocks[::7, 1:] = 0
+        for k in range(10):
+            d, b = rng.integers(0, 256, (12, 16)).astype(np.uint8), blocks[k].copy()
+            ed, eb = d.copy(), b.copy()
+            fn(8, kind, d.ctypes.data + 2 * 16 + 4, b.ctypes.data, 16)
+            O.orc_h264_idct(kind, C.cast(ed.ctypes.data + 2 * 16 + 4, cl.u8p), cl.ptr(eb, cl.i16p), 16)
+            assert np.array_equal(d, ed) and np.array_equal(b, eb), (kind, k)
+        pic = aligned(rng.integers(0, 256, (48, 64)).astype(np.uint8))
+        doff = np.array([(k // 6) * 8 * 64 + (k % 6) * 8 for k in range(len(blocks))], np.int64)
+        boff = np.arange(len(blocks), dtype=np.int64) * N
+        got, exp, gb, eb = pic.copy(), pic.copy(), aligned(blocks), blocks.copy()
+        assert L.b200_h264_idct_batch_device(dev, kind, len(blocks), gb.ctypes.data, boff.ctypes.data, got.ctypes.data, doff.ctypes.data, 64) == 0
+        for k in range(len(blocks)):
+            O.orc_h264_idct(kind, C.cast(exp.ctypes.data + int(doff[k]), cl.u8p), cl.ptr(eb[k], cl.i16p), 64)
+        assert np.array_equal(got, exp) and np.array_equal(gb, eb), kind
+    assert L.b200_h264_idct_init(C.byref(H264IDCTContext()), 11, 1) == -38
 
 
 def test_host_tx_pfa_create_and_launch(emuhost):

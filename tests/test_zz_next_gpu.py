@@ -1114,19 +1114,21 @@ def test_h264_idct_hbd(device):
         N, B = (64, 8) if kind & 1 else (16, 4)
         nb = (W // B) * (H // B)
         blocks = rng.integers(-3000, 3000, (nb, N)).astype(np.int32)
-        pic = rng.integers(0, 1 << depth, (H, W)).astype(np.uint16)
+        # one spare row: the last block shifted by a sample ends a sample into it
+        pic = rng.integers(0, 1 << depth, (H + 1, W)).astype(np.uint16)
         boff = np.arange(nb, dtype=np.int64) * N
-        doff = np.array([((k // (W // B)) * B * W + (k % (W // B)) * B) * 2 for k in range(nb)], np.int64)
-        exp, eb = pic.copy(), blocks.copy()
-        for k in range(nb):
-            O.orc_h264_idct_hbd(depth, kind, exp.ctypes.data + int(doff[k]), eb.ctypes.data + 4 * int(boff[k]), W * 2)
-        with on_stream(device):
-            d_b, d_bo, d_do = torch.from_numpy(blocks).cuda(), torch.from_numpy(boff).cuda(), torch.from_numpy(doff).cuda()
-            d_p = torch.from_numpy(pic.view(np.int16)).cuda()
-            check(lib().b200_h264_idct_hbd_batch_device(device.handle, depth, kind, nb, vp(d_b.data_ptr()), vp(d_bo.data_ptr()), vp(d_p.data_ptr()), vp(d_do.data_ptr()), W * 2), "h264_idct_hbd_batch")
-            device.sync()
-            got, gb = d_p.cpu().numpy().view(np.uint16), d_b.cpu().numpy()
-        assert np.array_equal(got, exp) and np.array_equal(gb, eb), kind
+        for shift in (0, 2):                                        # aligned rows (one access per row), then one sample further
+            doff = np.array([((k // (W // B)) * B * W + (k % (W // B)) * B) * 2 + shift for k in range(nb)], np.int64)
+            exp, eb = pic.copy(), blocks.copy()
+            for k in range(nb):
+                O.orc_h264_idct_hbd(depth, kind, exp.ctypes.data + int(doff[k]), eb.ctypes.data + 4 * int(boff[k]), W * 2)
+            with on_stream(device):
+                d_b, d_bo, d_do = torch.from_numpy(blocks).cuda(), torch.from_numpy(boff).cuda(), torch.from_numpy(doff).cuda()
+                d_p = torch.from_numpy(pic.view(np.int16)).cuda()
+                check(lib().b200_h264_idct_hbd_batch_device(device.handle, depth, kind, nb, vp(d_b.data_ptr()), vp(d_bo.data_ptr()), vp(d_p.data_ptr()), vp(d_do.data_ptr()), W * 2), "h264_idct_hbd_batch")
+                device.sync()
+                got, gb = d_p.cpu().numpy().view(np.uint16), d_b.cpu().numpy()
+            assert np.array_equal(got, exp) and np.array_equal(gb, eb), (kind, shift)
 
 
 # ---------------------------------------------------------------------------------------------- H.264 deblocking, 16-bit samples

@@ -198,6 +198,28 @@ class HEVCPredContext(C.Structure):
                 ("ref_filter_strong", vp)]
 
 
+VP9_MC_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_ssize_t, C.c_int, C.c_int, C.c_int)
+VP9_SCALED_MC_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_ssize_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int)
+
+
+class VP9DSPContext(C.Structure):
+    """libavcodec/vp9dsp.h:40-122 (same member order; the members this library does not fill are plain pointers here)"""
+    _fields_ = [("intra_pred", vp * 15 * 4), ("itxfm_add", vp * 4 * 5), ("loop_filter_8", vp * 2 * 3), ("loop_filter_16", vp * 2),
+                ("loop_filter_mix2", vp * 2 * 2 * 2), ("mc", VP9_MC_FUNC * 2 * 2 * 2 * 4 * 5), ("smc", VP9_SCALED_MC_FUNC * 2 * 4 * 5)]
+
+
+class Vp9McRef(C.Structure):
+    """B200Vp9McRef (include/b200dsp.h), 32 bytes"""
+    _fields_ = [("data", C.c_void_p), ("stride", C.c_ssize_t), ("w", C.c_int32), ("h", C.c_int32), ("dx", C.c_int32), ("dy", C.c_int32)]
+
+
+class Vp9McOp(C.Structure):
+    """B200Vp9McOp (include/b200dsp.h), 40 bytes"""
+    _fields_ = [("dst_off", C.c_int64), ("x", C.c_int32 * 2), ("y", C.c_int32 * 2), ("ref", C.c_uint8 * 2), ("mx", C.c_uint8 * 2),
+                ("my", C.c_uint8 * 2), ("w", C.c_uint8), ("h", C.c_uint8), ("filter", C.c_uint8), ("kind", C.c_uint8),
+                ("reserved", C.c_uint8 * 6)]
+
+
 class ProresDSPContext(C.Structure):
     """libavcodec/proresdsp.h:28-35"""
     _fields_ = [("idct_permutation_type", C.c_int), ("idct_permutation", C.c_uint8 * 64),
@@ -318,6 +340,8 @@ PROTOTYPES = {
     "b200_hevc_pred_init": (C.c_int, [vp, C.c_int]),
     "b200_hevc_intra_pred_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_ssize_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64, vp, vp,
                                                     C.c_ssize_t, C.c_int]),
+    "b200_vp9_dsp_init": (C.c_int, [vp, C.c_int]),
+    "b200_vp9_mc_batch_device": (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_int64, vp, vp, C.c_ssize_t]),
     "b200_proresdsp_init": (C.c_int, [vp, C.c_int]),
     "b200_prores_idct_put_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, vp, vp, vp, C.c_int]),
     "b200_float_dsp_init": (C.c_int, [vp]),

@@ -1,0 +1,36 @@
+"""Host-side mirror of libavcodec's VP9 DSP: the mc / smc tables of VP9DSPContext as ff_vp9dsp_init installs them
+(libavcodec/vp9dsp_template.c:2302-2361, :2540-2569) and the batched device entry b200_vp9_mc_batch_device."""
+import ctypes as C
+
+import numpy as np
+
+from ._lib import lib, check, vp, VP9DSPContext, Vp9McRef, Vp9McOp, VP9_MC_FUNC, VP9_SCALED_MC_FUNC  # noqa: F401
+
+SINGLE, COMPOUND = range(2)                                          # B200Vp9McOp.kind
+FILTER_8TAP_SMOOTH, FILTER_8TAP_REGULAR, FILTER_8TAP_SHARP, FILTER_BILINEAR = range(4)   # B200Vp9McOp.filter, libavcodec/vp9.h:64-71
+MAX_REFS = 8
+OP_DTYPE = np.dtype([("dst_off", "<i8"), ("x", "<i4", 2), ("y", "<i4", 2), ("ref", "u1", 2), ("mx", "u1", 2), ("my", "u1", 2),
+                     ("w", "u1"), ("h", "u1"), ("filter", "u1"), ("kind", "u1"), ("reserved", "u1", 6)])
+assert OP_DTYPE.itemsize == C.sizeof(Vp9McOp) == 40
+
+
+def _dptr(x):
+    return int(x.data_ptr()) if hasattr(x, "data_ptr") else int(x)
+
+
+def ff_vp9dsp_init(bit_depth=8):
+    """VP9DSPContext with mc[5][4][2][2][2] and smc[5][4][2] filled (HOST pointers), every other member NULL"""
+    c = VP9DSPContext()
+    check(lib().b200_vp9_dsp_init(C.byref(c), bit_depth), "ff_vp9dsp_init")
+    return c
+
+
+def vp9_mc_batch_device(device, bit_depth, refs, nops, ops, dst, dst_stride):
+    """one plane's inter blocks; refs = up to 8 (plane, stride, w, h, dx, dy) with plane a sample tensor or device address of sample
+    (0, 0), stride in bytes, steps in sixteenths (16, 16 = same size as the current picture); ops = OP_DTYPE records (a uint8 tensor of
+    nops * 40 bytes); dst a sample tensor, dst_stride in bytes (device)"""
+    arr = (Vp9McRef * max(1, len(refs)))()
+    for k, (plane, stride, w, h, dx, dy) in enumerate(refs):
+        arr[k] = Vp9McRef(_dptr(plane), stride, w, h, dx, dy)
+    return check(lib().b200_vp9_mc_batch_device(device.handle, bit_depth, len(refs), C.cast(arr, vp), nops, vp(_dptr(ops)), vp(_dptr(dst)),
+                                                dst_stride), "vp9_mc_batch_device")

@@ -654,6 +654,88 @@ int  b200_hevc_intra_pred_batch_device(B200Device *dev, int bit_depth, uint8_t *
                                        int vshift, int64_t nops, const B200HevcIntraOp *ops, const uint8_t *intra_map, ptrdiff_t map_stride,
                                        int log2_min_pu_size);
 
+/* VP9 motion compensation: VP9DSPContext (libavcodec/vp9dsp.h:40-122) in the reference's member order and types.
+ * b200_vp9_dsp_init() fills mc[5][4][2][2][2] and smc[5][4][2] completely, as ff_vp9dsp_init does through ff_vp9dsp_mc_init
+ * (vp9dsp_template.c:2302-2361) and ff_vp9dsp_scaled_mc_init (:2540-2569): [size 0..4 = 64, 32, 16, 8, 4 columns][filter bank in
+ * FilterMode order: smooth, regular, sharp, bilinear (vp9.h:64-71)][0 put, 1 avg][filters horizontally][filters vertically]; the four
+ * [0][0] full-pel entries of a size and put / avg are one function, as in the reference (:2308-2322).  Every other member stays NULL.
+ * HOST pointers, the reference's signatures: samples uint8 at 8 bit and uint16 at 10 / 12, strides in bytes, h 1..64, mx / my 0..15
+ * (sixteenths), dx / dy 1..32 (sixteenths of a source sample per output sample: the range the reference's tmp[64 * 135] allows,
+ * :2369-2370, a reference 2x larger to 16x smaller).
+ *   8-tap banks  clip((sum F[k] * src[-3 + k] + 64) >> 7), F = ff_vp9_subpel_filters[bank][phase] (vp9dsp.c:32-85, the subpel_filters
+ *                of the VP9 bitstream specification); in two dimensions the horizontal results are clipped samples for rows -3 .. h + 3
+ *                and the vertical pass filters those (FILTER_8TAP :2026-2034, do_8tap_2d_c :2076-2113)
+ *   bilinear     src[0] + ((m * (src[1] - src[0]) + 8) >> 4), no clip (:2150-2151), the horizontal results for rows 0 .. h
+ *   put          dst = v;   avg: dst = (dst + v + 1) >> 1
+ *   smc          source column of output column x is (mx + x * dx) >> 4 with phase (mx + x * dx) & 15, likewise rows with my, dy;
+ *                always both passes (do_scaled_8tap_c :2363-2409, do_scaled_bilin_c :2439-2482)
+ * A member filters in the directions its table position names, with the phase it is handed: phase 0 in a filtered direction is the
+ * identity row { 0, 0, 0, 128, 0, 0, 0, 0 } / bilinear weight 0.  It reads exactly the samples its reference function reads: columns
+ * -3..+4 around the block only where it filters horizontally with an 8-tap bank, 0..+1 for bilinear, the same for rows; an smc member
+ * always the window of (((w - 1) * dx + mx) >> 4) + 8 columns by (((h - 1) * dy + my) >> 4) + 8 rows from (-3, -3) for an 8-tap bank,
+ * + 2 from (0, 0) for bilinear.  A call with h, a phase or a step outside these ranges writes nothing and records the reason
+ * (b200_last_error()). */
+typedef void (*b200_vp9_mc_func)(uint8_t *dst, ptrdiff_t dst_stride, const uint8_t *ref, ptrdiff_t ref_stride, int h, int mx, int my);
+typedef void (*b200_vp9_scaled_mc_func)(uint8_t *dst, ptrdiff_t dst_stride, const uint8_t *ref, ptrdiff_t ref_stride, int h, int mx, int my,
+                                        int dx, int dy);
+typedef struct B200VP9DSPContext {
+    void (*intra_pred[4][15])(uint8_t *dst, ptrdiff_t stride, const uint8_t *left, const uint8_t *top);
+    void (*itxfm_add[5][4])(uint8_t *dst, ptrdiff_t stride, int16_t *block, int eob);
+    void (*loop_filter_8[3][2])(uint8_t *dst, ptrdiff_t stride, int mb_lim, int lim, int hev_thr);
+    void (*loop_filter_16[2])(uint8_t *dst, ptrdiff_t stride, int mb_lim, int lim, int hev_thr);
+    void (*loop_filter_mix2[2][2][2])(uint8_t *dst, ptrdiff_t stride, int mb_lim, int lim, int hev_thr);
+    b200_vp9_mc_func mc[5][4][2][2][2];
+    b200_vp9_scaled_mc_func smc[5][4][2];
+} B200VP9DSPContext;
+/* 0; B200_EINVAL for c == NULL; B200_ENOSYS for depths other than 8, 10 and 12 (the reference asserts there, vp9dsp.c:95);
+ * B200_ENODEV. */
+int  b200_vp9_dsp_init(B200VP9DSPContext *c, int bit_depth);
+
+/* One reference plane of b200_vp9_mc_batch_device: `data` is the DEVICE address of its sample (0, 0), `stride` in bytes, w x h its size
+ * in samples, dx / dy its scale steps in sixteenths (vp9.c: s->mvstep[ref]).  dx == dy == 16 is a reference of the current picture's
+ * size, predicted through the mc table; any other pair in 1..32 goes through smc (the decoder's switch, vp9recon.c:426-429). */
+typedef struct B200Vp9McRef {
+    const uint8_t *data;
+    ptrdiff_t stride;
+    int32_t w, h;
+    int32_t dx, dy;
+} B200Vp9McRef;
+/* One inter block of b200_vp9_mc_batch_device: w (4, 8, 16, 32, 64) x h (1..64) samples at dst + dst_off (bytes), filter bank 0..3
+ * (FilterMode order).  Slot r (0; and 1 for COMPOUND) predicts from reference ref[r] of the call's array: integer sample position
+ * (x[r], y[r]) in that plane (any value) and phase (mx[r], my[r]) in sixteenths, 0..15.  These are the values the decoder has after
+ * its motion-vector arithmetic: mc_luma_unscaled (vp9recon.c:309-313, with mx << 1, my << 1 as at :336), mc_chroma_unscaled
+ * (:349-356), and for scaled references the clipped and scaled vectors of mc_luma_scaled (:437-449) / mc_chroma_scaled (:497-520).
+ *   B200_VP9_MC_SINGLE    mc[size][filter][0][!!mx0][!!my0] (smc[size][filter][0] for a scaled reference) from slot 0
+ *   B200_VP9_MC_COMPOUND  the same, then mc[size][filter][1][!!mx1][!!my1] / smc[size][filter][1] from slot 1 into the same block
+ *                         (vp9_mc_template.c); the two slots may name references of different size and steps */
+enum { B200_VP9_MC_SINGLE = 0, B200_VP9_MC_COMPOUND = 1 };
+typedef struct B200Vp9McOp {
+    int64_t dst_off;
+    int32_t x[2], y[2];
+    uint8_t ref[2];
+    uint8_t mx[2], my[2];
+    uint8_t w, h, filter, kind;
+    uint8_t reserved[6];
+} B200Vp9McOp;
+#ifdef __cplusplus
+static_assert(sizeof(B200Vp9McOp) == 40, "B200Vp9McOp is 40 bytes");
+#else
+_Static_assert(sizeof(B200Vp9McOp) == 40, "B200Vp9McOp is 40 bytes");
+#endif
+/* Batched VP9 inter prediction of one plane: `refs` is a HOST array of 1 <= nrefs <= 8 planes (copied into the launch), `ops` and
+ * `dst` are DEVICE pointers.  Every op's result is the reference's call sequence above with each output sample stored once, its
+ * source samples read through coordinates clamped to [0, w) x [0, h) of that reference.  This is what the decoder's
+ * emulated_edge_mc windows give, windows wholly outside the picture included, because whenever the decoder does not emulate, every
+ * sample the function reads lies inside the picture (vp9recon.c:325-335, :460-468), so no separate edge emulation pass is needed.
+ * The caller guarantees that the ops of one call write disjoint blocks and that no op reads samples another op of the call writes.
+ * An op with an undefined kind, filter or width, a reference index >= nrefs, h outside 1..64, a phase above 15 or, at 10 / 12 bit,
+ * an odd dst_off writes nothing.  Offsets are 64-bit; more ops than one launch takes are split inside the entry.
+ * Returns 0, or B200_EINVAL (launching nothing) for NULL pointers, nops < 0, nrefs outside 1..8, a stride or pointer not a multiple
+ * of the sample size, ops not aligned to 8 bytes, a reference with w or h < 1 or a step outside 1..32, or a depth other than 8, 10
+ * or 12; nops == 0 returns 0. */
+int  b200_vp9_mc_batch_device(B200Device *dev, int bit_depth, int nrefs, const B200Vp9McRef *refs, int64_t nops, const B200Vp9McOp *ops,
+                              uint8_t *dst, ptrdiff_t dst_stride);
+
 /* mpegvideo inverse quantisers: the members of MPVUnquantDSPContext (libavcodec/mpegvideo_unquantize.h:31-44) as
  * ff_mpv_unquantize_init() installs them (libavcodec/mpegvideo_unquantize.c:50-290), i.e. what runs in front of the IDCT in
  * mpv_reconstruct_mb's put_dct / add_dequant_dct (libavcodec/mpegvideo_dec.c).  The reference functions take the whole

@@ -220,6 +220,15 @@ class Vp9McOp(C.Structure):
                 ("reserved", C.c_uint8 * 6)]
 
 
+VP9_ITXFM_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_int)
+
+
+class Vp9TxOp(C.Structure):
+    """B200Vp9TxOp (include/b200dsp.h), 24 bytes"""
+    _fields_ = [("dst_off", C.c_int64), ("coef_off", C.c_int64), ("tx", C.c_uint8), ("type", C.c_uint8), ("eob", C.c_uint16),
+                ("reserved", C.c_uint8 * 4)]
+
+
 class ProresDSPContext(C.Structure):
     """libavcodec/proresdsp.h:28-35"""
     _fields_ = [("idct_permutation_type", C.c_int), ("idct_permutation", C.c_uint8 * 64),
@@ -342,6 +351,8 @@ PROTOTYPES = {
                                                     C.c_ssize_t, C.c_int]),
     "b200_vp9_dsp_init": (C.c_int, [vp, C.c_int]),
     "b200_vp9_mc_batch_device": (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_int64, vp, vp, C.c_ssize_t]),
+    "b200_vp9_dsp_init_itxfm": (C.c_int, [vp, C.c_int]),
+    "b200_vp9_itxfm_add_batch_device": (C.c_int, [vp, C.c_int, C.c_int64, vp, vp, vp, C.c_ssize_t]),
     "b200_proresdsp_init": (C.c_int, [vp, C.c_int]),
     "b200_prores_idct_put_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, vp, vp, vp, C.c_int]),
     "b200_float_dsp_init": (C.c_int, [vp]),

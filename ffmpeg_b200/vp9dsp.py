@@ -1,10 +1,11 @@
 """Host-side mirror of libavcodec's VP9 DSP: the mc / smc tables of VP9DSPContext as ff_vp9dsp_init installs them
-(libavcodec/vp9dsp_template.c:2302-2361, :2540-2569) and the batched device entry b200_vp9_mc_batch_device."""
+(libavcodec/vp9dsp_template.c:2302-2361, :2540-2569) and the batched device entry b200_vp9_mc_batch_device; the itxfm_add members
+(vp9dsp_template.c:1755-1778) and b200_vp9_itxfm_add_batch_device."""
 import ctypes as C
 
 import numpy as np
 
-from ._lib import lib, check, vp, VP9DSPContext, Vp9McRef, Vp9McOp, VP9_MC_FUNC, VP9_SCALED_MC_FUNC  # noqa: F401
+from ._lib import lib, check, vp, VP9DSPContext, Vp9McRef, Vp9McOp, VP9_MC_FUNC, VP9_SCALED_MC_FUNC, Vp9TxOp, VP9_ITXFM_FUNC  # noqa: F401
 
 SINGLE, COMPOUND = range(2)                                          # B200Vp9McOp.kind
 FILTER_8TAP_SMOOTH, FILTER_8TAP_REGULAR, FILTER_8TAP_SHARP, FILTER_BILINEAR = range(4)   # B200Vp9McOp.filter, libavcodec/vp9.h:64-71
@@ -12,6 +13,10 @@ MAX_REFS = 8
 OP_DTYPE = np.dtype([("dst_off", "<i8"), ("x", "<i4", 2), ("y", "<i4", 2), ("ref", "u1", 2), ("mx", "u1", 2), ("my", "u1", 2),
                      ("w", "u1"), ("h", "u1"), ("filter", "u1"), ("kind", "u1"), ("reserved", "u1", 6)])
 assert OP_DTYPE.itemsize == C.sizeof(Vp9McOp) == 40
+DCT_DCT, DCT_ADST, ADST_DCT, ADST_ADST = range(4)                     # B200Vp9TxOp.type, libavcodec/vp9.h TxfmType
+TX_4X4, TX_8X8, TX_16X16, TX_32X32, TX_LOSSLESS = range(5)            # B200Vp9TxOp.tx
+TX_DTYPE = np.dtype([("dst_off", "<i8"), ("coef_off", "<i8"), ("tx", "u1"), ("type", "u1"), ("eob", "<u2"), ("reserved", "u1", 4)])
+assert TX_DTYPE.itemsize == C.sizeof(Vp9TxOp) == 24
 
 
 def _dptr(x):
@@ -34,3 +39,17 @@ def vp9_mc_batch_device(device, bit_depth, refs, nops, ops, dst, dst_stride):
         arr[k] = Vp9McRef(_dptr(plane), stride, w, h, dx, dy)
     return check(lib().b200_vp9_mc_batch_device(device.handle, bit_depth, len(refs), C.cast(arr, vp), nops, vp(_dptr(ops)), vp(_dptr(dst)),
                                                 dst_stride), "vp9_mc_batch_device")
+
+
+def ff_vp9dsp_init_itxfm(ctx, bit_depth=8):
+    """fills ctx.itxfm_add (HOST pointers, plain addresses in the VP9DSPContext mirror: call one through
+    VP9_ITXFM_FUNC(ctx.itxfm_add[tx][type])) and touches no other member; returns ctx"""
+    check(lib().b200_vp9_dsp_init_itxfm(C.byref(ctx), bit_depth), "ff_vp9dsp_init_itxfm")
+    return ctx
+
+
+def vp9_itxfm_add_batch_device(device, bit_depth, nops, ops, coef, dst, dst_stride):
+    """one plane's transform blocks: ops = TX_DTYPE records (a uint8 tensor of nops * 24 bytes), coef = int16 (8 bit) / int32 (10 / 12
+    bit) coefficients, read only; dst a sample tensor, dst_stride in bytes (device)"""
+    return check(lib().b200_vp9_itxfm_add_batch_device(device.handle, bit_depth, nops, vp(_dptr(ops)), vp(_dptr(coef)), vp(_dptr(dst)),
+                                                       dst_stride), "vp9_itxfm_add_batch_device")

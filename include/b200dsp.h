@@ -736,6 +736,45 @@ _Static_assert(sizeof(B200Vp9McOp) == 40, "B200Vp9McOp is 40 bytes");
 int  b200_vp9_mc_batch_device(B200Device *dev, int bit_depth, int nrefs, const B200Vp9McRef *refs, int64_t nops, const B200Vp9McOp *ops,
                               uint8_t *dst, ptrdiff_t dst_stride);
 
+/* VP9 inverse transforms and residual add: b200_vp9_dsp_init_itxfm() fills the 20 itxfm_add[5][4] pointers of a B200VP9DSPContext as
+ * vp9dsp_itxfm_init does (vp9dsp_template.c:1755-1778) and touches no other member (call it after b200_vp9_dsp_init, which leaves
+ * them NULL): [tx 0..2 = 4x4, 8x8, 16x16][type in TxfmType order: DCT_DCT idct / idct, DCT_ADST iadst / idct, ADST_DCT idct / iadst,
+ * ADST_ADST iadst / iadst] ("a / b" = the type of pass 1 / pass 2), [3][*] one function (32x32 idct / idct), [4][*] one function
+ * (lossless: the Walsh-Hadamard transform).  HOST pointers and the reference's signature: `block` holds sz * sz int16 coefficients at
+ * 8 bit and int32 ones at 10 / 12 bit (the int16_t * of the signature), the stride is in bytes.
+ *   passes    pass 1 applies type a to every column i of the block (block[i + k sz]), giving row i of tmp; pass 2 applies type b to
+ *             every column i of tmp, and its output j is added to dst row j, column i as clip(dst + ((int)(out + 2^(bits-1)) >> bits)),
+ *             bits 4 / 5 / 6 / 6 for 4 / 8 / 16 / 32; the Walsh-Hadamard transform takes pass 1's inputs >> 2 and adds out unshifted
+ *   storage   8 bit: tmp and out int16, arithmetic 32-bit; 10 / 12 bit: int32 and int64; every coefficient value is accepted
+ *   DC only   idct / idct at 4..16 and every 32x32 slot with eob == 1: only block[0] is read and cleared; any other eob (0 included)
+ *             runs the full transform, which clears all sz * sz coefficients.  Nothing else reads eob.
+ * 0; B200_EINVAL for c == NULL; B200_ENOSYS for depths other than 8, 10 and 12; B200_ENODEV. */
+int  b200_vp9_dsp_init_itxfm(B200VP9DSPContext *c, int bit_depth);
+
+/* One transform block of b200_vp9_itxfm_add_batch_device: itxfm_add[tx][type](dst + dst_off, dst_stride, coef + coef_off, eob). */
+typedef struct B200Vp9TxOp {
+    int64_t dst_off;    /* bytes, into dst */
+    int64_t coef_off;   /* coefficient elements (int16 at 8 bit, int32 at 10 / 12) into coef: the block's dense sz * sz coefficients */
+    uint8_t tx;         /* itxfm_add's first index: 0..3 = 4x4..32x32, 4 = lossless */
+    uint8_t type;       /* second index 0..3, TxfmType order (vp9.h) */
+    uint16_t eob;       /* as the decoder passes it (vp9recon.c:624, :643) */
+    uint8_t reserved[4];
+} B200Vp9TxOp;
+#ifdef __cplusplus
+static_assert(sizeof(B200Vp9TxOp) == 24, "B200Vp9TxOp is 24 bytes");
+#else
+_Static_assert(sizeof(B200Vp9TxOp) == 24, "B200Vp9TxOp is 24 bytes");
+#endif
+/* Batched VP9 residual reconstruction of one plane (inter_recon's loop over transform blocks, vp9recon.c:608-652, as one call):
+ * `ops`, `coef` and `dst` are DEVICE pointers; asynchronous on the device's stream.  Each op's block of dst becomes what the member
+ * above makes of it.  `coef` is read only: the decoder clears its coefficient buffer itself.  The caller guarantees that the ops of
+ * one call write disjoint blocks.  An op with tx > 4, type > 3, coef_off not a multiple of 16 or dst_off not a multiple of 4 samples
+ * writes nothing.  Offsets are 64-bit; more ops than one launch takes are split inside the entry.
+ * Returns 0, or B200_EINVAL (launching nothing) for NULL pointers, nops < 0, a depth other than 8, 10 or 12, ops not aligned to 8
+ * bytes, coef not aligned to 16 bytes, dst not aligned to 4 samples or dst_stride not a multiple of 4 samples; nops == 0 returns 0. */
+int  b200_vp9_itxfm_add_batch_device(B200Device *dev, int bit_depth, int64_t nops, const B200Vp9TxOp *ops, const void *coef, uint8_t *dst,
+                                     ptrdiff_t dst_stride);
+
 /* mpegvideo inverse quantisers: the members of MPVUnquantDSPContext (libavcodec/mpegvideo_unquantize.h:31-44) as
  * ff_mpv_unquantize_init() installs them (libavcodec/mpegvideo_unquantize.c:50-290), i.e. what runs in front of the IDCT in
  * mpv_reconstruct_mb's put_dct / add_dequant_dct (libavcodec/mpegvideo_dec.c).  The reference functions take the whole

@@ -229,6 +229,14 @@ class Vp9TxOp(C.Structure):
                 ("reserved", C.c_uint8 * 4)]
 
 
+VP9_LF_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_int, C.c_int, C.c_int)
+
+
+class Vp9Filter(C.Structure):
+    """B200Vp9Filter (include/b200dsp.h) = VP9Filter (libavcodec/vp9dec.h:79-83), 192 bytes"""
+    _fields_ = [("level", C.c_uint8 * 64), ("mask", C.c_uint8 * 4 * 8 * 2 * 2)]
+
+
 class ProresDSPContext(C.Structure):
     """libavcodec/proresdsp.h:28-35"""
     _fields_ = [("idct_permutation_type", C.c_int), ("idct_permutation", C.c_uint8 * 64),
@@ -353,6 +361,10 @@ PROTOTYPES = {
     "b200_vp9_mc_batch_device": (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_int64, vp, vp, C.c_ssize_t]),
     "b200_vp9_dsp_init_itxfm": (C.c_int, [vp, C.c_int]),
     "b200_vp9_itxfm_add_batch_device": (C.c_int, [vp, C.c_int, C.c_int64, vp, vp, vp, C.c_ssize_t]),
+    "b200_vp9_dsp_init_loopfilter": (C.c_int, [vp, C.c_int]),
+    "b200_vp9_loopfilter_frame_device": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_ssize_t, C.c_ssize_t, vp,
+                                                   C.c_int64, vp, vp]),
+    "b200_vp9_loopfilter_timeouts": (C.c_int, [vp, vp]),
     "b200_proresdsp_init": (C.c_int, [vp, C.c_int]),
     "b200_prores_idct_put_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, vp, vp, vp, C.c_int]),
     "b200_float_dsp_init": (C.c_int, [vp]),

@@ -1,11 +1,12 @@
 """Host-side mirror of libavcodec's VP9 DSP: the mc / smc tables of VP9DSPContext as ff_vp9dsp_init installs them
 (libavcodec/vp9dsp_template.c:2302-2361, :2540-2569) and the batched device entry b200_vp9_mc_batch_device; the itxfm_add members
-(vp9dsp_template.c:1755-1778) and b200_vp9_itxfm_add_batch_device."""
+(vp9dsp_template.c:1755-1778) and b200_vp9_itxfm_add_batch_device; the loop-filter members (vp9dsp_template.c:1947-1967) and the frame
+entry b200_vp9_loopfilter_frame_device (ff_vp9_loopfilter_sb over every superblock, vp9lpf.c:179-203)."""
 import ctypes as C
 
 import numpy as np
 
-from ._lib import lib, check, vp, VP9DSPContext, Vp9McRef, Vp9McOp, VP9_MC_FUNC, VP9_SCALED_MC_FUNC, Vp9TxOp, VP9_ITXFM_FUNC  # noqa: F401
+from ._lib import lib, check, vp, VP9DSPContext, Vp9McRef, Vp9McOp, VP9_MC_FUNC, VP9_SCALED_MC_FUNC, Vp9TxOp, VP9_ITXFM_FUNC, Vp9Filter, VP9_LF_FUNC  # noqa: F401
 
 SINGLE, COMPOUND = range(2)                                          # B200Vp9McOp.kind
 FILTER_8TAP_SMOOTH, FILTER_8TAP_REGULAR, FILTER_8TAP_SHARP, FILTER_BILINEAR = range(4)   # B200Vp9McOp.filter, libavcodec/vp9.h:64-71
@@ -17,6 +18,8 @@ DCT_DCT, DCT_ADST, ADST_DCT, ADST_ADST = range(4)                     # B200Vp9T
 TX_4X4, TX_8X8, TX_16X16, TX_32X32, TX_LOSSLESS = range(5)            # B200Vp9TxOp.tx
 TX_DTYPE = np.dtype([("dst_off", "<i8"), ("coef_off", "<i8"), ("tx", "u1"), ("type", "u1"), ("eob", "<u2"), ("reserved", "u1", 4)])
 assert TX_DTYPE.itemsize == C.sizeof(Vp9TxOp) == 24
+LF_DTYPE = np.dtype([("level", "u1", 64), ("mask", "u1", (2, 2, 8, 4))])    # B200Vp9Filter: [luma / chroma][column / row edges][row][width]
+assert LF_DTYPE.itemsize == C.sizeof(Vp9Filter) == 192
 
 
 def _dptr(x):
@@ -53,3 +56,27 @@ def vp9_itxfm_add_batch_device(device, bit_depth, nops, ops, coef, dst, dst_stri
     bit) coefficients, read only; dst a sample tensor, dst_stride in bytes (device)"""
     return check(lib().b200_vp9_itxfm_add_batch_device(device.handle, bit_depth, nops, vp(_dptr(ops)), vp(_dptr(coef)), vp(_dptr(dst)),
                                                        dst_stride), "vp9_itxfm_add_batch_device")
+
+
+def ff_vp9dsp_init_loopfilter(ctx, bit_depth=8):
+    """fills ctx.loop_filter_8, loop_filter_16 and loop_filter_mix2 (HOST pointers: call one through VP9_LF_FUNC(ctx.loop_filter_8[wd][dir]))
+    and touches no other member; returns ctx"""
+    check(lib().b200_vp9_dsp_init_loopfilter(C.byref(ctx), bit_depth), "ff_vp9dsp_init_loopfilter")
+    return ctx
+
+
+def vp9_loopfilter_frame_device(device, bit_depth, ss_h, ss_v, width, height, planes, ls_y, ls_uv, lflvl, lflvl_stride, lim_lut, mblim_lut):
+    """the whole frame's loop filter in place: planes = 3 sample tensors (or device addresses), line sizes in bytes; lflvl = LF_DTYPE records
+    (a uint8 tensor), lflvl_stride records per superblock row; lim_lut / mblim_lut = 64 host bytes each (the decoder's filter_lut)"""
+    arr = (C.c_void_p * 3)(*[_dptr(p) for p in planes])
+    lim = (C.c_uint8 * 64)(*[int(v) for v in lim_lut])
+    mblim = (C.c_uint8 * 64)(*[int(v) for v in mblim_lut])
+    return check(lib().b200_vp9_loopfilter_frame_device(device.handle, bit_depth, ss_h, ss_v, width, height, arr, ls_y, ls_uv, vp(_dptr(lflvl)),
+                                                        lflvl_stride, lim, mblim), "vp9_loopfilter_frame_device")
+
+
+def vp9_loopfilter_timeouts(device):
+    """waits of the frame entry that ran out on this device since the process started (after the device's stream is done)"""
+    n = C.c_int64()
+    check(lib().b200_vp9_loopfilter_timeouts(device.handle, C.byref(n)), "vp9_loopfilter_timeouts")
+    return n.value

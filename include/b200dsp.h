@@ -775,6 +775,64 @@ _Static_assert(sizeof(B200Vp9TxOp) == 24, "B200Vp9TxOp is 24 bytes");
 int  b200_vp9_itxfm_add_batch_device(B200Device *dev, int bit_depth, int64_t nops, const B200Vp9TxOp *ops, const void *coef, uint8_t *dst,
                                      ptrdiff_t dst_stride);
 
+/* VP9 loop filter: b200_vp9_dsp_init_loopfilter() fills loop_filter_8[3][2], loop_filter_16[2] and loop_filter_mix2[2][2][2] of a
+ * B200VP9DSPContext as vp9dsp_loopfilter_init does (vp9dsp_template.c:1947-1967): 16 distinct functions; it touches no other member.
+ * The last index is the direction: 0 filters the edge between two columns (samples across the edge are dst[-8..7], the lines run down
+ * the rows), 1 the edge between two rows (dst[-8 stride .. 7 stride], the lines run along the row).  HOST pointers and the reference's
+ * signature (dst, stride in bytes, E, I, H); samples uint8 at 8 bit and uint16 at 10 / 12 bit.
+ *   loop_filter_8[wd][dir]        8 lines of width 4 << wd (4, 8, 16) with E, I, H
+ *   loop_filter_16[dir]           16 lines of width 16 with the same E, I, H
+ *   loop_filter_mix2[a][b][dir]   8 lines of width 4 << a with E & 0xff, I & 0xff, H & 0xff, then the next 8 lines of width 4 << b with
+ *                                 E >> 8, I >> 8, H >> 8 (:1926-1933)
+ * Per line (:1780-1889): E, I and H are shifted left by depth - 8 and F = 1 << (depth - 8); nothing unless every neighbour difference
+ * p3..q3 is <= I and 2 |p0 - q0| + |p1 - q1| / 2 <= E; width 16 with p7..q7 all within F of p0 / q0 and p3..q3 within F: the 15-tap
+ * smoothing of p6..q6; width >= 8 with p3..q3 within F: the 7-tap smoothing of p2..q2; otherwise the 4-tap filter of p1..q1 (p0 / q0 only
+ * when |p1 - p0| or |q1 - q0| exceeds H).  A member reads only dst[-4..3] across the edge for widths 4 / 8 and dst[-8..7] for width 16,
+ * and writes only dst[-2..1], dst[-3..2] or dst[-7..6].
+ * 0; B200_EINVAL for c == NULL; B200_ENOSYS for depths other than 8, 10 and 12; B200_ENODEV. */
+int  b200_vp9_dsp_init_loopfilter(B200VP9DSPContext *c, int bit_depth);
+
+/* One superblock's loop-filter record: VP9Filter's layout (libavcodec/vp9dec.h:79-83).  level[row * 8 + col] is the filter level of the
+ * 8x8 luma block (row, col) of the superblock; mask[0 luma, 1 chroma][0 column edges, 1 row edges][8x8 luma row][0 16-wide, 1 8-wide,
+ * 2 4-wide, 3 inner 4-wide], bit k = 8x8 luma column k, as the decoder's mask_edges leaves them (vp9block.c:1142-1262). */
+typedef struct B200Vp9Filter {
+    uint8_t level[8 * 8];
+    uint8_t mask[2][2][8][4];
+} B200Vp9Filter;
+#ifdef __cplusplus
+static_assert(sizeof(B200Vp9Filter) == 192, "B200Vp9Filter is 192 bytes");
+#else
+_Static_assert(sizeof(B200Vp9Filter) == 192, "B200Vp9Filter is 192 bytes");
+#endif
+/* Loop-filters a whole VP9 frame in place, DEVICE pointers (planes[0..2], lflvl), asynchronous on the device's stream.  The result is
+ * ff_vp9_loopfilter_sb (vp9lpf.c:179-203) applied to every superblock in raster order, over Y, U and V: per plane all column edges of the
+ * superblock in filter_plane_cols' order, then all its row edges in filter_plane_rows' order (vp9lpf.c:27-177), with that dispatch's
+ * quirks, the chroma planes from mask[ss_h | ss_v] (4:4:4 uses the luma masks), the picture's left column and top row edges skipped,
+ * E = mblim_lut[L], I = lim_lut[L], H = L >> 4 for the level L (lim_lut / mblim_lut are the decoder's s->filter_lut, HOST arrays copied
+ * into the launch; levels index them modulo 64).
+ * width and height are the luma picture size: cols = (width + 7) >> 3, rows = (height + 7) >> 3 8x8 blocks, and the superblock grid is
+ * ((cols + 7) >> 3) x ((rows + 7) >> 3) records, lflvl[sb_row * lflvl_stride + sb_col].  The planes must cover the 8-aligned area: luma
+ * cols * 8 x rows * 8 samples, chroma (cols * 8 >> ss_h) x (rows * 8 >> ss_v) rounded up to a multiple of 8 (the decoder's 8-line chroma
+ * edges at an odd cols / rows reach that far).  Ignored, because mask_edges never sets them (vp9block.c:1436-1446, :1206-1225): mask
+ * bits of 8x8 columns >= cols and rows >= rows, and the chroma 16-wide bits at column bit 7 (with ss_h) and in row 7 (with ss_v) of the
+ * column / row masks, whose edges would reach into the next superblock.  No sample outside the area is read or written; a chroma
+ * 16-wide edge whose 16 samples would leave the area (4 samples from its left or top edge, or past its right or bottom edge; the
+ * decoder sets none) reads unspecified values for the missing ones.
+ * The work runs as a wavefront: superblock (r, c) of a plane starts once (r, c - 1) and (r - 1, c + 1) are done, the order the result
+ * depends on.  Offsets are 64-bit.
+ * lflvl needs no alignment beyond a byte.
+ * Returns 0, or B200_EINVAL (launching nothing) for NULL pointers, a depth other than 8, 10 or 12, ss_h / ss_v outside {0, 1}, width or
+ * height < 1, a stride shorter than a plane row or not a multiple of the sample size, a plane not aligned to a sample, or lflvl_stride
+ * below the superblock column count. */
+int  b200_vp9_loopfilter_frame_device(B200Device *dev, int bit_depth, int ss_h, int ss_v, int width, int height, uint8_t *const planes[3],
+                                      ptrdiff_t ls_y, ptrdiff_t ls_uv, const B200Vp9Filter *lflvl, int64_t lflvl_stride,
+                                      const uint8_t lim_lut[64], const uint8_t mblim_lut[64]);
+/* The frame entry's superblocks wait on the row above; every such wait is bounded by about one second, after which the superblock is
+ * filtered anyway (wrong samples rather than a hung GPU) and a per-device counter is incremented.  This waits for the device's stream
+ * and stores the number of waits that ran out on that device since the process started (0 unless something kept the row above from
+ * running for a second) in *count.  0; B200_EINVAL for count == NULL; B200_ENODEV; B200_EEXTERNAL. */
+int  b200_vp9_loopfilter_timeouts(B200Device *dev, int64_t *count);
+
 /* mpegvideo inverse quantisers: the members of MPVUnquantDSPContext (libavcodec/mpegvideo_unquantize.h:31-44) as
  * ff_mpv_unquantize_init() installs them (libavcodec/mpegvideo_unquantize.c:50-290), i.e. what runs in front of the IDCT in
  * mpv_reconstruct_mb's put_dct / add_dequant_dct (libavcodec/mpegvideo_dec.c).  The reference functions take the whole

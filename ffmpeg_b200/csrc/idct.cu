@@ -16,11 +16,8 @@
 
 namespace {
 
-constexpr int W1 = 22725, W2 = 21407, W3 = 19266, W4 = 16383, W5 = 12873, W6 = 8867, W7 = 4520;
-
-__device__ __forceinline__ int lo16(unsigned v) { return (int)(short)(v & 0xffff); }
-__device__ __forceinline__ int hi16(unsigned v) { return (int)v >> 16; }
-__device__ __forceinline__ unsigned pk16(int a, int b) { return ((unsigned)a & 0xffff) | ((unsigned)b << 16); }
+#include "simple_idct.cuh"
+#include "mpv_unquant.cuh"
 
 // 8x8 transpose of 16-bit elements held as 4 packed words per lane by groups of 8 lanes.
 __device__ __forceinline__ void transpose8x8(unsigned q[4], int lane)
@@ -48,66 +45,6 @@ __device__ __forceinline__ void transpose8x8(unsigned q[4], int lane)
     }
 }
 
-// simple_idct_template.c:114-206.  in/out: 8 coefficients of one row as 4 packed words.
-__device__ __forceinline__ void row_pass(unsigned q[4])
-{
-    const int r0 = lo16(q[0]), r1 = hi16(q[0]), r2 = lo16(q[1]), r3 = hi16(q[1]);
-    const int r4 = lo16(q[2]), r5 = hi16(q[2]), r6 = lo16(q[3]), r7 = hi16(q[3]);
-    const bool dc_only = ((q[0] >> 16) | q[1] | q[2] | q[3]) == 0;
-    unsigned a0 = (unsigned)W4 * (unsigned)r0 + (1u << 10), a1 = a0, a2 = a0, a3 = a0;
-    a0 += (unsigned)W2 * (unsigned)r2; a1 += (unsigned)W6 * (unsigned)r2;
-    a2 -= (unsigned)W6 * (unsigned)r2; a3 -= (unsigned)W2 * (unsigned)r2;
-    unsigned b0 = (unsigned)W1 * (unsigned)r1 + (unsigned)W3 * (unsigned)r3;
-    unsigned b1 = (unsigned)W3 * (unsigned)r1 - (unsigned)W7 * (unsigned)r3;
-    unsigned b2 = (unsigned)W5 * (unsigned)r1 - (unsigned)W1 * (unsigned)r3;
-    unsigned b3 = (unsigned)W7 * (unsigned)r1 - (unsigned)W5 * (unsigned)r3;
-    a0 += (unsigned)W4 * (unsigned)r4 + (unsigned)W6 * (unsigned)r6;
-    a1 -= (unsigned)W4 * (unsigned)r4 + (unsigned)W2 * (unsigned)r6;
-    a2 += (unsigned)W2 * (unsigned)r6 - (unsigned)W4 * (unsigned)r4;
-    a3 += (unsigned)W4 * (unsigned)r4 - (unsigned)W6 * (unsigned)r6;
-    b0 += (unsigned)W5 * (unsigned)r5 + (unsigned)W7 * (unsigned)r7;
-    b1 -= (unsigned)W1 * (unsigned)r5 + (unsigned)W5 * (unsigned)r7;
-    b2 += (unsigned)W7 * (unsigned)r5 + (unsigned)W3 * (unsigned)r7;
-    b3 += (unsigned)W3 * (unsigned)r5 - (unsigned)W1 * (unsigned)r7;
-    const int o0 = (int)(a0 + b0) >> 11, o7 = (int)(a0 - b0) >> 11;
-    const int o1 = (int)(a1 + b1) >> 11, o6 = (int)(a1 - b1) >> 11;
-    const int o2 = (int)(a2 + b2) >> 11, o5 = (int)(a2 - b2) >> 11;
-    const int o3 = (int)(a3 + b3) >> 11, o4 = (int)(a3 - b3) >> 11;
-    if (dc_only) {
-        const unsigned dc = ((unsigned)r0 << 3) & 0xffff;
-        q[0] = q[1] = q[2] = q[3] = dc | (dc << 16);
-    } else {
-        q[0] = pk16(o0, o1); q[1] = pk16(o2, o3); q[2] = pk16(o4, o5); q[3] = pk16(o6, o7);
-    }
-}
-
-// IDCT_COLS, simple_idct_template.c:209-257 (the zero tests there only skip additions of zero).
-__device__ __forceinline__ void col_pass(unsigned q[4])
-{
-    const int c0 = lo16(q[0]), c1 = hi16(q[0]), c2 = lo16(q[1]), c3 = hi16(q[1]);
-    const int c4 = lo16(q[2]), c5 = hi16(q[2]), c6 = lo16(q[3]), c7 = hi16(q[3]);
-    unsigned a0 = (unsigned)W4 * (unsigned)(c0 + ((1 << 19) / W4)), a1 = a0, a2 = a0, a3 = a0;
-    a0 += (unsigned)W2 * (unsigned)c2; a1 += (unsigned)W6 * (unsigned)c2;
-    a2 -= (unsigned)W6 * (unsigned)c2; a3 -= (unsigned)W2 * (unsigned)c2;
-    unsigned b0 = (unsigned)W1 * (unsigned)c1 + (unsigned)W3 * (unsigned)c3;
-    unsigned b1 = (unsigned)W3 * (unsigned)c1 - (unsigned)W7 * (unsigned)c3;
-    unsigned b2 = (unsigned)W5 * (unsigned)c1 - (unsigned)W1 * (unsigned)c3;
-    unsigned b3 = (unsigned)W7 * (unsigned)c1 - (unsigned)W5 * (unsigned)c3;
-    a0 += (unsigned)W4 * (unsigned)c4 + (unsigned)W6 * (unsigned)c6;
-    a1 -= (unsigned)W4 * (unsigned)c4 + (unsigned)W2 * (unsigned)c6;
-    a2 += (unsigned)W2 * (unsigned)c6 - (unsigned)W4 * (unsigned)c4;
-    a3 += (unsigned)W4 * (unsigned)c4 - (unsigned)W6 * (unsigned)c6;
-    b0 += (unsigned)W5 * (unsigned)c5 + (unsigned)W7 * (unsigned)c7;
-    b1 -= (unsigned)W1 * (unsigned)c5 + (unsigned)W5 * (unsigned)c7;
-    b2 += (unsigned)W7 * (unsigned)c5 + (unsigned)W3 * (unsigned)c7;
-    b3 += (unsigned)W3 * (unsigned)c5 - (unsigned)W1 * (unsigned)c7;
-    // results fit in 12 bits signed, so packing them as int16 loses nothing
-    q[0] = pk16((int)(a0 + b0) >> 20, (int)(a1 + b1) >> 20);
-    q[1] = pk16((int)(a2 + b2) >> 20, (int)(a3 + b3) >> 20);
-    q[2] = pk16((int)(a3 - b3) >> 20, (int)(a2 - b2) >> 20);
-    q[3] = pk16((int)(a1 - b1) >> 20, (int)(a0 - b0) >> 20);
-}
-
 __device__ __forceinline__ unsigned clip4(int a, int b, int c, int d)
 {
     return (unsigned)min(max(a, 0), 255) | ((unsigned)min(max(b, 0), 255) << 8) |
@@ -131,20 +68,25 @@ idct8x8_kernel(const int16_t *blocks, int16_t *blocks_out, long long nblocks,
     const long long warp = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     const long long blk = warp * 4 + (lane >> 3);
     const bool live = blk < nblocks;
-    unsigned q[4] = { 0, 0, 0, 0 };
+    uint4 v = make_uint4(0, 0, 0, 0);
     if (live) {
         const uint4 *src = reinterpret_cast<const uint4 *>(blocks) + blk * 8 + row;
-        const uint4 v = KIND == B200_IDCT ? *src : __ldg(src);   // in-place variant must not use the read-only path
-        q[0] = v.x; q[1] = v.y; q[2] = v.z; q[3] = v.w;
+        v = KIND == B200_IDCT ? *src : __ldg(src);   // in-place variant must not use the read-only path
     }
-    row_pass(q);
+    unsigned q[4];
+    row_pass<8>(v, q);
     transpose8x8(q, lane);        // lane now owns column `row`
-    col_pass(q);
+    {
+        int o[8];
+        col_pass<8>(sx_lo(q[0]), sx_hi(q[0]), sx_lo(q[1]), sx_hi(q[1]), sx_lo(q[2]), sx_hi(q[2]), sx_lo(q[3]), sx_hi(q[3]), o);
+        // results fit in 12 bits signed, so packing them as int16 loses nothing
+#pragma unroll
+        for (int k = 0; k < 4; k++) q[k] = __byte_perm((unsigned)o[2 * k], (unsigned)o[2 * k + 1], 0x5410);
+    }
     transpose8x8(q, lane);        // lane owns output row `row` again
     if (!live) return;
     if (KIND == B200_IDCT) {
-        uint4 v; v.x = q[0]; v.y = q[1]; v.z = q[2]; v.w = q[3];
-        reinterpret_cast<uint4 *>(blocks_out)[blk * 8 + row] = v;
+        reinterpret_cast<uint4 *>(blocks_out)[blk * 8 + row] = make_uint4(q[0], q[1], q[2], q[3]);
         return;
     }
     uint8_t *d; long long ls;
@@ -166,8 +108,8 @@ idct8x8_kernel(const int16_t *blocks, int16_t *blocks_out, long long nblocks,
         d = dest + __ldg(dest_off + blk);
     }
     d += row * ls;
-    int v0 = lo16(q[0]), v1 = hi16(q[0]), v2 = lo16(q[1]), v3 = hi16(q[1]);
-    int v4 = lo16(q[2]), v5 = hi16(q[2]), v6 = lo16(q[3]), v7 = hi16(q[3]);
+    int v0 = sx_lo(q[0]), v1 = sx_hi(q[0]), v2 = sx_lo(q[1]), v3 = sx_hi(q[1]);
+    int v4 = sx_lo(q[2]), v5 = sx_hi(q[2]), v6 = sx_lo(q[3]), v7 = sx_hi(q[3]);
     const bool al8 = ((reinterpret_cast<uintptr_t>(d)) & 7) == 0;
     if (KIND == B200_IDCT_ADD) {
         uint2 p;
@@ -200,92 +142,6 @@ idct8x8_kernel(const int16_t *blocks, int16_t *blocks_out, long long nblocks,
 //        chunks of whole rows (128-byte lines).  For `add` the tile is first filled from the destination the same way.
 // HBM traffic stays the algorithmic 128 B in + 64 B out (+ 64 B) per block.
 
-// sign-extend the low half in one PRMT: selector nibble 9 = "replicate the sign of byte 1".  __byte_perm() masks the
-// selector to 3 bits per nibble, so the sign-replicate mode needs the PTX instruction itself.
-__device__ __forceinline__ int sx_lo(unsigned v)
-{
-    int d;
-    asm("prmt.b32 %0, %1, %2, %3;" : "=r"(d) : "r"(v), "r"(0u), "r"(0x9910u));
-    return d;
-}
-__device__ __forceinline__ int sx_hi(unsigned v) { return (int)v >> 16; }
-// The 8-point butterfly shared by both passes (simple_idct_template.c:157-199 rows, :209-257 columns), all sums mod 2^32
-// like the reference's unsigned arithmetic.  Every output sum is ONE multiply-add chain that starts from the even part
-// (a_i + b_i accumulated in place) and its mirror output is 2*a_i - (a_i + b_i): 22 multiply-adds + 8 adds per
-// transform instead of 22 + 14, and the adds that remain are the only work left for the ALU pipe.
-//   e[0..7] = a0+b0, a1+b1, a2+b2, a3+b3, a3-b3, a2-b2, a1-b1, a0-b0   (before the final shift)
-// mad.lo through inline PTX so that the compiler cannot re-associate the chains back into separate sums
-__device__ __forceinline__ unsigned mad(unsigned k, unsigned x, unsigned acc)
-{
-    unsigned d;
-    asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(x), "r"(k), "r"(acc));
-    return d;
-}
-template <unsigned K1, unsigned K2, unsigned K3, unsigned K4, unsigned K5, unsigned K6, unsigned K7>
-__device__ __forceinline__ void odd_even_sums(int c0, int c1, int c2, int c3, int c4, int c5, int c6, int c7, unsigned rnd, unsigned *e)
-{
-    const unsigned u1 = (unsigned)c1, u2 = (unsigned)c2, u3 = (unsigned)c3, u5 = (unsigned)c5, u6 = (unsigned)c6, u7 = (unsigned)c7;
-    const unsigned p = mad(K4, (unsigned)(c0 + c4), rnd), q = mad(K4, (unsigned)(c0 - c4), rnd);
-    const unsigned a0 = mad(K2, u2, mad(K6, u6, p)), a3 = 2u * p - a0;
-    const unsigned a1 = mad(K6, u2, mad(0u - K2, u6, q)), a2 = 2u * q - a1;
-    e[0] = mad(K1, u1, mad(K3, u3, mad(K5, u5, mad(K7, u7, a0))));
-    e[1] = mad(K3, u1, mad(0u - K7, u3, mad(0u - K1, u5, mad(0u - K5, u7, a1))));
-    e[2] = mad(K5, u1, mad(0u - K1, u3, mad(K7, u5, mad(K3, u7, a2))));
-    e[3] = mad(K7, u1, mad(0u - K5, u3, mad(K3, u5, mad(0u - K1, u7, a3))));
-    e[7] = 2u * a0 - e[0]; e[6] = 2u * a1 - e[1]; e[5] = 2u * a2 - e[2]; e[4] = 2u * a3 - e[3];
-}
-__device__ __forceinline__ void col_sums(int c0, int c1, int c2, int c3, int c4, int c5, int c6, int c7, unsigned *e)
-{
-    odd_even_sums<W1, W2, W3, W4, W5, W6, W7>(c0, c1, c2, c3, c4, c5, c6, c7, (unsigned)W4 * (unsigned)((1 << 19) / W4), e);
-}
-
-// Row pass with every constant pre-multiplied by 32: only bits 11..26 of the reference's 32-bit row sums survive the
-// ">> 11, store as int16" step, and those are bits 16..31 of (32 * sum) mod 2^32 — so (int)sum32 >> 16 IS the
-// sign-extended int16 the reference stores (one shift instead of shift + wrap).
-// simple_idct_template.c:114-206 on packed input, 8 sign-extended int16 results
-__device__ __forceinline__ void row_pass_i(const uint4 &in, int *o)
-{
-    constexpr unsigned X1 = 32u * W1, X2 = 32u * W2, X3 = 32u * W3, X4 = 32u * W4, X5 = 32u * W5, X6 = 32u * W6, X7 = 32u * W7;
-    const int r0 = sx_lo(in.x), r1 = sx_hi(in.x), r2 = sx_lo(in.y), r3 = sx_hi(in.y);
-    const int r4 = sx_lo(in.z), r5 = sx_hi(in.z), r6 = sx_lo(in.w), r7 = sx_hi(in.w);
-    if (((in.x >> 16) | in.y | in.z | in.w) == 0) {
-        const int dc = (int)(short)(((unsigned)r0 << 3) & 0xffff);
-#pragma unroll
-        for (int i = 0; i < 8; i++) o[i] = dc;
-        return;
-    }
-    unsigned e[8];
-    odd_even_sums<X1, X2, X3, X4, X5, X6, X7>(r0, r1, r2, r3, r4, r5, r6, r7, 32u << 10, e);
-#pragma unroll
-    for (int i = 0; i < 8; i++) o[i] = (int)e[i] >> 16;
-}
-
-// same, results left packed as four (int16, int16) words: the high halves of the x32 sums are picked by PRMT
-__device__ __forceinline__ void row_pass_packed(const uint4 &in, unsigned *o)
-{
-    constexpr unsigned X1 = 32u * W1, X2 = 32u * W2, X3 = 32u * W3, X4 = 32u * W4, X5 = 32u * W5, X6 = 32u * W6, X7 = 32u * W7;
-    if (((in.x >> 16) | in.y | in.z | in.w) == 0) {
-        const unsigned dc = ((in.x & 0xffffu) << 3) & 0xffffu;
-        o[0] = o[1] = o[2] = o[3] = dc | (dc << 16);
-        return;
-    }
-    const int r0 = sx_lo(in.x), r1 = sx_hi(in.x), r2 = sx_lo(in.y), r3 = sx_hi(in.y);
-    const int r4 = sx_lo(in.z), r5 = sx_hi(in.z), r6 = sx_lo(in.w), r7 = sx_hi(in.w);
-    unsigned e[8];
-    odd_even_sums<X1, X2, X3, X4, X5, X6, X7>(r0, r1, r2, r3, r4, r5, r6, r7, 32u << 10, e);
-    o[0] = __byte_perm(e[0], e[1], 0x7632); o[1] = __byte_perm(e[2], e[3], 0x7632);
-    o[2] = __byte_perm(e[4], e[5], 0x7632); o[3] = __byte_perm(e[6], e[7], 0x7632);
-}
-
-// IDCT_COLS (simple_idct_template.c:209-257): eight inputs of one column -> eight results (already >> 20)
-__device__ __forceinline__ void col_pass_i(int c0, int c1, int c2, int c3, int c4, int c5, int c6, int c7, int *o)
-{
-    unsigned e[8];
-    col_sums(c0, c1, c2, c3, c4, c5, c6, c7, e);
-#pragma unroll
-    for (int i = 0; i < 8; i++) o[i] = (int)e[i] >> 20;
-}
-
 // 16-byte LDGSTS to a 32-bit shared-window address (convert the base pointer ONCE with smem_addr(): doing the
 // generic->shared conversion per copy costs three extra instructions each)
 __device__ __forceinline__ unsigned smem_addr(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
@@ -303,13 +159,13 @@ __device__ __forceinline__ void idct_block(const uint4 *rows, int key, const uin
 {
     int R[8][8];
 #pragma unroll
-    for (int j = 0; j < 8; j++) row_pass_i(rows[j ^ key], R[j]);
+    for (int j = 0; j < 8; j++) row_pass<8>(rows[j ^ key], R[j]);
     unsigned P[8][4];                                  // per output row: four s16x2 pairs (clamped for put/add)
 #pragma unroll
     for (int c = 0; c < 8; c += 2) {
         int oa[8], ob[8];
-        col_pass_i(R[0][c], R[1][c], R[2][c], R[3][c], R[4][c], R[5][c], R[6][c], R[7][c], oa);
-        col_pass_i(R[0][c + 1], R[1][c + 1], R[2][c + 1], R[3][c + 1], R[4][c + 1], R[5][c + 1], R[6][c + 1], R[7][c + 1], ob);
+        col_pass<8>(R[0][c], R[1][c], R[2][c], R[3][c], R[4][c], R[5][c], R[6][c], R[7][c], oa);
+        col_pass<8>(R[0][c + 1], R[1][c + 1], R[2][c + 1], R[3][c + 1], R[4][c + 1], R[5][c + 1], R[6][c + 1], R[7][c + 1], ob);
 #pragma unroll
         for (int k = 0; k < 8; k++) {
             if (KIND == B200_IDCT_ADD) {
@@ -405,46 +261,19 @@ idct_tpb_kernel(const int16_t *blocks, int16_t *blocks_out, long long nblocks, u
 // Luma tile rows 8..15 are stored with their 64-byte halves swapped so that blocks Y0/Y2 (and Y1/Y3) of one
 // macroblock, which sit 8 rows = 1024 B apart, do not share banks.
 // ---- inverse quantisation fused in front of the transform (put_dct / add_dequant_dct, libavcodec/mpegvideo_dec.c:907-922): the
-// same arithmetic as unquant.cu's kernel (libavcodec/mpegvideo_unquantize.c:50-276), applied by the thread that owns the block to the
-// eight rows it takes out of shared memory — the dequantised coefficients never exist in HBM (128 B read + 128 B written per block saved
-// against the two-kernel sequence).  V = -1: no dequantisation (the plain IDCT kernels).
-struct FusedUnquant {                     // passed by value (kernel parameter: every table index is a compile-time constant)
-    uint16_t intra[64], inter[64];
-    uint8_t scanpos[64];                  // scan index of each raster coefficient
-    uint8_t raster_end[64];
-    int y_dc, c_dc, q_type, aic, ac_pred;
+// arithmetic of mpv_unquant.cuh (libavcodec/mpegvideo_unquantize.c:50-276) that unquant.cu's kernel uses too, applied by the thread
+// that owns the block to the eight rows it takes out of shared memory — the dequantised coefficients never exist in HBM (128 B read +
+// 128 B written per block saved against the two-kernel sequence).  V = -1: no dequantisation (the plain IDCT kernels).
+struct FusedUnquant : UnquantDev {        // passed by value (kernel parameter: every table index is a compile-time constant)
     const uint8_t *qscale;                // per block
     const int8_t *last_index;             // per block
 };
-__constant__ uint8_t c_fused_nonlinear_qscale[32] = {              // ff_mpeg2_non_linear_qscale
-    0, 1, 2, 3, 4, 5, 6, 7, 8, 10, 12, 14, 16, 18, 20, 22, 24, 28, 32, 36, 40, 44, 48, 52, 56, 64, 72, 80, 88, 96, 104, 112,
-};
-template <int V> __device__ __forceinline__ int fused_dequant(int level, int q, int m)
-{
-    const unsigned a = (unsigned)(level < 0 ? -level : level);
-    int v;
-    if (V == B200_UNQUANT_MPEG1_INTRA)      { v = (int)(a * q * m) >> 3; v = (v - 1) | 1; }
-    else if (V == B200_UNQUANT_MPEG1_INTER) { v = (int)(((a << 1) + 1) * q * m) >> 4; v = (v - 1) | 1; }
-    else if (V == B200_UNQUANT_MPEG2_INTER) { v = (int)(((a << 1) + 1) * q * m) >> 5; }
-    else                                    { v = (int)(a * q * m) >> 4; }
-    return level < 0 ? -v : v;
-}
 // the eight rows of one block (row j in r[j], 8 int16 each) dequantised in place; n = block number inside its macroblock
 template <int V>
 __device__ __forceinline__ void fused_unquant_rows(uint4 (&r)[8], const FusedUnquant &P, int n, int qs, int last)
 {
-    constexpr bool H263 = V == B200_UNQUANT_H263_INTRA || V == B200_UNQUANT_H263_INTER;
-    constexpr bool INTRA = V == B200_UNQUANT_MPEG1_INTRA || V == B200_UNQUANT_MPEG2_INTRA ||
-                           V == B200_UNQUANT_MPEG2_INTRA_BITEXACT || V == B200_UNQUANT_H263_INTRA;
-    constexpr bool MISMATCH = V == B200_UNQUANT_MPEG2_INTRA_BITEXACT || V == B200_UNQUANT_MPEG2_INTER;
-    int q = qs, qadd = 0, ncoef = last, parity = 0;
-    if (H263) {
-        q = qs << 1;
-        qadd = (INTRA && P.aic) ? 0 : ((qs - 1) | 1);
-        ncoef = (INTRA && P.ac_pred) ? 63 : (last >= 0 ? (int)P.raster_end[last] : -1);
-    } else if (V >= B200_UNQUANT_MPEG2_INTRA) {
-        q = P.q_type ? (int)c_fused_nonlinear_qscale[qs & 31] : qs << 1;
-    }
+    const MpvBlock blk = mpv_block<V>(P, qs, last);
+    int parity = 0;
 #pragma unroll
     for (int row = 0; row < 8; row++) {
         unsigned w[4] = { r[row].x, r[row].y, r[row].z, r[row].w };
@@ -452,19 +281,8 @@ __device__ __forceinline__ void fused_unquant_rows(uint4 (&r)[8], const FusedUnq
         for (int k = 0; k < 8; k++) {
             const int j = 8 * row + k;
             int level = (k & 1) ? (int)w[k >> 1] >> 16 : (int)(short)(w[k >> 1] & 0xffffu);
-            if (INTRA && j == 0 && !(H263 && P.aic)) {
-                level = (int)(int16_t)(level * (n < 4 ? P.y_dc : P.c_dc));
-                if (MISMATCH) parity ^= level & 1;
-            }
-            const int pos = H263 ? j : (int)P.scanpos[j];
-            if (pos >= (INTRA ? 1 : 0) && pos <= ncoef && level != 0) {
-                int v;
-                if (H263) v = level < 0 ? level * q - qadd : level * q + qadd;
-                else      v = fused_dequant<V>(level, q, (int)(INTRA ? P.intra[j] : P.inter[j]));
-                if (MISMATCH) parity ^= v & 1;
-                level = (int)(int16_t)v;
-            }
-            if (MISMATCH && j == 63) level ^= (int)(1u ^ ((unsigned)parity & 1u));      // sum starts at -1: block[63] ^= sum & 1
+            mpv_coef<V>(P, blk, n, j, mpv_matrix<V>(P, j), mpv_scanpos<V>(P, j), level, parity);
+            if (MpvVariant<V>::MISMATCH && j == 63) level ^= (int)(1u ^ ((unsigned)parity & 1u));      // sum starts at -1: block[63] ^= sum & 1
             w[k >> 1] = (k & 1) ? (w[k >> 1] & 0xffffu) | ((unsigned)level << 16) : (w[k >> 1] & 0xffff0000u) | ((unsigned)level & 0xffffu);
         }
         r[row] = make_uint4(w[0], w[1], w[2], w[3]);
@@ -543,23 +361,23 @@ idct_mb420_kernel(const int16_t *blocks, Mb420Geom g, int segs_per_cta, const __
             for (int j = 0; j < 8; j++) rr[j] = rows[j ^ key];
             fused_unquant_rows<V < 0 ? 0 : V>(rr, UQ, k, (int)__ldg(UQ.qscale + bi), last);
 #pragma unroll
-            for (int j = 0; j < 8; j++) row_pass_packed(rr[j], R2[j]);
+            for (int j = 0; j < 8; j++) row_pass<8>(rr[j], R2[j]);
         } else {
 #pragma unroll
-            for (int j = 0; j < 8; j++) row_pass_packed(rows[j ^ key], R2[j]);
+            for (int j = 0; j < 8; j++) row_pass<8>(rows[j ^ key], R2[j]);
         }
         if (!skip) {
 #pragma unroll
         for (int half = 0; half < 2; half++) {             // four columns (one 32-bit tile word per row) at a time
             unsigned e0[8], e1[8], e2[8], e3[8];             // column sums before the >> 20 (rows in the order 0,1,2,3,4,5,6,7)
             const int c0 = 2 * half, c1 = 2 * half + 1;
-            col_sums(sx_lo(R2[0][c0]), sx_lo(R2[1][c0]), sx_lo(R2[2][c0]), sx_lo(R2[3][c0]),
+            col_sums<8>(sx_lo(R2[0][c0]), sx_lo(R2[1][c0]), sx_lo(R2[2][c0]), sx_lo(R2[3][c0]),
                      sx_lo(R2[4][c0]), sx_lo(R2[5][c0]), sx_lo(R2[6][c0]), sx_lo(R2[7][c0]), e0);
-            col_sums(sx_hi(R2[0][c0]), sx_hi(R2[1][c0]), sx_hi(R2[2][c0]), sx_hi(R2[3][c0]),
+            col_sums<8>(sx_hi(R2[0][c0]), sx_hi(R2[1][c0]), sx_hi(R2[2][c0]), sx_hi(R2[3][c0]),
                      sx_hi(R2[4][c0]), sx_hi(R2[5][c0]), sx_hi(R2[6][c0]), sx_hi(R2[7][c0]), e1);
-            col_sums(sx_lo(R2[0][c1]), sx_lo(R2[1][c1]), sx_lo(R2[2][c1]), sx_lo(R2[3][c1]),
+            col_sums<8>(sx_lo(R2[0][c1]), sx_lo(R2[1][c1]), sx_lo(R2[2][c1]), sx_lo(R2[3][c1]),
                      sx_lo(R2[4][c1]), sx_lo(R2[5][c1]), sx_lo(R2[6][c1]), sx_lo(R2[7][c1]), e2);
-            col_sums(sx_hi(R2[0][c1]), sx_hi(R2[1][c1]), sx_hi(R2[2][c1]), sx_hi(R2[3][c1]),
+            col_sums<8>(sx_hi(R2[0][c1]), sx_hi(R2[1][c1]), sx_hi(R2[2][c1]), sx_hi(R2[3][c1]),
                      sx_hi(R2[4][c1]), sx_hi(R2[5][c1]), sx_hi(R2[6][c1]), sx_hi(R2[7][c1]), e3);
 #pragma unroll
             for (int r = 0; r < 8; r++) {
@@ -725,17 +543,7 @@ B200_API int b200_mpv_unquant_idct_mb420_device(B200Device *dev, int variant, co
     if (((uintptr_t)blocks) & 15) return B200_EINVAL;
     if (nframes == 0) return 0;
     FusedUnquant U;
-    memcpy(U.intra, p->intra_matrix, sizeof(U.intra));
-    memcpy(U.inter, p->inter_matrix, sizeof(U.inter));
-    memcpy(U.raster_end, p->raster_end, sizeof(U.raster_end));
-    bool seen[64] = { false };
-    for (int i = 0; i < 64; i++) {
-        const int j = p->permutated[i];
-        if (j > 63 || seen[j]) { b200_set_error("b200_mpv_unquant_idct: permutated[] is not a permutation of 0..63"); return B200_EINVAL; }
-        seen[j] = true;
-        U.scanpos[j] = (uint8_t)i;
-    }
-    U.y_dc = p->y_dc_scale; U.c_dc = p->c_dc_scale; U.q_type = p->q_scale_type; U.aic = p->h263_aic; U.ac_pred = p->ac_pred;
+    if (!mpv_unquant_params(p, &U)) { b200_set_error("b200_mpv_unquant_idct: permutated[] is not a permutation of 0..63"); return B200_EINVAL; }
     U.qscale = qscale; U.last_index = last_index;
     B200_CUDA_OK(cudaSetDevice(dev->ordinal));
     Mb420Geom g{};

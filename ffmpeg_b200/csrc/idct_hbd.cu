@@ -7,6 +7,9 @@
 //   :209-327  IDCT_COLS, idctSparseCol{,Put,Add}; :329-368 ff_simple_idct_{put,add,}_int16_{10,12}bit
 // which ff_idctdsp_init installs for bits_per_raw_sample 9, 10 (the 10-bit set) and 12 (idctdsp.c:248-266).  Sums mod 2^32.
 //
+// The constants of each depth, the row pass and the column sums come from simple_idct.cuh, which the 8-bit kernels (idct.cu) use
+// too; this file holds the kernels (how a block is loaded, stored and clipped) and the entry points.
+//
 // First version, correctness before speed: one thread per 8x8 block, the block held in registers (eight 16-byte loads), row
 // pass and column pass fully unrolled.  HBM-bound by bytes (128 B in + 128 B out per block); the 8-bit kernel's staging through
 // shared memory (idct.cu) is the model for the tuned version.
@@ -16,60 +19,8 @@
 namespace {
 
 // [device-code idct_hbd] (tests/cuda_emu runs this block on the CPU against the checker; comment markers only)
-template <int DEPTH> struct K;
-template <> struct K<10> { static constexpr unsigned W1 = 22725, W2 = 21407, W3 = 19265, W4 = 16384, W5 = 12873, W6 = 8867, W7 = 4520;
-                           static constexpr int ROW = 12, COL = 19, DC = 2; };
-template <> struct K<12> { static constexpr unsigned W1 = 45451, W2 = 42813, W3 = 38531, W4 = 32767, W5 = 25746, W6 = 17734, W7 = 9041;
-                           static constexpr int ROW = 16, COL = 17, DC = -1; };
-// the EXTRA_SHIFT instantiation proresdsp.c makes of the 10-bit constants (simple_idct_template.c:73-76: ROW_SHIFT 13, COL_SHIFT 18,
-// DC_SHIFT 1) with the two extra bits its row pass is called with (proresdsp.c:61-62) folded in: ROW 13 + 2, DC 1 - 2
-template <> struct K<110> { static constexpr unsigned W1 = 22725, W2 = 21407, W3 = 19265, W4 = 16384, W5 = 12873, W6 = 8867, W7 = 4520;
-                            static constexpr int ROW = 15, COL = 18, DC = -1; };
-
-template <int DEPTH> __device__ __forceinline__ void row_pass(int *r)     // r[0..7]: one row, values are int16 in int registers
-{
-    using C = K<DEPTH>;
-    if (!(r[1] | r[2] | r[3] | r[4] | r[5] | r[6] | r[7])) {
-        const int t = C::DC >= 0 ? r[0] * (1 << (C::DC >= 0 ? C::DC : 0)) : (r[0] + (1 << (C::DC < 0 ? -C::DC - 1 : 0))) >> (C::DC < 0 ? -C::DC : 0);
-        const int dc = (int)(int16_t)(uint16_t)(t & 0xffff);
-#pragma unroll
-        for (int i = 0; i < 8; i++) r[i] = dc;
-        return;
-    }
-    unsigned a0 = C::W4 * (unsigned)r[0] + (1u << (C::ROW - 1)), a1 = a0, a2 = a0, a3 = a0;
-    a0 += C::W2 * (unsigned)r[2]; a1 += C::W6 * (unsigned)r[2]; a2 -= C::W6 * (unsigned)r[2]; a3 -= C::W2 * (unsigned)r[2];
-    unsigned b0 = C::W1 * (unsigned)r[1] + C::W3 * (unsigned)r[3];
-    unsigned b1 = C::W3 * (unsigned)r[1] - C::W7 * (unsigned)r[3];
-    unsigned b2 = C::W5 * (unsigned)r[1] - C::W1 * (unsigned)r[3];
-    unsigned b3 = C::W7 * (unsigned)r[1] - C::W5 * (unsigned)r[3];
-    a0 += C::W4 * (unsigned)r[4] + C::W6 * (unsigned)r[6];
-    a1 -= C::W4 * (unsigned)r[4] + C::W2 * (unsigned)r[6];
-    a2 += C::W2 * (unsigned)r[6] - C::W4 * (unsigned)r[4];
-    a3 += C::W4 * (unsigned)r[4] - C::W6 * (unsigned)r[6];
-    b0 += C::W5 * (unsigned)r[5] + C::W7 * (unsigned)r[7];
-    b1 -= C::W1 * (unsigned)r[5] + C::W5 * (unsigned)r[7];
-    b2 += C::W7 * (unsigned)r[5] + C::W3 * (unsigned)r[7];
-    b3 += C::W3 * (unsigned)r[5] - C::W1 * (unsigned)r[7];
-    r[0] = (int)(int16_t)((int)(a0 + b0) >> C::ROW); r[7] = (int)(int16_t)((int)(a0 - b0) >> C::ROW);
-    r[1] = (int)(int16_t)((int)(a1 + b1) >> C::ROW); r[6] = (int)(int16_t)((int)(a1 - b1) >> C::ROW);
-    r[2] = (int)(int16_t)((int)(a2 + b2) >> C::ROW); r[5] = (int)(int16_t)((int)(a2 - b2) >> C::ROW);
-    r[3] = (int)(int16_t)((int)(a3 + b3) >> C::ROW); r[4] = (int)(int16_t)((int)(a3 - b3) >> C::ROW);
-}
-
-template <int DEPTH> __device__ __forceinline__ void col_pass(const int *c, int *o)   // c[0..7]: one column, top to bottom
-{
-    using C = K<DEPTH>;
-    unsigned a0 = C::W4 * (unsigned)(c[0] + (int)((1u << (C::COL - 1)) / C::W4)), a1 = a0, a2 = a0, a3 = a0;
-    a0 += C::W2 * (unsigned)c[2]; a1 += C::W6 * (unsigned)c[2]; a2 -= C::W6 * (unsigned)c[2]; a3 -= C::W2 * (unsigned)c[2];
-    unsigned b0 = C::W1 * (unsigned)c[1], b1 = C::W3 * (unsigned)c[1], b2 = C::W5 * (unsigned)c[1], b3 = C::W7 * (unsigned)c[1];
-    b0 += C::W3 * (unsigned)c[3]; b1 -= C::W7 * (unsigned)c[3]; b2 -= C::W1 * (unsigned)c[3]; b3 -= C::W5 * (unsigned)c[3];
-    a0 += C::W4 * (unsigned)c[4]; a1 -= C::W4 * (unsigned)c[4]; a2 -= C::W4 * (unsigned)c[4]; a3 += C::W4 * (unsigned)c[4];
-    b0 += C::W5 * (unsigned)c[5]; b1 -= C::W1 * (unsigned)c[5]; b2 += C::W7 * (unsigned)c[5]; b3 += C::W3 * (unsigned)c[5];
-    a0 += C::W6 * (unsigned)c[6]; a1 -= C::W2 * (unsigned)c[6]; a2 += C::W2 * (unsigned)c[6]; a3 -= C::W6 * (unsigned)c[6];
-    b0 += C::W7 * (unsigned)c[7]; b1 -= C::W5 * (unsigned)c[7]; b2 += C::W3 * (unsigned)c[7]; b3 -= C::W1 * (unsigned)c[7];
-    o[0] = (int)(a0 + b0) >> C::COL; o[1] = (int)(a1 + b1) >> C::COL; o[2] = (int)(a2 + b2) >> C::COL; o[3] = (int)(a3 + b3) >> C::COL;
-    o[4] = (int)(a3 - b3) >> C::COL; o[5] = (int)(a2 - b2) >> C::COL; o[6] = (int)(a1 - b1) >> C::COL; o[7] = (int)(a0 - b0) >> C::COL;
-}
+// named from include/, a search path of every build of this block: tests/cuda_emu compiles a copy of it from another directory
+#include "../ffmpeg_b200/csrc/simple_idct.cuh"
 
 // KIND 0: in place on the coefficients, 1: put, 2: add.  dest = uint16 pixels; offsets and line sizes in BYTES (even).
 template <int DEPTH, int KIND>
@@ -78,17 +29,13 @@ idct_hbd_kernel(int16_t *blocks, long long n, uint8_t *dest, const int64_t *dest
 {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    int v[64];
+    uint4 rows[8];                                        // every row requested before the first row pass branches
     const uint4 *src = reinterpret_cast<const uint4 *>(blocks + 64 * i);
 #pragma unroll
-    for (int r = 0; r < 8; r++) {
-        const uint4 q = src[r];
-        const unsigned w[4] = { q.x, q.y, q.z, q.w };
+    for (int r = 0; r < 8; r++) rows[r] = src[r];
+    int v[64];
 #pragma unroll
-        for (int k = 0; k < 4; k++) { v[8 * r + 2 * k] = (int)(int16_t)(w[k] & 0xffffu); v[8 * r + 2 * k + 1] = (int)(int16_t)(w[k] >> 16); }
-    }
-#pragma unroll
-    for (int r = 0; r < 8; r++) row_pass<DEPTH>(v + 8 * r);
+    for (int r = 0; r < 8; r++) row_pass<DEPTH>(rows[r], v + 8 * r);
     constexpr int MAXV = (1 << DEPTH) - 1;
     uint16_t *d = nullptr;
     long long ls = 0;
@@ -98,10 +45,8 @@ idct_hbd_kernel(int16_t *blocks, long long n, uint8_t *dest, const int64_t *dest
     }
 #pragma unroll
     for (int c = 0; c < 8; c++) {
-        int col[8], o[8];
-#pragma unroll
-        for (int j = 0; j < 8; j++) col[j] = v[8 * j + c];
-        col_pass<DEPTH>(col, o);
+        int o[8];
+        col_pass<DEPTH>(v[c], v[8 + c], v[16 + c], v[24 + c], v[32 + c], v[40 + c], v[48 + c], v[56 + c], o);
 #pragma unroll
         for (int j = 0; j < 8; j++) v[8 * j + c] = o[j];
     }
@@ -159,21 +104,21 @@ prores_idct_put_kernel(const int16_t *blocks, long long n, const int16_t *qmat, 
 {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    unsigned w[32];                                       // the dequantised block as (int16, int16) pairs, all loaded before the row passes
+#pragma unroll
+    for (int k = 0; k < 32; k++)
+        w[k] = ((unsigned)(blocks[64 * i + 2 * k] * qmat[2 * k]) & 0xffffu) | ((unsigned)(blocks[64 * i + 2 * k + 1] * qmat[2 * k + 1]) << 16);
     int v[64];
 #pragma unroll
-    for (int k = 0; k < 64; k++) v[k] = (int)(int16_t)((int)blocks[64 * i + k] * (int)qmat[k]);
-#pragma unroll
-    for (int r = 0; r < 8; r++) row_pass<VARIANT>(v + 8 * r);
+    for (int r = 0; r < 8; r++) row_pass<VARIANT>(make_uint4(w[4 * r], w[4 * r + 1], w[4 * r + 2], w[4 * r + 3]), v + 8 * r);
     constexpr int BITS = VARIANT == 110 ? 10 : 12, LO = 4, HI = (1 << BITS) - 4 - 1;
     uint16_t *d = reinterpret_cast<uint16_t *>(dest + dest_off[i]);
     const long long ls = (line_size ? line_size[i] : uniform_ls) >> 1;
 #pragma unroll
     for (int c = 0; c < 8; c++) {
-        int col[8], o[8];
+        int o[8];
         v[c] = (int)(int16_t)(v[c] + 8192);
-#pragma unroll
-        for (int j = 0; j < 8; j++) col[j] = v[8 * j + c];
-        col_pass<VARIANT>(col, o);
+        col_pass<VARIANT>(v[c], v[8 + c], v[16 + c], v[24 + c], v[32 + c], v[40 + c], v[48 + c], v[56 + c], o);
 #pragma unroll
         for (int j = 0; j < 8; j++) d[j * ls + c] = (uint16_t)min(max((int)(int16_t)o[j], LO), HI);
     }

@@ -19,48 +19,22 @@ namespace {
 constexpr int WARPS = 4;
 
 // [device-code unquant] (tests/cuda_emu runs this block on the CPU against the checker; comment markers only)
-struct UnquantDev {                       // passed by value as a __grid_constant__ parameter: the per-lane table look-ups index the constant bank
-                                          // directly (a plain by-value parameter is copied to local memory per thread when indexed at run time:
-                                          // the round-2 launch list showed this kernel at 1.1 G blocks/s because of it)
-    uint16_t intra[64], inter[64];
-    uint8_t scanpos[64];                  // scan index of each raster coefficient (inverse of ScanTable.permutated)
-    uint8_t raster_end[64];
-    int y_dc, c_dc, q_type, aic, ac_pred;
-};
-
-__constant__ uint8_t c_nonlinear_qscale[32] = {                    // ff_mpeg2_non_linear_qscale (ISO/IEC 13818-2 table 7-6)
-    0, 1, 2, 3, 4, 5, 6, 7, 8, 10, 12, 14, 16, 18, 20, 22, 24, 28, 32, 36, 40, 44, 48, 52, 56, 64, 72, 80, 88, 96, 104, 112,
-};
-
-template <int V> __device__ __forceinline__ int dequant(int level, int q, int m)
-{
-    const unsigned a = (unsigned)(level < 0 ? -level : level);
-    int v;
-    if (V == B200_UNQUANT_MPEG1_INTRA)      { v = (int)(a * q * m) >> 3; v = (v - 1) | 1; }
-    else if (V == B200_UNQUANT_MPEG1_INTER) { v = (int)(((a << 1) + 1) * q * m) >> 4; v = (v - 1) | 1; }
-    else if (V == B200_UNQUANT_MPEG2_INTER) { v = (int)(((a << 1) + 1) * q * m) >> 5; }
-    else                                    { v = (int)(a * q * m) >> 4; }
-    return level < 0 ? -v : v;
-}
+// named from include/, a search path of every build of this block: tests/cuda_emu compiles a copy of it from another directory
+#include "../ffmpeg_b200/csrc/mpv_unquant.cuh"
 
 template <int V>
 __global__ void __launch_bounds__(32 * WARPS)
 mpv_unquant_kernel(const __grid_constant__ UnquantDev P, int16_t *blocks, long long nblocks, const uint8_t *blk_n, const uint8_t *qscale,
                    const int8_t *last_index)
 {
-    constexpr bool H263 = V == B200_UNQUANT_H263_INTRA || V == B200_UNQUANT_H263_INTER;
-    constexpr bool INTRA = V == B200_UNQUANT_MPEG1_INTRA || V == B200_UNQUANT_MPEG2_INTRA ||
-                           V == B200_UNQUANT_MPEG2_INTRA_BITEXACT || V == B200_UNQUANT_H263_INTRA;
-    constexpr bool MISMATCH = V == B200_UNQUANT_MPEG2_INTRA_BITEXACT || V == B200_UNQUANT_MPEG2_INTER;
     const int lane = threadIdx.x & 31;
     // a lane always owns coefficients 2 * lane and 2 * lane + 1: its matrix entries and scan positions are fetched once (32 different
     // constant-bank addresses per warp instruction are served one after the other), then the warp walks over blocks
     int mat[2], spos[2];
 #pragma unroll
     for (int k = 0; k < 2; k++) {
-        const int j = 2 * lane + k;
-        mat[k] = (int)(INTRA ? P.intra[j] : P.inter[j]);
-        spos[k] = H263 ? j : (int)P.scanpos[j];
+        mat[k] = mpv_matrix<V>(P, 2 * lane + k);
+        spos[k] = mpv_scanpos<V>(P, 2 * lane + k);
     }
     const long long nwarps = (long long)gridDim.x * WARPS;
     for (long long b = (long long)blockIdx.x * WARPS + (threadIdx.x >> 5); b < nblocks; b += nwarps) {      // whole warps leave together
@@ -70,33 +44,10 @@ mpv_unquant_kernel(const __grid_constant__ UnquantDev P, int16_t *blocks, long l
         const unsigned word = *wp;
         int lv[2] = { (int)(int16_t)(word & 0xffffu), (int)(int16_t)(word >> 16) };
         int parity = 0;
-        int q = qs, qadd = 0, ncoef = last;
-        if (H263) {
-            q = qs << 1;
-            qadd = (INTRA && P.aic) ? 0 : ((qs - 1) | 1);
-            ncoef = (INTRA && P.ac_pred) ? 63 : (last >= 0 ? (int)P.raster_end[last] : -1);
-        } else if (V >= B200_UNQUANT_MPEG2_INTRA) {
-            q = P.q_type ? (int)c_nonlinear_qscale[qs & 31] : qs << 1;
-        }
+        const MpvBlock blk = mpv_block<V>(P, qs, last);
 #pragma unroll
-        for (int k = 0; k < 2; k++) {
-            const int j = 2 * lane + k;
-            int level = lv[k];
-            if (INTRA && j == 0 && !(H263 && P.aic)) {
-                level = (int)(int16_t)(level * (n < 4 ? P.y_dc : P.c_dc));
-                if (MISMATCH) parity ^= level & 1;
-            }
-            const int pos = spos[k];
-            if (pos >= (INTRA ? 1 : 0) && pos <= ncoef && level != 0) {
-                int v;
-                if (H263) v = level < 0 ? level * q - qadd : level * q + qadd;
-                else      v = dequant<V>(level, q, mat[k]);
-                if (MISMATCH) parity ^= v & 1;
-                level = (int)(int16_t)v;
-            }
-            lv[k] = level;
-        }
-        if (MISMATCH) {
+        for (int k = 0; k < 2; k++) mpv_coef<V>(P, blk, n, 2 * lane + k, mat[k], spos[k], lv[k], parity);
+        if (MpvVariant<V>::MISMATCH) {
             const unsigned par = __reduce_xor_sync(0xffffffffu, (unsigned)parity);
             if (lane == 31) lv[1] ^= (int)(1u ^ (par & 1u));                    // sum starts at -1: block[63] ^= sum & 1
         }
@@ -116,17 +67,7 @@ B200_API int b200_mpv_unquantize_batch_device(B200Device *dev, int variant, cons
     if (nblocks == 0) return 0;
     if (!blocks || !qscale || !last_index || (reinterpret_cast<uintptr_t>(blocks) & 3)) return B200_EINVAL;
     UnquantDev P;
-    memcpy(P.intra, p->intra_matrix, sizeof(P.intra));
-    memcpy(P.inter, p->inter_matrix, sizeof(P.inter));
-    memcpy(P.raster_end, p->raster_end, sizeof(P.raster_end));
-    bool seen[64] = { false };
-    for (int i = 0; i < 64; i++) {
-        const int j = p->permutated[i];
-        if (j > 63 || seen[j]) { b200_set_error("b200_mpv_unquantize: permutated[] is not a permutation of 0..63"); return B200_EINVAL; }
-        seen[j] = true;
-        P.scanpos[j] = (uint8_t)i;
-    }
-    P.y_dc = p->y_dc_scale; P.c_dc = p->c_dc_scale; P.q_type = p->q_scale_type; P.aic = p->h263_aic; P.ac_pred = p->ac_pred;
+    if (!mpv_unquant_params(p, &P)) { b200_set_error("b200_mpv_unquantize: permutated[] is not a permutation of 0..63"); return B200_EINVAL; }
     B200_CUDA_OK(cudaSetDevice(dev->ordinal));
     long long grid = (nblocks + WARPS - 1) / WARPS;
     const long long cap = (long long)(dev->sm_count > 0 ? dev->sm_count : 132) * 16 * 8;      // persistent warps: each walks nblocks / (grid * WARPS) blocks

@@ -140,9 +140,7 @@ int emu_unquant(int variant, const B200MpvUnquant *p, int16_t *blocks, long long
                 const int8_t *last_index)
 {
     unq::UnquantDev P;
-    for (int i = 0; i < 64; i++) { P.intra[i] = p->intra_matrix[i]; P.inter[i] = p->inter_matrix[i]; P.raster_end[i] = p->raster_end[i]; }
-    for (int i = 0; i < 64; i++) P.scanpos[p->permutated[i]] = (uint8_t)i;
-    P.y_dc = p->y_dc_scale; P.c_dc = p->c_dc_scale; P.q_type = p->q_scale_type; P.aic = p->h263_aic; P.ac_pred = p->ac_pred;
+    if (!unq::mpv_unquant_params(p, &P)) return -1;
     const dim3 g(ceil_div(nblocks, unq::WARPS)), t(32 * unq::WARPS);
     switch (variant) {
 #define CASE(V) case V: emu_launch_warps(g, t, [&] { unq::mpv_unquant_kernel<V>(P, blocks, nblocks, blk_n, qscale, last_index); }); return 0;

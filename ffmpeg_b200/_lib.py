@@ -237,6 +237,15 @@ class Vp9Filter(C.Structure):
     _fields_ = [("level", C.c_uint8 * 64), ("mask", C.c_uint8 * 4 * 8 * 2 * 2)]
 
 
+VP9_INTRA_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_void_p)
+
+
+class Vp9IntraOp(C.Structure):
+    """B200Vp9IntraOp (include/b200dsp.h), 32 bytes"""
+    _fields_ = [("coef_off", C.c_int64), ("x", C.c_int32), ("y", C.c_int32), ("eob", C.c_uint16), ("plane", C.c_uint8), ("tx", C.c_uint8),
+                ("mode", C.c_uint8), ("flags", C.c_uint8), ("reserved", C.c_uint8 * 10)]
+
+
 class ProresDSPContext(C.Structure):
     """libavcodec/proresdsp.h:28-35"""
     _fields_ = [("idct_permutation_type", C.c_int), ("idct_permutation", C.c_uint8 * 64),
@@ -365,6 +374,10 @@ PROTOTYPES = {
     "b200_vp9_loopfilter_frame_device": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_ssize_t, C.c_ssize_t, vp,
                                                    C.c_int64, vp, vp]),
     "b200_vp9_loopfilter_timeouts": (C.c_int, [vp, vp]),
+    "b200_vp9_dsp_init_intrapred": (C.c_int, [vp, C.c_int]),
+    "b200_vp9_intra_recon_frame_device": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_ssize_t, C.c_ssize_t, C.c_int64,
+                                                    vp, vp]),
+    "b200_vp9_intra_timeouts": (C.c_int, [vp, vp]),
     "b200_proresdsp_init": (C.c_int, [vp, C.c_int]),
     "b200_prores_idct_put_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, vp, vp, vp, C.c_int]),
     "b200_float_dsp_init": (C.c_int, [vp]),

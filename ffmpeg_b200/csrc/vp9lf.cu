@@ -27,6 +27,7 @@
 // each wait that runs out is counted in a per-device word that b200_vp9_loopfilter_timeouts() reads back.
 // The column pass gives each thread one line and the row pass one column; each walks its edges in the driver's order.
 #include "common.h"
+#include "wait_timeouts.h"
 #include <cstring>
 
 namespace {
@@ -292,25 +293,6 @@ __global__ void __launch_bounds__(kThreads) vp9_lf_kernel(const __grid_constant_
 
 bool depth_ok(int d) { return d == 8 || d == 10 || d == 12; }
 
-// the wait-timeout counter of each device ordinal: one int of device memory for the life of the process, made at the first frame call
-constexpr int kMaxOrdinals = 64;
-std::mutex g_timeouts_mu;
-int *g_timeouts[kMaxOrdinals];
-
-int *timeouts_word(int ordinal, bool create)
-{
-    if (ordinal < 0 || ordinal >= kMaxOrdinals) return nullptr;
-    std::lock_guard<std::mutex> lock(g_timeouts_mu);
-    if (!g_timeouts[ordinal] && create) {
-        int *w = nullptr;
-        const int zero = 0;
-        if (cudaMalloc(&w, sizeof(int)) != cudaSuccess) return nullptr;
-        if (cudaMemcpy(w, &zero, sizeof(int), cudaMemcpyHostToDevice) != cudaSuccess) { cudaFree(w); return nullptr; }
-        g_timeouts[ordinal] = w;
-    }
-    return g_timeouts[ordinal];
-}
-
 void die(const char *what)
 {
     fprintf(stderr, "libb200dsp: vp9 loop filter failed: %s (%s)\n", what, b200_last_error());
@@ -438,7 +420,7 @@ B200_API int b200_vp9_loopfilter_frame_device(B200Device *dev, int bit_depth, in
     if (!dev) return B200_ENODEV;
     B200_CUDA_OK(cudaSetDevice(dev->ordinal));
     B200_LOCK_DEVICE(dev);
-    int *timeouts = timeouts_word(dev->ordinal, true);
+    int *timeouts = b200_wait_timeouts_word(dev->ordinal, B200_WAIT_VP9_LOOPFILTER, true);
     if (!timeouts) { b200_set_error("vp9 loop filter frame: no timeout counter for device %d", dev->ordinal); return B200_ENOMEM; }
     const size_t sync_bytes = sizeof(int) * (1 + 3 * (size_t)sb_rows);
     int *sync = (int *)b200_scratch(dev, sync_bytes);
@@ -478,7 +460,7 @@ B200_API int b200_vp9_loopfilter_timeouts(B200Device *dev, int64_t *count)
     B200_CUDA_OK(cudaSetDevice(dev->ordinal));
     B200_CUDA_OK(cudaStreamSynchronize(dev->stream));
     int v = 0;
-    int *w = timeouts_word(dev->ordinal, false);
+    int *w = b200_wait_timeouts_word(dev->ordinal, B200_WAIT_VP9_LOOPFILTER, false);
     if (w) B200_CUDA_OK(cudaMemcpy(&v, w, sizeof(int), cudaMemcpyDeviceToHost));
     *count = v;
     return 0;

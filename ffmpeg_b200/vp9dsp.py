@@ -1,12 +1,14 @@
 """Host-side mirror of libavcodec's VP9 DSP: the mc / smc tables of VP9DSPContext as ff_vp9dsp_init installs them
 (libavcodec/vp9dsp_template.c:2302-2361, :2540-2569) and the batched device entry b200_vp9_mc_batch_device; the itxfm_add members
 (vp9dsp_template.c:1755-1778) and b200_vp9_itxfm_add_batch_device; the loop-filter members (vp9dsp_template.c:1947-1967) and the frame
-entry b200_vp9_loopfilter_frame_device (ff_vp9_loopfilter_sb over every superblock, vp9lpf.c:179-203)."""
+entry b200_vp9_loopfilter_frame_device (ff_vp9_loopfilter_sb over every superblock, vp9lpf.c:179-203); the intra_pred members
+(vp9dsp_template.c:1120-1152) and the frame entry b200_vp9_intra_recon_frame_device (intra_recon over every intra transform block,
+vp9recon.c:219-287)."""
 import ctypes as C
 
 import numpy as np
 
-from ._lib import lib, check, vp, VP9DSPContext, Vp9McRef, Vp9McOp, VP9_MC_FUNC, VP9_SCALED_MC_FUNC, Vp9TxOp, VP9_ITXFM_FUNC, Vp9Filter, VP9_LF_FUNC  # noqa: F401
+from ._lib import lib, check, vp, VP9DSPContext, Vp9McRef, Vp9McOp, VP9_MC_FUNC, VP9_SCALED_MC_FUNC, Vp9TxOp, VP9_ITXFM_FUNC, Vp9Filter, VP9_LF_FUNC, Vp9IntraOp, VP9_INTRA_FUNC  # noqa: F401
 
 SINGLE, COMPOUND = range(2)                                          # B200Vp9McOp.kind
 FILTER_8TAP_SMOOTH, FILTER_8TAP_REGULAR, FILTER_8TAP_SHARP, FILTER_BILINEAR = range(4)   # B200Vp9McOp.filter, libavcodec/vp9.h:64-71
@@ -20,6 +22,12 @@ TX_DTYPE = np.dtype([("dst_off", "<i8"), ("coef_off", "<i8"), ("tx", "u1"), ("ty
 assert TX_DTYPE.itemsize == C.sizeof(Vp9TxOp) == 24
 LF_DTYPE = np.dtype([("level", "u1", 64), ("mask", "u1", (2, 2, 8, 4))])    # B200Vp9Filter: [luma / chroma][column / row edges][row][width]
 assert LF_DTYPE.itemsize == C.sizeof(Vp9Filter) == 192
+(VERT_PRED, HOR_PRED, DC_PRED, DIAG_DOWN_LEFT_PRED, DIAG_DOWN_RIGHT_PRED, VERT_RIGHT_PRED, HOR_DOWN_PRED, VERT_LEFT_PRED, HOR_UP_PRED,
+ TM_VP8_PRED, LEFT_DC_PRED, TOP_DC_PRED, DC_128_PRED, DC_127_PRED, DC_129_PRED) = range(15)    # IntraPredMode, libavcodec/vp9.h:45-61
+INTRA_HAVE_LEFT, INTRA_HAVE_RIGHT, INTRA_LOSSLESS = 1, 2, 4            # B200Vp9IntraOp.flags
+INTRA_DTYPE = np.dtype([("coef_off", "<i8"), ("x", "<i4"), ("y", "<i4"), ("eob", "<u2"), ("plane", "u1"), ("tx", "u1"), ("mode", "u1"),
+                        ("flags", "u1"), ("reserved", "u1", 10)])
+assert INTRA_DTYPE.itemsize == C.sizeof(Vp9IntraOp) == 32
 
 
 def _dptr(x):
@@ -79,4 +87,27 @@ def vp9_loopfilter_timeouts(device):
     """waits of the frame entry that ran out on this device since the process started (after the device's stream is done)"""
     n = C.c_int64()
     check(lib().b200_vp9_loopfilter_timeouts(device.handle, C.byref(n)), "vp9_loopfilter_timeouts")
+    return n.value
+
+
+def ff_vp9dsp_init_intrapred(ctx, bit_depth=8):
+    """fills ctx.intra_pred (HOST pointers: call one through VP9_INTRA_FUNC(ctx.intra_pred[tx][mode])) and touches no other member;
+    returns ctx"""
+    check(lib().b200_vp9_dsp_init_intrapred(C.byref(ctx), bit_depth), "ff_vp9dsp_init_intrapred")
+    return ctx
+
+
+def vp9_intra_recon_frame_device(device, bit_depth, ss_h, ss_v, width, height, planes, ls_y, ls_uv, nops, ops, coef):
+    """every intra transform block of a frame in decode order, in place: planes = 3 sample tensors (or device addresses), line sizes in
+    bytes; ops = INTRA_DTYPE records (a uint8 tensor of nops * 32 bytes); coef = int16 (8 bit) / int32 (10 / 12 bit) coefficients, read
+    only (device)"""
+    arr = (C.c_void_p * 3)(*[_dptr(p) for p in planes])
+    return check(lib().b200_vp9_intra_recon_frame_device(device.handle, bit_depth, ss_h, ss_v, width, height, arr, ls_y, ls_uv, nops,
+                                                         vp(_dptr(ops)), vp(_dptr(coef))), "vp9_intra_recon_frame_device")
+
+
+def vp9_intra_timeouts(device):
+    """waits of the intra frame entry that ran out on this device since the process started (after the device's stream is done)"""
+    n = C.c_int64()
+    check(lib().b200_vp9_intra_timeouts(device.handle, C.byref(n)), "vp9_intra_timeouts")
     return n.value

@@ -833,6 +833,63 @@ int  b200_vp9_loopfilter_frame_device(B200Device *dev, int bit_depth, int ss_h, 
  * running for a second) in *count.  0; B200_EINVAL for count == NULL; B200_ENODEV; B200_EEXTERNAL. */
 int  b200_vp9_loopfilter_timeouts(B200Device *dev, int64_t *count);
 
+/* VP9 intra prediction: b200_vp9_dsp_init_intrapred() fills the 60 intra_pred[4][15] pointers of a B200VP9DSPContext as
+ * ff_vp9dsp_intrapred_init does (vp9dsp_template.c:1120-1152): [tx 0..3 = 4x4 .. 32x32][mode in IntraPredMode order, vp9.h:45-61];
+ * at 12 bit every mode but TM_VP8 and DC_127 / 128 / 129 is the 10-bit function, as in the reference.  It touches no other member.
+ * HOST pointers and the reference's signature (dst, stride in bytes, left, top); samples uint8 at 8 bit and uint16 at 10 / 12 bit.
+ * `left` is the column bottom-to-top (left[size - 1] is the sample beside row 0) except for HOR_UP, which takes it top-to-bottom.
+ * A member reads exactly the samples its reference function reads: top[-1] for TM, DIAG_DOWN_RIGHT, VERT_RIGHT and HOR_DOWN
+ * (HOR_DOWN reads top[-1 .. size - 2]); top[0 .. 7] for the 4x4 DIAG_DOWN_LEFT and top[0 .. 6] for the 4x4 VERT_LEFT; left[1 .. size - 1]
+ * for VERT_RIGHT; the DC_127 / 128 / 129 functions read nothing.  It writes only the size x size block.
+ * 0; B200_EINVAL for c == NULL; B200_ENOSYS for depths other than 8, 10 and 12; B200_ENODEV. */
+int  b200_vp9_dsp_init_intrapred(B200VP9DSPContext *c, int bit_depth);
+
+/* One transform block of intra_recon (vp9recon.c:219-287) for b200_vp9_intra_recon_frame_device.  The flags are the call site's:
+ *   B200_VP9_INTRA_HAVE_LEFT   col > td->tile_col_start || x > 0 (vp9recon.c:42)
+ *   B200_VP9_INTRA_HAVE_RIGHT  x < w - 1 in 4x4 units of the block, w = w4 for luma and w4 >> ss_h for chroma (:43, :259)
+ *   B200_VP9_INTRA_LOSSLESS    s->s.h.lossless: the residual goes through itxfm_add[4] (tx must be 0) */
+enum { B200_VP9_INTRA_HAVE_LEFT = 1, B200_VP9_INTRA_HAVE_RIGHT = 2, B200_VP9_INTRA_LOSSLESS = 4 };
+typedef struct B200Vp9IntraOp {
+    int64_t coef_off;   /* element offset of td->block + 16 * n * bytesperpixel (or of td->uvblock[p] + ...) in coef: a multiple of 16 */
+    int32_t x, y;       /* top-left sample of the transform block in its plane, multiples of 4 */
+    uint16_t eob;       /* as intra_recon reads it: 0 when b->skip */
+    uint8_t plane;      /* 0, 1, 2 */
+    uint8_t tx;         /* b->tx or b->uvtx, 0..3: the intra_pred size index */
+    uint8_t mode;       /* b->mode[...] or b->uvmode, 0..9, before mode_conv */
+    uint8_t flags;      /* B200_VP9_INTRA_* */
+    uint8_t reserved[10];
+} B200Vp9IntraOp;
+#ifdef __cplusplus
+static_assert(sizeof(B200Vp9IntraOp) == 32, "B200Vp9IntraOp is 32 bytes");
+#else
+_Static_assert(sizeof(B200Vp9IntraOp) == 32, "B200Vp9IntraOp is 32 bytes");
+#endif
+/* Intra reconstruction of a whole VP9 frame in one call, DEVICE pointers (planes[0..2], ops, coef), asynchronous on the device's
+ * stream.  `ops` lists every intra transform block of the frame, all three planes, in decode order: the order intra_recon visits them,
+ * block after block (each block's luma, then U, then V).  The result is intra_recon's check_intra_mode, intra_pred[tx][mode] and, when
+ * eob is non-zero, itxfm_add[4 * lossless + tx][txtp] (txtp = ff_vp9_intra_txfm_type[mode] for luma, DCT_DCT for chroma) applied to
+ * every op in that order, on planes that already hold the frame's inter reconstruction.  The entry derives from each op: have_top =
+ * y > 0; the top row's n_px_have = (cols * 8 >> ss_h) - x and the left column's (rows * 8 >> ss_v) - y (vp9recon.c:99, :188).
+ * `coef` holds int16 coefficients at 8 bit and int32 ones at 10 / 12 bit and is read only (clearing stays with the decoder).
+ * width and height are the luma picture size; cols = (width + 7) >> 3, rows = (height + 7) >> 3.  The planes must cover the 8-aligned
+ * area: luma cols * 8 x rows * 8 samples, chroma (cols * 8 >> ss_h) x (rows * 8 >> ss_v).  Only samples inside it are read or written:
+ * the part of a block that lies outside is not stored (the decoder's emulated-edge buffers drop it too, vp9block.c:1368-1430), and
+ * nothing reads it.  The top row of a superblock row is read from the plane: run the loop filter after this call, so that the plane
+ * row above still holds the decoder's intra_pred_data (vp9.c:1387-1398).
+ * The ops of one call write disjoint blocks, and an op reads only samples of ops listed before it, of inter blocks or of earlier calls
+ * (decode order guarantees both).  An op waits for the earlier ops that write the samples it reads; an op with plane > 2, tx > 3,
+ * mode > 9, a negative or unaligned x, y or coef_off, or LOSSLESS with tx != 0, and an op outside the plane, writes nothing.
+ * Returns 0, or B200_EINVAL (launching nothing) for NULL planes, a depth other than 8, 10 or 12, ss_h / ss_v outside {0, 1}, width or
+ * height outside 1..65536, nops outside 0..2^30, a stride shorter than a plane row or not a multiple of the sample size, a plane not
+ * aligned to a sample, or (nops > 0) ops NULL or not aligned to 8 bytes, coef NULL or not aligned to 16 bytes; nops == 0 returns 0. */
+int  b200_vp9_intra_recon_frame_device(B200Device *dev, int bit_depth, int ss_h, int ss_v, int width, int height, uint8_t *const planes[3],
+                                       ptrdiff_t ls_y, ptrdiff_t ls_uv, int64_t nops, const B200Vp9IntraOp *ops, const void *coef);
+/* The frame entry's ops wait on earlier ops; every such wait is bounded by about one second, after which the op runs anyway (wrong
+ * samples rather than a hung GPU) and a per-device counter is incremented.  This waits for the device's stream and stores the number of
+ * the intra entry's waits that ran out on that device since the process started in *count (the loop filter's are counted apart, by
+ * b200_vp9_loopfilter_timeouts).  0; B200_EINVAL for count == NULL; B200_ENODEV; B200_EEXTERNAL. */
+int  b200_vp9_intra_timeouts(B200Device *dev, int64_t *count);
+
 /* mpegvideo inverse quantisers: the members of MPVUnquantDSPContext (libavcodec/mpegvideo_unquantize.h:31-44) as
  * ff_mpv_unquantize_init() installs them (libavcodec/mpegvideo_unquantize.c:50-290), i.e. what runs in front of the IDCT in
  * mpv_reconstruct_mb's put_dct / add_dequant_dct (libavcodec/mpegvideo_dec.c).  The reference functions take the whole

@@ -400,17 +400,25 @@ sws_vscale_rgb24_fast_kernel(SwsFrameArgs a, SwsDevTables t, SwsColorConst c, in
 // whose chroma windows coincide.  With 2x vertical chroma up-sampling the bicubic window of output lines 2k+1 and 2k+2 starts at the same
 // chroma line (vChrFilterPos equal, only the coefficients differ; the host checks this for the whole bank), so the four chroma lines are
 // interleaved once (PRMT) and both lines are evaluated from the same registers.
-// One thread = 16 px of a band of up to PairShape<KIND>::band consecutive pairs of one frame, walked top to bottom:
-//  - the raw chroma tap lines stay in registers as a sliding window: when the next pair's window starts one line lower (2x up-sampling)
+// One thread walks a band of up to PairShape<KIND>::band consecutive pairs of one frame, top to bottom:
+//  - the chroma tap lines stay in registers as a sliding window: when the next pair's window starts one line lower (2x up-sampling)
 //    only the line it gains is loaded (one line per plane per pair instead of four); any other step reloads the window;
 //  - the next pair's luma rows, gained chroma line and coefficients are loaded before the current pair is computed, and the positions
 //    two pairs ahead, so that no load waits for another load issued in the same step.
-// Threads do not share data (no shared memory, no shuffles).  Grid: x over 16-px groups, y over bands, z over frames.
-// Band length and CTAs per SM as measured on the H100 (DESIGN.md §5).  24-bit rows: bands of 16 pairs at 6 CTAs per SM (80 registers).
-// 32-bit rows: one pair per thread at 5 CTAs per SM (96 registers): with their 64-byte stores, bands of 4 or 16 pairs were slower than
-// one pair, whatever the occupancy; with one pair the steps ahead reload the same pair's rows (L1 hits) and the window never slides.
+// What a thread writes depends on the row width:
+//  - 24-bit rows: one 16-byte chunk of each line (pair_chunks).  Adjacent lanes write adjacent chunks in the same instruction, so one
+//    warp store covers 512 contiguous bytes and fills whole 32-byte sectors when dst and ds are 32-byte aligned (16-byte alignment
+//    stays correct, only with a half sector at each end of a warp's span).  A chunk is not a whole number of pixels, so three lanes
+//    read the same 16-px group's luma and chroma (served by L1 as a broadcast) and each computes the 8 pixels under its chunk.
+//  - 32-bit rows: 16 px, four 128-bit stores per line at a 64-byte lane stride.
+// Threads do not share data (no shared memory, no shuffles).  Grid: x over chunks (24-bit) or 16-px groups (32-bit), y over bands, z
+// over frames.  Band length and CTAs per SM as measured on the H100 (DESIGN.md §5).  24-bit rows: bands of 32 pairs at 8 CTAs per SM
+// (64 registers) from planar chroma, 7 (72 registers) from nv12 / nv21: each source ran about 7 % slower at the other's count.
+// 32-bit rows: one pair per thread at 5 CTAs per SM (96 registers): with their 64-byte stores, bands of 4 or 16 pairs
+// were slower than one pair, whatever the occupancy; with one pair the steps ahead reload the same pair's rows (L1 hits) and the
+// window never slides.
 constexpr int PAIR_THREADS = 128;
-template <int KIND> struct PairShape { static constexpr int band = KIND <= SWS_OUT_BGR24 ? 16 : 1, ctas = KIND <= SWS_OUT_BGR24 ? 6 : 5; };
+template <int KIND, int NV = 0> struct PairShape { static constexpr int band = KIND <= SWS_OUT_BGR24 ? 32 : 1, ctas = KIND <= SWS_OUT_BGR24 ? (NV ? 7 : 8) : 5; };
 __device__ __forceinline__ void interleave2(const uint2 &r0, const uint2 &r1, unsigned *w)
 {
     w[0] = __byte_perm(r0.x, r1.x, 0x5140); w[1] = __byte_perm(r0.x, r1.x, 0x7362);
@@ -444,11 +452,105 @@ __device__ __forceinline__ void pair_interleave(const uint4 &r0, const uint4 &r1
     }
 }
 
-// pairs [0, npairs) of output lines (a.y0 + 2p, a.y0 + 2p + 1), a.y0 odd
+// x, y or z for r = 0, 1 or 2: two SELs, the same instructions in every lane
+__device__ __forceinline__ unsigned sel3(unsigned x, unsigned y, unsigned z, int r) { return r == 0 ? x : r == 1 ? y : z; }
+// 24-bit rows, one thread = one 16-byte chunk: chroma samples 2r .. 2r+3 of one tap line of the chunk's group (r = chunk % 3), U in .x and
+// V in .y.  The lanes of a warp have all three phases, so the selection is by lane-dependent PRMT selectors and SELs, not by branches.
+template <int NV>
+__device__ __forceinline__ uint2 chunk_chroma_line(const uint8_t *ub, const uint8_t *vb, int us, int vs, int l, int r, unsigned sel)
+{
+    if (NV) {                                                           // 16 interleaved bytes: samples 2r .. 2r+3 are words r, r + 1
+        const uint4 q = __ldg(reinterpret_cast<const uint4 *>(ub + l * us));
+        const unsigned w0 = sel3(q.x, q.y, q.z, r), w1 = sel3(q.y, q.z, q.w, r);
+        return NV == 1 ? make_uint2(__byte_perm(w0, w1, 0x6420), __byte_perm(w0, w1, 0x7531))
+                       : make_uint2(__byte_perm(w0, w1, 0x7531), __byte_perm(w0, w1, 0x6420));
+    }
+    const uint2 u = __ldg(reinterpret_cast<const uint2 *>(ub + l * us)), v = __ldg(reinterpret_cast<const uint2 *>(vb + l * vs));
+    return make_uint2(__byte_perm(u.x, u.y, sel), __byte_perm(v.x, v.y, sel));
+}
+// words r, r + 1 of a 16-px luma row: the chunk's pixels 4r .. 4r+7
+__device__ __forceinline__ uint2 chunk_luma(const uint4 &q, int r) { return make_uint2(sel3(q.x, q.y, q.z, r), sel3(q.y, q.z, q.w, r)); }
+
+// 24-bit rows.  Chunk r of a 16-px group (bytes 16r .. 16r+15 of its 48) starts r bytes into pixel 5r and ends in pixel 5r+5.  The thread
+// computes the 8 pixels 4r .. 4r+7 (chroma samples 2r .. 2r+3, 24 bytes from byte 12r of the group): the chunk is their words r .. r+3.
 template <int KIND, int NV>
-__global__ void __launch_bounds__(PAIR_THREADS, PairShape<KIND>::ctas)
+__device__ __forceinline__ void pair_chunks(const SwsFrameArgs &a, const SwsDevTables &t, const SwsColorConst &c, int ngroups, int npairs)
+{
+    constexpr int BAND = PairShape<KIND>::band;
+    const int xc = blockIdx.x * blockDim.x + threadIdx.x;
+    if (xc >= 3 * ngroups) return;
+    const int xg = xc / 3, r = xc - 3 * xg;
+    const unsigned csel = 0x3210u + 0x2222u * r;                        // bytes 2r .. 2r+3 of a chroma uint2
+    const int dA0 = a.y0 + 2 * blockIdx.y * BAND, np = min(BAND, npairs - (int)blockIdx.y * BAND);
+    const long long f = blockIdx.z;
+    const int ys = (int)a.ys, us = (int)a.us, vs = (int)a.vs, chmax = a.chrSrcH - 1, lmax = a.srcH - 1;
+    const uint8_t *yb = a.y + f * a.yfs + xg * 16;
+    const uint8_t *ub = a.u + f * a.ufs + xg * (NV ? 16 : 8), *vb = NV ? nullptr : a.v + f * a.vfs + xg * 8;
+    uint8_t *d = a.dst + f * a.dfs + (long long)dA0 * a.ds + xc * 16;                    // line 2i of the band
+    auto line = [&](int l) { return chunk_chroma_line<NV>(ub, vb, us, vs, min(max(l, 0), chmax), r, csel); };
+    auto luma = [&](int dy) { return chunk_luma(__ldg(reinterpret_cast<const uint4 *>(yb + min(max(__ldg(t.vLumPos + dy), 0), lmax) * ys)), r); };
+    auto first_chr = [&](int p) { return max(-3, __ldg(t.vChrPos + dA0 + 2 * p)); };          // == vChrPos[dA + 1]
+
+    // pair 0: the whole window; pair 1: its positions
+    int fc = first_chr(0);
+    uint2 W0 = line(fc), W1 = line(fc + 1), W2 = line(fc + 2), W3 = line(fc + 3);
+    uint2 YA = luma(dA0), YB = luma(dA0 + 1);
+    int2 kA = __ldg(reinterpret_cast<const int2 *>(t.vChr2 + 2 * dA0)), kB = __ldg(reinterpret_cast<const int2 *>(t.vChr2 + 2 * dA0 + 2));
+    const int p1 = min(1, np - 1);
+    int fcN = first_chr(p1);
+    int lyNA = min(max(__ldg(t.vLumPos + dA0 + 2 * p1), 0), lmax) * ys, lyNB = min(max(__ldg(t.vLumPos + dA0 + 2 * p1 + 1), 0), lmax) * ys;
+    for (int i = 0; i < np; i++) {
+        // pair i + 1 (the last pair repeats itself): the line its window gains, its luma rows and coefficients; pair i + 2: positions
+        const int in = min(i + 1, np - 1), i2 = min(i + 2, np - 1), dN = dA0 + 2 * in, d2 = dA0 + 2 * i2;
+        const bool slide = fcN == fc + 1;
+        const uint2 G = slide ? line(fcN + 3) : W3;
+        const uint2 NA = chunk_luma(__ldg(reinterpret_cast<const uint4 *>(yb + lyNA)), r), NB = chunk_luma(__ldg(reinterpret_cast<const uint4 *>(yb + lyNB)), r);
+        const int2 kNA = __ldg(reinterpret_cast<const int2 *>(t.vChr2 + 2 * dN)), kNB = __ldg(reinterpret_cast<const int2 *>(t.vChr2 + 2 * dN + 2));
+        const int fc2 = first_chr(i2);
+        const int ly2A = min(max(__ldg(t.vLumPos + d2), 0), lmax) * ys, ly2B = min(max(__ldg(t.vLumPos + d2 + 1), 0), lmax) * ys;
+
+        unsigned IU[2][2], IV[2][2];                                        // [tap pair][word]: two chroma samples x two lines each
+        interleave2(make_uint2(W0.x, W2.x), make_uint2(W1.x, W3.x), &IU[0][0]);   // IU[0] = taps 0 / 1, IU[1] = taps 2 / 3
+        interleave2(make_uint2(W0.y, W2.y), make_uint2(W1.y, W3.y), &IV[0][0]);
+#pragma unroll
+        for (int L = 0; L < 2; L++) {
+            const int kx = L ? kB.x : kA.x, ky = L ? kB.y : kA.y;
+            int aU[4], aV[4];
+#pragma unroll
+            for (int w = 0; w < 2; w++) {
+                aU[2 * w]     = dp2a_lo_su(ky, IU[1][w], dp2a_lo_su(kx, IU[0][w], 1 << 11));
+                aU[2 * w + 1] = dp2a_hi_su(ky, IU[1][w], dp2a_hi_su(kx, IU[0][w], 1 << 11));
+                aV[2 * w]     = dp2a_lo_su(ky, IV[1][w], dp2a_lo_su(kx, IV[0][w], 1 << 11));
+                aV[2 * w + 1] = dp2a_hi_su(ky, IV[1][w], dp2a_hi_su(kx, IV[0][w], 1 << 11));
+            }
+            const uint2 q = L ? YB : YA;
+            const unsigned yw[2] = { q.x, q.y };
+            unsigned m[12], o[6];
+#pragma unroll
+            for (int j = 0; j < 4; j++) {
+                const ChromaBase cb = chroma_base(c, aU[j] >> 12, aV[j] >> 12);
+                pair_out<KIND>(c.cy, cb, byte_of(yw[j >> 1], 2 * (j & 1)), byte_of(yw[j >> 1], 2 * (j & 1) + 1), m + 3 * j);
+            }
+#pragma unroll
+            for (int k = 0; k < 6; k++) o[k] = __byte_perm(m[2 * k], m[2 * k + 1], 0x6420);
+            *reinterpret_cast<uint4 *>(L ? d + a.ds : d) = make_uint4(sel3(o[0], o[1], o[2], r), sel3(o[1], o[2], o[3], r),
+                                                                     sel3(o[2], o[3], o[4], r), sel3(o[3], o[4], o[5], r));
+        }
+
+        if (slide) { W0 = W1; W1 = W2; W2 = W3; W3 = G; }
+        else if (fcN != fc) { W0 = line(fcN); W1 = line(fcN + 1); W2 = line(fcN + 2); W3 = line(fcN + 3); }
+        d += 2 * a.ds;
+        YA = NA; YB = NB; kA = kNA; kB = kNB;
+        fc = fcN; fcN = fc2; lyNA = ly2A; lyNB = ly2B;
+    }
+}
+
+// pairs [0, npairs) of output lines (a.y0 + 2p, a.y0 + 2p + 1), a.y0 odd; ngroups 16-px groups per line (24-bit rows: 3 * ngroups threads)
+template <int KIND, int NV>
+__global__ void __launch_bounds__(PAIR_THREADS, PairShape<KIND, NV>::ctas)
 sws_vscale_rgb24_pair_kernel(SwsFrameArgs a, SwsDevTables t, SwsColorConst c, int ngroups, int npairs)
 {
+    if (KIND <= SWS_OUT_BGR24) { pair_chunks<KIND, NV>(a, t, c, ngroups, npairs); return; }
     constexpr int PW = OutWords<KIND>::per_pair, BAND = PairShape<KIND>::band;
     const int xg = blockIdx.x * blockDim.x + threadIdx.x;
     if (xg >= ngroups) return;
@@ -1673,7 +1775,8 @@ static void launch_vscale_pair(int kind, int ngroups, int npairs, int nf, cudaSt
                                const SwsColorConst &col)
 {
     const dim3 block(PAIR_THREADS);
-    auto grid = [&](int band) { return dim3(b200_ceil_div(ngroups, PAIR_THREADS), b200_ceil_div(npairs, band), nf); };
+    // x: one thread per 16-byte chunk of a line (24-bit rows: three per 16-px group) or per 16-px group (32-bit rows)
+    auto grid = [&](int band) { return dim3(b200_ceil_div((kind <= SWS_OUT_BGR24 ? 3 : 1) * ngroups, PAIR_THREADS), b200_ceil_div(npairs, band), nf); };
     switch (kind) {
     case SWS_OUT_RGB24: sws_vscale_rgb24_pair_kernel<SWS_OUT_RGB24, NV><<<grid(PairShape<SWS_OUT_RGB24>::band), block, 0, stream>>>(b, dt, col, ngroups, npairs); break;
     case SWS_OUT_BGR24: sws_vscale_rgb24_pair_kernel<SWS_OUT_BGR24, NV><<<grid(PairShape<SWS_OUT_BGR24>::band), block, 0, stream>>>(b, dt, col, ngroups, npairs); break;

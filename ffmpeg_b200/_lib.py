@@ -240,6 +240,13 @@ class Vp9Filter(C.Structure):
 VP9_INTRA_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_void_p)
 
 
+class HevcIntraReconOp(C.Structure):
+    """B200HevcIntraReconOp (include/b200dsp.h), 32 bytes"""
+    _fields_ = [("coef_off", C.c_int64), ("x", C.c_int32), ("y", C.c_int32), ("plane", C.c_uint8), ("log2_size", C.c_uint8), ("mode", C.c_uint8),
+                ("tu_kind", C.c_uint8), ("flags", C.c_uint16), ("tu_flags", C.c_uint8), ("reserved0", C.c_uint8), ("col_limit", C.c_int32),
+                ("reserved", C.c_uint8 * 4)]
+
+
 class Vp9IntraOp(C.Structure):
     """B200Vp9IntraOp (include/b200dsp.h), 32 bytes"""
     _fields_ = [("coef_off", C.c_int64), ("x", C.c_int32), ("y", C.c_int32), ("eob", C.c_uint16), ("plane", C.c_uint8), ("tx", C.c_uint8),
@@ -366,6 +373,9 @@ PROTOTYPES = {
     "b200_hevc_pred_init": (C.c_int, [vp, C.c_int]),
     "b200_hevc_intra_pred_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_ssize_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64, vp, vp,
                                                     C.c_ssize_t, C.c_int]),
+    "b200_hevc_intra_recon_picture_device": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_ssize_t, C.c_ssize_t, C.c_int64, vp,
+                                                       vp, vp, C.c_ssize_t, C.c_int]),
+    "b200_hevc_intra_timeouts": (C.c_int, [vp, vp]),
     "b200_vp9_dsp_init": (C.c_int, [vp, C.c_int]),
     "b200_vp9_mc_batch_device": (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_int64, vp, vp, C.c_ssize_t]),
     "b200_vp9_dsp_init_itxfm": (C.c_int, [vp, C.c_int]),

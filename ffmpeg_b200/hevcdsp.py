@@ -7,7 +7,8 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import lib, check, vp, HEVCDSPContext, HevcMcOp, HevcTuOp, HevcDbkSeg, HevcSaoCtb, SAOParams, HevcIntraOp, HEVCPredContext
+from ._lib import lib, check, vp, HEVCDSPContext, HevcMcOp, HevcTuOp, HevcDbkSeg, HevcSaoCtb, SAOParams, HevcIntraOp, HEVCPredContext, \
+    HevcIntraReconOp
 
 UNI, UNI_W, BI, BI_W = range(4)                 # B200HevcMcOp.kind
 OP_DTYPE = np.dtype([("dst_off", "<i8"), ("ref_off", "<i8", 2), ("x", "<i4", 2), ("y", "<i4", 2), ("mx", "u1", 2), ("my", "u1", 2),
@@ -57,6 +58,12 @@ SAO_EDGE_RESTORE = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_ss
  INTRA_STRONG) = (1 << k for k in range(8))     # B200HevcIntraOp.flags
 INTRA_DTYPE = np.dtype([("x", "<i4"), ("y", "<i4"), ("log2_size", "u1"), ("mode", "u1"), ("flags", "<u2"), ("reserved", "u1", 4)])
 assert INTRA_DTYPE.itemsize == C.sizeof(HevcIntraOp) == 16
+
+TU_NONE = 0xFF                                  # B200HevcIntraReconOp.tu_kind of a TU without residual (cbf 0)
+RECON_DTYPE = np.dtype([("coef_off", "<i8"), ("x", "<i4"), ("y", "<i4"), ("plane", "u1"), ("log2_size", "u1"), ("mode", "u1"),
+                        ("tu_kind", "u1"), ("flags", "<u2"), ("tu_flags", "u1"), ("reserved0", "u1"), ("col_limit", "<i4"),
+                        ("reserved", "u1", 4)])
+assert RECON_DTYPE.itemsize == C.sizeof(HevcIntraReconOp) == 32
 
 # HEVCPredContext's member signatures: planar (src, top, left, stride); dc (src, top, left, stride, log2_size, c_idx); angular (src,
 # top, left, stride, c_idx, mode); 3-tap (filtered_left, filtered_top, left, top, size); strong (filtered_top, left, top)
@@ -138,6 +145,25 @@ def hevc_intra_pred_batch_device(device, bit_depth, pix, stride, width, height, 
     return check(lib().b200_hevc_intra_pred_batch_device(device.handle, bit_depth, vp(_dptr(pix)), stride, width, height, hshift, vshift, nops,
                                                          vp(_dptr(ops)), None if intra_map is None else vp(_dptr(intra_map)), map_stride,
                                                          log2_min_pu_size), "hevc_intra_pred_batch_device")
+
+
+def hevc_intra_recon_picture_device(device, bit_depth, chroma_format_idc, width, height, planes, ls_y, ls_uv, nops, ops, coef,
+                                    intra_map=None, map_stride=0, log2_min_pu_size=0):
+    """every intra TU of a picture, all components, in decode order, in place (device): planes = 3 sample tensors (or device addresses;
+    only the first with chroma_format_idc 0), line sizes in bytes; ops = RECON_DTYPE records (a uint8 tensor of nops * 32 bytes); coef
+    an int16 tensor, read only; intra_map as for hevc_intra_pred_batch_device"""
+    arr = (C.c_void_p * 3)(*[_dptr(p) if p is not None else None for p in (list(planes) + [None, None])[:3]])
+    return check(lib().b200_hevc_intra_recon_picture_device(device.handle, bit_depth, chroma_format_idc, width, height, arr, ls_y, ls_uv, nops,
+                                                            vp(_dptr(ops)), vp(_dptr(coef)),
+                                                            None if intra_map is None else vp(_dptr(intra_map)), map_stride,
+                                                            log2_min_pu_size), "hevc_intra_recon_picture_device")
+
+
+def hevc_intra_timeouts(device):
+    """waits of the intra picture entry that ran out on this device since the process started (after the device's stream is done)"""
+    n = C.c_int64()
+    check(lib().b200_hevc_intra_timeouts(device.handle, C.byref(n)), "hevc_intra_timeouts")
+    return n.value
 
 
 def hevc_mc_batch_device(device, bit_depth, epel, nops, ops, dst, dst_stride, ref, ref_stride, pic_w, pic_h):

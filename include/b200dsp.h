@@ -654,6 +654,59 @@ int  b200_hevc_intra_pred_batch_device(B200Device *dev, int bit_depth, uint8_t *
                                        int vshift, int64_t nops, const B200HevcIntraOp *ops, const uint8_t *intra_map, ptrdiff_t map_stride,
                                        int log2_min_pu_size);
 
+/* One intra transform unit of b200_hevc_intra_recon_picture_device: a call of s->hpc.intra_pred[log2_size - 2] and the residual of
+ * ff_hevc_hls_residual_coding that hls_transform_unit (hevc/hevcdec.c:1306-1513) adds after it.  plane, x, y, log2_size, mode and flags
+ * mean what B200HevcIntraOp's fields mean for that plane (x / y multiples of 4).  The residual is B200HevcTuOp's: tu_kind, tu_flags
+ * (B200_HEVC_TU_RDPCM / RDPCM_VER / ROTATE), col_limit and the (1 << log2_size)^2 coefficients at coef + coef_off (a multiple of 8);
+ * tu_kind = B200_HEVC_TU_NONE for a TU whose cbf is 0 (prediction only, coef_off ignored). */
+#define B200_HEVC_TU_NONE 0xFF
+typedef struct B200HevcIntraReconOp {
+    int64_t  coef_off;    /* int16 elements, into coef */
+    int32_t  x, y;        /* the TU's top-left in plane samples */
+    uint8_t  plane;       /* 0 luma, 1 Cb, 2 Cr */
+    uint8_t  log2_size;   /* 2..5 */
+    uint8_t  mode;        /* as B200HevcIntraOp.mode */
+    uint8_t  tu_kind;     /* B200_HEVC_TU_* or B200_HEVC_TU_NONE */
+    uint16_t flags;       /* B200_HEVC_INTRA_* */
+    uint8_t  tu_flags;    /* B200_HEVC_TU_RDPCM, B200_HEVC_TU_RDPCM_VER, B200_HEVC_TU_ROTATE */
+    uint8_t  reserved0;
+    int32_t  col_limit;   /* B200_HEVC_TU_IDCT only */
+    uint8_t  reserved[4];
+} B200HevcIntraReconOp;
+#ifdef __cplusplus
+static_assert(sizeof(B200HevcIntraReconOp) == 32, "B200HevcIntraReconOp is 32 bytes");
+#else
+_Static_assert(sizeof(B200HevcIntraReconOp) == 32, "B200HevcIntraReconOp is 32 bytes");
+#endif
+/* Intra reconstruction of a whole HEVC picture in one call, DEVICE pointers (planes, ops, coef, intra_map), asynchronous on the device's
+ * stream.  `ops` lists every intra TU of the picture, all components, in decode order (the order hls_transform_unit calls intra_pred).
+ * The result is, for each op in that order, intra_pred as b200_hevc_intra_pred_batch_device defines it, then the residual as
+ * b200_hevc_transform_add_batch_device defines it, on planes that already hold the picture's inter reconstruction and PCM samples: record
+ * one op per TU and make this call after the inter MC and residual calls and before deblocking.  width / height: the luma picture size;
+ * chroma_format_idc 0..3 gives the chroma planes' shifts (4:2:0, 4:2:2, 4:4:4; 0: luma only, planes[1] / [2] unused).  ls_y / ls_uv:
+ * the line sizes in bytes.  intra_map, map_stride and log2_min_pu_size mean what they mean for the batch entry (one map for all
+ * components).  `coef` (int16) is read only.
+ * Not covered: cross-component prediction (4:4:4 range extensions, hevcdec.c:1398, where a chroma TU adds part of the luma residual) and
+ * pictures whose PPS enables current-picture referencing; decode those with the batch entries.
+ * The ops of one call write disjoint blocks (decode order gives that; where ops overlap, the samples of the overlap and of the ops
+ * that read them are undefined).  An op waits for the earlier ops of its plane that write the samples it reads.  An op that the batch
+ * entries would refuse writes nothing and holds up no later op: log2_size or mode out of range, an undefined tu_kind, DST4 on a TU other than 4x4, x / y not
+ * multiples of 4, coef_off negative or not a multiple of 8 (with a residual), the block or its flagged neighbours outside the plane, a
+ * plane index above 2 or above 0 with chroma_format_idc 0.
+ * Returns 0, or B200_EINVAL (launching nothing) for NULL planes, a depth other than 8, 9, 10 or 12, chroma_format_idc outside 0..3,
+ * width or height outside 1..65536, a line size shorter than a plane row or not a multiple of 4 samples, a plane not aligned to 4
+ * samples, nops outside 0..2^30, an intra_map with map_stride < (width >> log2_min_pu_size) or log2_min_pu_size outside 2..6, or
+ * (nops > 0) ops NULL or not aligned to 16 bytes, coef NULL or not aligned to 16 bytes; nops == 0 returns 0. */
+int  b200_hevc_intra_recon_picture_device(B200Device *dev, int bit_depth, int chroma_format_idc, int width, int height,
+                                          uint8_t *const planes[3], ptrdiff_t ls_y, ptrdiff_t ls_uv, int64_t nops,
+                                          const B200HevcIntraReconOp *ops, const int16_t *coef, const uint8_t *intra_map,
+                                          ptrdiff_t map_stride, int log2_min_pu_size);
+/* The picture entry's waits are bounded by about one second each, after which the op runs anyway (wrong samples rather than a hung
+ * GPU) and a per-device counter is incremented.  This waits for the device's stream and stores in *count the number of the picture
+ * entry's waits that ran out on that device since the process started (the VP9 entries count theirs apart).  0; B200_EINVAL for
+ * count == NULL; B200_ENODEV; B200_EEXTERNAL. */
+int  b200_hevc_intra_timeouts(B200Device *dev, int64_t *count);
+
 /* VP9 motion compensation: VP9DSPContext (libavcodec/vp9dsp.h:40-122) in the reference's member order and types.
  * b200_vp9_dsp_init() fills mc[5][4][2][2][2] and smc[5][4][2] completely, as ff_vp9dsp_init does through ff_vp9dsp_mc_init
  * (vp9dsp_template.c:2302-2361) and ff_vp9dsp_scaled_mc_init (:2540-2569): [size 0..4 = 64, 32, 16, 8, 4 columns][filter bank in

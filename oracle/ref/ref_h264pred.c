@@ -1,5 +1,5 @@
 /* TEST INFRASTRUCTURE — the reference's H.264 intra prediction (libavcodec/h264pred.c, compiled unmodified where it lies by
- * oracle/ref/h264pred.mk into oracle/_ref/libffref_h264pred.so, next to libffref.so which it links against for ff_crop_tab and
+ * oracle/ref/Makefile into oracle/_ref/libffref_h264pred.so, next to libffref.so which it links against for ff_crop_tab and
  * libavutil) exposed through a flat C ABI, plus the compile-time proof that include/b200dsp.h's B200H264PredContext can be copied
  * member for member into H264PredContext (same size, member offsets and function-pointer types) and that B200_CODEC_ID_H264 is
  * AV_CODEC_ID_H264.  tests/h264predlib.py loads it and reads the marker below. */

@@ -1,5 +1,5 @@
 /* TEST INFRASTRUCTURE — the reference's HEVC deblocking members (libavcodec/hevc/dsp.c, compiled unmodified where it lies by
- * oracle/ref/hevcdbk.mk into oracle/_ref/libffref_hevcdbk.so) exposed through a flat C ABI, called through the HEVCDSPContext that
+ * oracle/ref/Makefile into oracle/_ref/libffref_hevcdbk.so) exposed through a flat C ABI, called through the HEVCDSPContext that
  * ff_hevc_dsp_init fills: one member per call, and a whole plane driven in the decoder's own order (hevc/filter.c:501-676, restated
  * in plane sample coordinates): CTBs in raster order; in each, per 8-row band, the band's vertical edges, then its horizontal edge
  * lagged 8 samples to the left (the last 8 columns of a CTB wait for the next CTB's first vertical edge).  tests/hevcdbklib.py loads it. */

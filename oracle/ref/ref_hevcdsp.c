@@ -1,4 +1,4 @@
-/* TEST INFRASTRUCTURE — the reference's HEVC DSP (libavcodec/hevc/dsp.c, compiled unmodified where it lies by oracle/ref/hevcdsp.mk
+/* TEST INFRASTRUCTURE — the reference's HEVC DSP (libavcodec/hevc/dsp.c, compiled unmodified where it lies by oracle/ref/Makefile
  * into oracle/_ref/libffref_hevcdsp.so, next to libffref.so which it links against for emulated_edge_mc) exposed through a flat C
  * ABI: one table member per call, and the decoder's per-prediction-unit sequence (hevcdec.c:1722-2040: the emulated_edge_mc window
  * where the block's window leaves the picture, then the member calls) for a batch of B200HevcMcOp.  Plus the compile-time proof that

@@ -1,5 +1,5 @@
 /* TEST INFRASTRUCTURE — the reference's HEVC residual members (libavcodec/hevc/dsp.c, compiled unmodified where it lies by
- * oracle/ref/hevcidct.mk into oracle/_ref/libffref_hevcidct.so) exposed through a flat C ABI: one member per call, and the decoder's
+ * oracle/ref/Makefile into oracle/_ref/libffref_hevcidct.so) exposed through a flat C ABI: one member per call, and the decoder's
  * per-transform-unit sequence (hevc/cabac.c:1550-1592, then add_residual) for a batch of B200HevcTuOp, each op on a copy of its
  * coefficients.  tests/hevcidctlib.py loads it. */
 #include <stdint.h>

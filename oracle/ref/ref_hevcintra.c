@@ -1,4 +1,4 @@
-/* TEST INFRASTRUCTURE — the reference's HEVC intra reconstruction of a whole picture (built by oracle/ref/hevcintra.mk into
+/* TEST INFRASTRUCTURE — the reference's HEVC intra reconstruction of a whole picture (built by oracle/ref/Makefile into
  * oracle/_ref/libffref_hevcintra.so; tests/hevcintralib.py loads it): all three components TU by TU in decode order, each TU through the
  * reference's own intra_pred[] (libavcodec/hevc/pred.c, compiled unmodified where it lies) over minimal decoder contexts, then its
  * residual through ffref_hevc_tu_batch (ref_hevcidct.c: the decoder's member sequence of hevc/cabac.c:1550-1592 and add_residual). */

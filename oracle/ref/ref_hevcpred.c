@@ -1,4 +1,4 @@
-/* TEST INFRASTRUCTURE — the reference's HEVC intra prediction exposed through a flat C ABI (built by oracle/ref/hevcpred.mk into
+/* TEST INFRASTRUCTURE — the reference's HEVC intra prediction exposed through a flat C ABI (built by oracle/ref/Makefile into
  * oracle/_ref/libffref_hevcpred.so; tests/hevcpredlib.py loads it):
  *  - the members of HEVCPredContext (libavcodec/hevc/pred.c, compiled unmodified where it lies), called through the context
  *    ff_hevc_pred_init fills;

@@ -1,4 +1,4 @@
-/* TEST INFRASTRUCTURE — the reference's HEVC sample adaptive offset exposed through a flat C ABI (built by oracle/ref/hevcsao.mk into
+/* TEST INFRASTRUCTURE — the reference's HEVC sample adaptive offset exposed through a flat C ABI (built by oracle/ref/Makefile into
  * oracle/_ref/libffref_hevcsao.so; tests/hevcsaolib.py loads it):
  *  - the SAO members of HEVCDSPContext (libavcodec/hevc/dsp.c, compiled unmodified where it lies), called through the context
  *    ff_hevc_dsp_init fills, one call at a time or, for sao_edge_restore, swept over every class, border and edge-flag combination

@@ -1,5 +1,5 @@
 /* TEST INFRASTRUCTURE — the reference's VP9 DSP (libavcodec/vp9dsp.c, vp9dsp_8bpp.c, vp9dsp_10bpp.c, vp9dsp_12bpp.c, compiled
- * unmodified where they lie by oracle/ref/vp9dsp.mk into oracle/_ref/libffref_vp9dsp.so, next to libffref.so which it links against
+ * unmodified where they lie by oracle/ref/Makefile into oracle/_ref/libffref_vp9dsp.so, next to libffref.so which it links against
  * for emulated_edge_mc) exposed through a flat C ABI: one mc / smc table member per call, the address of ff_vp9_subpel_filters, and
  * the decoder's per-block sequence (vp9recon.c:299-551: the emulated_edge_mc window where the decoder's own test says the block's
  * window leaves the picture, then the member call; vp9_mc_template.c: put from the first reference, avg from the second) for a batch

@@ -1,6 +1,6 @@
 /* TEST INFRASTRUCTURE — the reference's VP9 intra reconstruction (libavcodec/vp9recon.c with vp9data.c and the predictors and
  * inverse transforms of vp9dsp.c, vp9dsp_8bpp.c, vp9dsp_10bpp.c, vp9dsp_12bpp.c, compiled unmodified where they lie by
- * oracle/ref/vp9intra.mk into oracle/_ref/libffref_vp9intra.so) exposed through a flat C ABI: one intra_pred member of
+ * oracle/ref/Makefile into oracle/_ref/libffref_vp9intra.so) exposed through a flat C ABI: one intra_pred member of
  * ff_vp9dsp_init(.., bpp, 0) per call, and ff_vp9_intra_recon_{8,16}bpp block by block over a frame on a hand-set VP9Context /
  * VP9TileData / VP9Block, the way decode_b and decode_tiles drive it: dst or the tmp_* buffers by the emu rule of vp9block.c:1368-1386
  * with the copy-back of :1399-1430, and intra_pred_data copied at the end of each superblock row as vp9.c:1387-1398 does.

@@ -1,5 +1,5 @@
 /* TEST INFRASTRUCTURE — the reference's VP9 inverse transforms (libavcodec/vp9dsp.c, vp9dsp_8bpp.c, vp9dsp_10bpp.c, vp9dsp_12bpp.c,
- * compiled unmodified where they lie by oracle/ref/vp9itxfm.mk into oracle/_ref/libffref_vp9itxfm.so) exposed through a flat C ABI:
+ * compiled unmodified where they lie by oracle/ref/Makefile into oracle/_ref/libffref_vp9itxfm.so) exposed through a flat C ABI:
  * one itxfm_add member of ff_vp9dsp_init(.., bpp, 1) per call, the decoder's residual sequence for a batch of B200Vp9TxOp (the member
  * on a copy of each op's coefficients, so the batch's coefficient buffer stays as it was, like the product's read-only entry), and
  * the pointer-sharing facts of the table (vp9dsp_template.c:1755-1778).  tests/vp9itxfmlib.py loads it. */

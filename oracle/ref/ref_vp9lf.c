@@ -1,5 +1,5 @@
 /* TEST INFRASTRUCTURE — the reference's VP9 loop filter (libavcodec/vp9lpf.c with the loop-filter functions of vp9dsp.c,
- * vp9dsp_8bpp.c, vp9dsp_10bpp.c, vp9dsp_12bpp.c, compiled unmodified where they lie by oracle/ref/vp9lf.mk into
+ * vp9dsp_8bpp.c, vp9dsp_10bpp.c, vp9dsp_12bpp.c, compiled unmodified where they lie by oracle/ref/Makefile into
  * oracle/_ref/libffref_vp9lf.so) exposed through a flat C ABI: one loop-filter member of ff_vp9dsp_init(.., bpp, 1) per call, and
  * ff_vp9_loopfilter_sb over a frame's superblocks on a hand-set VP9Context (the fields vp9lpf.c reads: dsp, filter_lut, bytesperpixel,
  * ss_h, ss_v and the current frame's data / linesize), in raster order or in a wavefront order.  tests/vp9lflib.py loads it. */

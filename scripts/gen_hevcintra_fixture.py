@@ -13,7 +13,7 @@ sys.path.insert(0, ROOT)
 import hevcintralib as hl  # noqa: E402
 
 if __name__ == "__main__":
-    assert hl.have_ref(), "build oracle/_ref/libffref_hevcintra.so first (oracle/ref/hevcintra.mk)"
+    assert hl.have_ref(), "build oracle/_ref/libffref_hevcintra.so first (oracle/ref/Makefile)"
     with open(hl.FIXTURE, "w") as out:
         for name in hl.FIXTURE_NAMES:
             out.write(f"{name} {hl.digest(hl.ref_picture(hl.fixture_case(name)))}\n")

@@ -11,7 +11,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import hevcpredlib as hl  # noqa: E402
 
 if __name__ == "__main__":
-    assert hl.have_ref(), "build oracle/_ref/libffref_hevcpred.so first (oracle/ref/hevcpred.mk)"
+    assert hl.have_ref(), "build oracle/_ref/libffref_hevcpred.so first (oracle/ref/Makefile)"
     with open(hl.FIXTURE, "w") as f:
         for depth in hl.DEPTHS:
             for name in hl.FIXTURE_CFMT:

@@ -15,7 +15,7 @@ sys.path.insert(0, ROOT)
 import vp9intralib as vi  # noqa: E402
 
 if __name__ == "__main__":
-    assert vi.have_ref(), "build oracle/_ref/libffref_vp9intra.so first (oracle/ref/vp9intra.mk)"
+    assert vi.have_ref(), "build oracle/_ref/libffref_vp9intra.so first (oracle/ref/Makefile)"
     with open(vi.FIXTURE, "w") as out:
         for name in vi.FIXTURE_NAMES:
             f = vi.frame_case(name)

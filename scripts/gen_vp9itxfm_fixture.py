@@ -12,7 +12,7 @@ sys.path.insert(0, ROOT)
 import vp9itxfmlib as vt  # noqa: E402
 
 if __name__ == "__main__":
-    assert vt.have_ref(), "build oracle/_ref/libffref_vp9itxfm.so first (oracle/ref/vp9itxfm.mk)"
+    assert vt.have_ref(), "build oracle/_ref/libffref_vp9itxfm.so first (oracle/ref/Makefile)"
     with open(vt.FIXTURE, "w") as f:
         for depth in vt.DEPTHS:
             for cls in vt.FIXTURE_CLASSES:

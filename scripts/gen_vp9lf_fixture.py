@@ -12,7 +12,7 @@ sys.path.insert(0, ROOT)
 import vp9lflib as vl  # noqa: E402
 
 if __name__ == "__main__":
-    assert vl.have_ref(), "build oracle/_ref/libffref_vp9lf.so first (oracle/ref/vp9lf.mk)"
+    assert vl.have_ref(), "build oracle/_ref/libffref_vp9lf.so first (oracle/ref/Makefile)"
     with open(vl.FIXTURE, "w") as f:
         for name in vl.FIXTURE_NAMES:
             f.write(f"{name} {vl.digest(vl.ref_frame(vl.frame_case(name)))}\n")

@@ -12,7 +12,7 @@ sys.path.insert(0, ROOT)
 import vp9mclib as vm  # noqa: E402
 
 if __name__ == "__main__":
-    assert vm.have_ref(), "build oracle/_ref/libffref_vp9dsp.so first (oracle/ref/vp9dsp.mk)"
+    assert vm.have_ref(), "build oracle/_ref/libffref_vp9dsp.so first (oracle/ref/Makefile)"
     with open(vm.FIXTURE, "w") as f:
         for depth in vm.DEPTHS:
             for chroma in (0, 1):

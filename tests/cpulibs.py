@@ -1,6 +1,7 @@
 """ctypes loaders for the two CPU checkers (test infrastructure only):
    - oracle/liboracle.so      : our plain-C restatement (travels, always built by __graft_entry__.build())
-   - oracle/_ref/libffref.so  : the unmodified reference compiled by oracle/ref/Makefile (present when built here)
+   - oracle/_ref/libffref.so  : the unmodified reference compiled by oracle/ref/Makefile (present when built here), and next to it
+                                one libffref_<feature>.so per DSP feature (ref_lib), which links against libffref.so
 """
 import ctypes as C
 import os
@@ -8,7 +9,8 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ORACLE_SO = os.path.join(ROOT, "oracle", "liboracle.so")
-REF_SO = os.path.join(ROOT, "oracle", "_ref", "libffref.so")
+REF_DIR = os.path.join(ROOT, "oracle", "_ref")
+REF_SO = os.path.join(REF_DIR, "libffref.so")
 
 SWS_FAST_BILINEAR, SWS_BILINEAR, SWS_BICUBIC, SWS_POINT, SWS_AREA, SWS_BICUBLIN = 1, 2, 4, 0x10, 0x20, 0x40
 SWS_FULL_CHR_H_INT, SWS_ACCURATE_RND, SWS_BITEXACT = 0x2000, 0x40000, 0x80000
@@ -26,6 +28,7 @@ def ptr(a, t=u8p):
 
 _oracle = None
 _ref = None
+_ref_libs = {}
 
 
 def oracle():
@@ -89,16 +92,25 @@ def oracle():
     return _oracle
 
 
-def have_ref():
-    return os.path.exists(REF_SO)
+def have_ref(lib=None):
+    """whether oracle/_ref/libffref.so is built and, given a feature library's name (e.g. "libffref_hevcsao"), that library too"""
+    return os.path.exists(REF_SO) and (lib is None or os.path.exists(os.path.join(REF_DIR, lib + ".so")))
+
+
+def ref_lib(lib):
+    """the feature library oracle/_ref/<lib>.so, loaded once"""
+    if lib not in _ref_libs:
+        _ref_libs[lib] = C.CDLL(os.path.join(REF_DIR, lib + ".so"))
+    return _ref_libs[lib]
 
 
 # What the reference computed, for machines without oracle/_ref: each RefCheck block of a test keeps one running digest of the
-# reference's results, keyed by the test's module file, name (with parameters) and the block's position in the test (the tests'
-# inputs are seeded, so the sequence is fixed).  With the reference built and FFDSP_RECORD_REF=1 in the environment, the digests are (re)written at exit.
+# reference's results, keyed by the test's module file, name (with parameters) and the block's position among the test's blocks on
+# the same digest file (the tests' inputs are seeded, so the sequence is fixed).  With the reference built and FFDSP_RECORD_REF=1 in
+# the environment, the digests are (re)written at exit.
 REF_DIGESTS = os.path.join(ROOT, "tests", "golden", "ref_digests.json")
 _digests = {}                                                       # digest file -> its stored digests
-_blocks = {}
+_blocks = {}                                                        # (digest file, test) -> blocks entered so far
 
 
 def _write_digests(path):
@@ -108,14 +120,35 @@ def _write_digests(path):
         f.write("\n")
 
 
+def ref_digest(values, h=None):
+    """RefCheck's digest of `values` (an array, a number or a sequence of them): the first 32 hex digits of their sha256.  Given a
+    running sha256 `h`, `values` are added to it and the digest is of everything it has been fed (a block's results so far)."""
+    import hashlib
+    h = hashlib.sha256() if h is None else h
+    for x in (values if isinstance(values, (list, tuple)) else [values]):
+        if isinstance(x, np.ndarray):
+            h.update(f"{x.dtype.str}{x.shape}".encode())
+            h.update(np.ascontiguousarray(x).tobytes())
+        else:
+            h.update(repr(x if x is None else int(x)).encode())
+    return h.hexdigest()[:32]
+
+
+def stored_digest(digests, key):
+    """the digest stored under `key` in the digest file `digests`, to compare a result with one that another test's RefCheck stored"""
+    import json
+    return json.load(open(digests))[key]
+
+
 class RefCheck:
     """with RefCheck() as rc: assert rc.same(ours, lambda: theirs) -- `ours` is an array, a number or a sequence of them.
-    Where oracle/_ref/libffref.so is built, every same() compares with the reference's result at once and the block's end also
+    Where the reference is built (have_ref(lib)), every same() compares with the reference's result at once and the block's end also
     checks the stored digest (so a stale file shows here too); elsewhere same() only accumulates `ours`, and the block's end
-    compares the accumulated digest with the stored one.  `digests` names the file that keeps them (default REF_DIGESTS)."""
+    compares the accumulated digest with the stored one.  `digests` names the file that keeps them (default REF_DIGESTS); `lib`
+    names the feature library that the block's reference calls load (None: libffref.so alone)."""
 
-    def __init__(self, digests=REF_DIGESTS):
-        self.path = digests
+    def __init__(self, digests=REF_DIGESTS, lib=None):
+        self.path, self.lib = digests, lib
 
     def __enter__(self):
         import hashlib
@@ -123,9 +156,10 @@ class RefCheck:
         nodeid = os.environ.get("PYTEST_CURRENT_TEST", "?").rsplit(" (", 1)[0]
         path, _, name = nodeid.partition("::")
         test = f"{os.path.basename(path)}::{name}"                   # the same whatever directory pytest runs from
-        k = _blocks[test] = _blocks.get(test, -1) + 1
+        k = _blocks[self.path, test] = _blocks.get((self.path, test), -1) + 1
         self.key, self.h = f"{test}#{k}", hashlib.sha256()
-        self.live, self.record = have_ref(), have_ref() and os.environ.get("FFDSP_RECORD_REF") == "1"
+        self.live = have_ref(self.lib)
+        self.record = self.live and os.environ.get("FFDSP_RECORD_REF") == "1"
         if self.path not in _digests:
             _digests[self.path] = json.load(open(self.path)) if os.path.exists(self.path) else {}
             if self.record:
@@ -135,20 +169,12 @@ class RefCheck:
         assert self.live or self.key in self.stored, f"no stored reference result for {self.key} ({self.path})"
         return self
 
-    def _add(self, v):
-        for x in (v if isinstance(v, (list, tuple)) else [v]):
-            if isinstance(x, np.ndarray):
-                self.h.update(f"{x.dtype.str}{x.shape}".encode())
-                self.h.update(np.ascontiguousarray(x).tobytes())
-            else:
-                self.h.update(repr(x if x is None else int(x)).encode())
-
     def same(self, ours, ref_fn):
         if not self.live:
-            self._add(ours)
+            ref_digest(ours, self.h)
             return True
         theirs = ref_fn()
-        self._add(theirs)
+        ref_digest(theirs, self.h)
         if isinstance(ours, (list, tuple)):
             return len(ours) == len(theirs) and all(np.array_equal(a, b) for a, b in zip(ours, theirs))
         return bool(np.array_equal(ours, theirs))
@@ -156,11 +182,12 @@ class RefCheck:
     def __exit__(self, typ, *_):
         if typ is not None:
             return False
+        digest = ref_digest((), self.h)
         if self.record:
-            self.stored[self.key] = self.h.hexdigest()[:32]
+            self.stored[self.key] = digest
         else:
             assert self.key in self.stored, f"no stored reference result for {self.key} ({self.path})"
-            assert self.h.hexdigest()[:32] == self.stored[self.key], f"differs from the stored reference results ({self.key})"
+            assert digest == self.stored[self.key], f"differs from the stored reference results ({self.key})"
         return False
 
 

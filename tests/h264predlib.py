@@ -1,10 +1,8 @@
 """Test infrastructure for H.264 intra prediction (H264PredContext): the seeded case generator, runners of the checker
-(oracle/liboracle.so, orc_h264_pred) and of the compiled reference (oracle/_ref/libffref_h264pred.so, built by oracle/ref/h264pred.mk),
+(oracle/liboracle.so, orc_h264_pred) and of the compiled reference (oracle/_ref/libffref_h264pred.so, built by oracle/ref/Makefile),
 and RefCheck, which keeps the reference's results as digests in tests/golden/h264pred_ref_digests.json for machines without the
 reference."""
 import ctypes as C
-import hashlib
-import json
 import os
 
 import numpy as np
@@ -12,78 +10,20 @@ import numpy as np
 import cpulibs as cl
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_SO = os.path.join(ROOT, "oracle", "_ref", "libffref_h264pred.so")
+REF_LIB = "libffref_h264pred"
 REF_DIGESTS = os.path.join(ROOT, "tests", "golden", "h264pred_ref_digests.json")
-_ref = None
 
 
 def have_ref():
-    return os.path.exists(REF_SO)
+    return cl.have_ref(REF_LIB)
 
 
 def ref():
-    global _ref
-    if _ref is None:
-        _ref = C.CDLL(REF_SO)
-    return _ref
+    return cl.ref_lib(REF_LIB)
 
 
-_digests = None
-_blocks = {}
-
-
-def _write_digests():
-    with open(REF_DIGESTS, "w") as f:
-        json.dump(_digests, f, indent=0, sort_keys=True)
-        f.write("\n")
-
-
-class RefCheck:
-    """with RefCheck() as rc: assert rc.same(ours, lambda: theirs) -- the scheme of cpulibs.RefCheck with this path's own digest file.
-    Where libffref_h264pred.so is built, every same() compares with the reference's result at once and the block's end also checks the
-    stored digest; elsewhere same() only accumulates `ours` and the block's end compares that digest with the stored one.  With the
-    reference built and FFDSP_RECORD_REF=1 in the environment, the digests are (re)written at exit."""
-
-    def __enter__(self):
-        global _digests
-        nodeid = os.environ.get("PYTEST_CURRENT_TEST", "?").rsplit(" (", 1)[0]
-        path, _, name = nodeid.partition("::")
-        test = f"{os.path.basename(path)}::{name}"
-        k = _blocks[test] = _blocks.get(test, -1) + 1
-        self.key, self.h = f"{test}#{k}", hashlib.sha256()
-        self.live, self.record = have_ref(), have_ref() and os.environ.get("FFDSP_RECORD_REF") == "1"
-        if _digests is None:
-            _digests = json.load(open(REF_DIGESTS)) if os.path.exists(REF_DIGESTS) else {}
-            if self.record:
-                import atexit
-                atexit.register(_write_digests)
-        assert self.live or self.key in _digests, f"no stored reference result for {self.key} ({REF_DIGESTS})"
-        return self
-
-    def _add(self, v):
-        for x in (v if isinstance(v, (list, tuple)) else [v]):
-            self.h.update(f"{x.dtype.str}{x.shape}".encode())
-            self.h.update(np.ascontiguousarray(x).tobytes())
-
-    def same(self, ours, ref_fn):
-        if not self.live:
-            self._add(ours)
-            return True
-        theirs = ref_fn()
-        self._add(theirs)
-        if isinstance(ours, (list, tuple)):
-            return len(ours) == len(theirs) and all(np.array_equal(a, b) for a, b in zip(ours, theirs))
-        return bool(np.array_equal(ours, theirs))
-
-    def __exit__(self, typ, *_):
-        if typ is not None:
-            return False
-        if self.record:
-            _digests[self.key] = self.h.hexdigest()[:32]
-        else:
-            assert self.key in _digests, f"no stored reference result for {self.key} ({REF_DIGESTS})"
-            assert self.h.hexdigest()[:32] == _digests[self.key], f"differs from the stored reference results ({self.key})"
-        return False
+def RefCheck():
+    return cl.RefCheck(REF_DIGESTS, REF_LIB)
 
 
 # ---------------------------------------------------------------- H.264 intra prediction (libavcodec/h264pred_template.c)

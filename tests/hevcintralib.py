@@ -5,7 +5,7 @@ optionally sparse intra TUs among prefilled inter samples) whose TUs of all comp
 (hevc/hevcdec.c:1306-1513) calls intra_pred: luma, then with a residual each Cb block then each Cr block, predicted and added one after
 the other, without one Cb, Cr and the second 4:2:2 pair; chroma of 4x4 luma at blk_idx 3.  The neighbour flags, z-scan checks, content
 and intra maps are hevcpredlib's; coefficients and TU kinds are hevcidctlib's.  Runners of the checker (orc_hevc_intra_picture, in decode
-order or with no dependencies), of the compiled reference (oracle/_ref/libffref_hevcintra.so, built by oracle/ref/hevcintra.mk), of the
+order or with no dependencies), of the compiled reference (oracle/_ref/libffref_hevcintra.so, built by oracle/ref/Makefile), of the
 per-level path (one prediction and one residual batch per dependency level and plane), and RefCheck with its own digest file
 tests/golden/hevcintra_ref_digests.json."""
 import ctypes as C
@@ -15,34 +15,33 @@ import os
 
 import numpy as np
 
+import cpulibs as cl
 import hevcidctlib as hi
 import hevcpredlib as hp
 from ffmpeg_b200.hevcdsp import (RECON_DTYPE, TU_NONE, INTRA_DTYPE, TU_DTYPE, INTRA_CAND_BL, INTRA_CAND_L, INTRA_CAND_UL, INTRA_CAND_U,
                                  INTRA_CAND_UR, INTRA_LUMA, INTRA_SMOOTH, INTRA_STRONG)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_SO = os.path.join(ROOT, "oracle", "_ref", "libffref_hevcintra.so")
+REF_LIB = "libffref_hevcintra"
 REF_DIGESTS = os.path.join(ROOT, "tests", "golden", "hevcintra_ref_digests.json")
 FIXTURE = os.path.join(ROOT, "tests", "golden", "hevcintra_hashes.txt")
 DEPTHS = (8, 9, 10, 12)
 MARGIN = 8                                             # guard samples around a plane (and up to 15 more on the right: rows of 16 samples)
 
-_ref = None
-
 
 def have_ref():
-    return os.path.exists(REF_SO)
+    return cl.have_ref(REF_LIB)
 
 
 def ref():
-    global _ref
-    if _ref is None:
-        _ref = C.CDLL(REF_SO)
-    return _ref
+    return cl.ref_lib(REF_LIB)
+
+
+def RefCheck():
+    return cl.RefCheck(REF_DIGESTS, REF_LIB)
 
 
 def orc():
-    import cpulibs as cl
     L = cl.oracle()
     if not getattr(L, "_hintra_types", False):
         vp = C.c_void_p
@@ -57,46 +56,6 @@ def digest(planes):
     for a in planes:
         h.update(np.ascontiguousarray(a).tobytes())
     return h.hexdigest()
-
-
-_digests = None
-_blocks = {}
-
-
-def _write_digests():
-    with open(REF_DIGESTS, "w") as f:
-        json.dump(_digests, f, indent=0, sort_keys=True)
-        f.write("\n")
-
-
-class RefCheck(hp.RefCheck):
-    """hevcpredlib.RefCheck's scheme with this path's own reference library and digest file"""
-
-    def __enter__(self):
-        global _digests
-        nodeid = os.environ.get("PYTEST_CURRENT_TEST", "?").rsplit(" (", 1)[0]
-        path, _, name = nodeid.partition("::")
-        test = f"{os.path.basename(path)}::{name}"
-        k = _blocks[test] = _blocks.get(test, -1) + 1
-        self.key, self.h = f"{test}#{k}", hashlib.sha256()
-        self.live, self.record = have_ref(), have_ref() and os.environ.get("FFDSP_RECORD_REF") == "1"
-        if _digests is None:
-            _digests = json.load(open(REF_DIGESTS)) if os.path.exists(REF_DIGESTS) else {}
-            if self.record:
-                import atexit
-                atexit.register(_write_digests)
-        assert self.live or self.key in _digests, f"no stored reference result for {self.key} ({REF_DIGESTS})"
-        return self
-
-    def __exit__(self, typ, *_):
-        if typ is not None:
-            return False
-        if self.record:
-            _digests[self.key] = self.h.hexdigest()[:32]
-        else:
-            assert self.key in _digests, f"no stored reference result for {self.key} ({REF_DIGESTS})"
-            assert self.h.hexdigest()[:32] == _digests[self.key], f"differs from the stored reference results ({self.key})"
-        return False
 
 
 # ---------------------------------------------------------------- pictures

@@ -3,22 +3,22 @@
 chroma, constrained intra prediction with mixed intra / inter maps, smoothing and strong smoothing on and off), the decoder's call
 sequence restated (ff_hevc_set_neighbour_available for the na bits, intra_pred's z-scan checks for the op flags, the chroma TU
 placement of hls_transform_unit), the dependency-level scheduler INTEGRATION.md describes (the bench imports it too), runners of the
-compiled reference (oracle/_ref/libffref_hevcpred.so, built by oracle/ref/hevcpred.mk: the members, and whole planes through the
+compiled reference (oracle/_ref/libffref_hevcpred.so, built by oracle/ref/Makefile: the members, and whole planes through the
 reference's own intra_pred), runners of the checker (oracle/liboracle.so: orc_hevc_pred_* / orc_hevc_filter_* / orc_hevc_intra_plane),
 seeded pictures whose 32x32 luma blocks put the strong-smoothing second differences on both sides of the threshold, and RefCheck, which keeps the reference's results as digests in tests/golden/hevcpred_ref_digests.json
 for machines without the reference."""
 import ctypes as C
 import hashlib
-import json
 import os
 
 import numpy as np
 
+import cpulibs as cl
 from ffmpeg_b200.hevcdsp import (INTRA_DTYPE, INTRA_CAND_BL, INTRA_CAND_L, INTRA_CAND_UL, INTRA_CAND_U, INTRA_CAND_UR, INTRA_LUMA,
                                  INTRA_SMOOTH, INTRA_STRONG)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_SO = os.path.join(ROOT, "oracle", "_ref", "libffref_hevcpred.so")
+REF_LIB = "libffref_hevcpred"
 REF_DIGESTS = os.path.join(ROOT, "tests", "golden", "hevcpred_ref_digests.json")
 FIXTURE = os.path.join(ROOT, "tests", "golden", "hevcpred_hashes.txt")
 DEPTHS = (8, 9, 10, 12)
@@ -26,22 +26,20 @@ SHIFTS = {0: (0, 0), 1: (1, 1), 2: (1, 0), 3: (0, 0)}  # chroma_format_idc -> ch
 MARGIN = 8                                             # guard samples around a plane
 SENT8, SENT16 = 0xA5, 0xA5A5
 
-_ref = None
-
 
 def have_ref():
-    return os.path.exists(REF_SO)
+    return cl.have_ref(REF_LIB)
 
 
 def ref():
-    global _ref
-    if _ref is None:
-        _ref = C.CDLL(REF_SO)
-    return _ref
+    return cl.ref_lib(REF_LIB)
+
+
+def RefCheck():
+    return cl.RefCheck(REF_DIGESTS, REF_LIB)
 
 
 def orc():
-    import cpulibs as cl
     L = cl.oracle()
     if not getattr(L, "_ipred_types", False):
         vp = C.c_void_p
@@ -66,79 +64,6 @@ def sentinel(depth):
 
 def digest(a):
     return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
-
-
-_digests = None
-_blocks = {}
-
-
-def _write_digests():
-    with open(REF_DIGESTS, "w") as f:
-        json.dump(_digests, f, indent=0, sort_keys=True)
-        f.write("\n")
-
-
-class RefCheck:
-    """with RefCheck() as rc: assert rc.same(ours, lambda: theirs) -- hevcsaolib.RefCheck's scheme with this path's own digest file:
-    live comparison (and a check of the stored digest) where libffref_hevcpred.so is built, the stored digest of `ours` elsewhere;
-    FFDSP_RECORD_REF=1 with the reference built rewrites the digests at exit."""
-
-    def __enter__(self):
-        global _digests
-        nodeid = os.environ.get("PYTEST_CURRENT_TEST", "?").rsplit(" (", 1)[0]
-        path, _, name = nodeid.partition("::")
-        test = f"{os.path.basename(path)}::{name}"
-        k = _blocks[test] = _blocks.get(test, -1) + 1
-        self.key, self.h = f"{test}#{k}", hashlib.sha256()
-        self.live, self.record = have_ref(), have_ref() and os.environ.get("FFDSP_RECORD_REF") == "1"
-        if _digests is None:
-            _digests = json.load(open(REF_DIGESTS)) if os.path.exists(REF_DIGESTS) else {}
-            if self.record:
-                import atexit
-                atexit.register(_write_digests)
-        assert self.live or self.key in _digests, f"no stored reference result for {self.key} ({REF_DIGESTS})"
-        return self
-
-    def _add(self, v):
-        for x in (v if isinstance(v, (list, tuple)) else [v]):
-            x = np.asarray(x)
-            self.h.update(f"{x.dtype.str}{x.shape}".encode())
-            self.h.update(np.ascontiguousarray(x).tobytes())
-
-    def same(self, ours, ref_fn):
-        if not self.live:
-            self._add(ours)
-            return True
-        theirs = ref_fn()
-        self._add(theirs)
-        if isinstance(ours, (list, tuple)):
-            return len(ours) == len(theirs) and all(np.array_equal(a, b) for a, b in zip(ours, theirs))
-        return bool(np.array_equal(ours, theirs))
-
-    def __exit__(self, typ, *_):
-        if typ is not None:
-            return False
-        if self.record:
-            _digests[self.key] = self.h.hexdigest()[:32]
-        else:
-            assert self.key in _digests, f"no stored reference result for {self.key} ({REF_DIGESTS})"
-            assert self.h.hexdigest()[:32] == _digests[self.key], f"differs from the stored reference results ({self.key})"
-        return False
-
-
-def stored_digest(key):
-    """the stored reference digest `key` of tests/golden/hevcpred_ref_digests.json"""
-    return json.load(open(REF_DIGESTS))[key]
-
-
-def digest_like_refcheck(values):
-    """RefCheck's digest of a list of arrays, to compare a result with a digest stored by another test"""
-    h = hashlib.sha256()
-    for x in values:
-        x = np.asarray(x)
-        h.update(f"{x.dtype.str}{x.shape}".encode())
-        h.update(np.ascontiguousarray(x).tobytes())
-    return h.hexdigest()[:32]
 
 
 # ---------------------------------------------------------------- pictures

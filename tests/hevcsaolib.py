@@ -1,12 +1,11 @@
 """Test infrastructure for HEVC sample adaptive offset (the SAO members of HEVCDSPContext and b200_hevc_sao_plane_device): seeded
 picture descriptions (slice and tile maps, loop_filter_across_slices / _tiles, PCM / bypass maps, per-CTB SAO syntax), the
 B200HevcSaoCtb grids derived from them by the recipe INTEGRATION.md documents, runners of the checker (oracle/liboracle.so:
-orc_hevc_sao_*) and of the compiled reference (oracle/_ref/libffref_hevcsao.so, built by oracle/ref/hevcsao.mk: the members, and
+orc_hevc_sao_*) and of the compiled reference (oracle/_ref/libffref_hevcsao.so, built by oracle/ref/Makefile: the members, and
 whole pictures through the decoder's own hevc/filter.c), and RefCheck, which keeps the reference's results as digests in
 tests/golden/hevcsao_ref_digests.json for machines without the reference."""
 import ctypes as C
 import hashlib
-import json
 import os
 
 import numpy as np
@@ -17,7 +16,7 @@ from ffmpeg_b200.hevcdsp import (SAO_DTYPE, SAO_NONE, SAO_BAND, SAO_EDGE, SAO_RE
                                  SAO_DIAG_TL, SAO_DIAG_TR, SAO_DIAG_BR, SAO_DIAG_BL)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_SO = os.path.join(ROOT, "oracle", "_ref", "libffref_hevcsao.so")
+REF_LIB = "libffref_hevcsao"
 REF_DIGESTS = os.path.join(ROOT, "tests", "golden", "hevcsao_ref_digests.json")
 FIXTURE = os.path.join(ROOT, "tests", "golden", "hevcsao_hashes.txt")
 DEPTHS = (8, 9, 10, 12)
@@ -28,19 +27,19 @@ MARGIN = 4         # samples of sentinel around a plane
 SENT8, SENT16 = 0xA5, 0xA5A5
 EDGE_STRIDE = 192  # the edge member's implicit source stride in bytes
 
-_ref = None
-
 
 def have_ref():
-    return os.path.exists(REF_SO)
+    return cl.have_ref(REF_LIB)
 
 
 def ref():
-    global _ref
-    if _ref is None:
-        _ref = C.CDLL(REF_SO)
-        _ref.ffref_hevc_sao_restore_fn.restype = C.c_void_p
-    return _ref
+    L = cl.ref_lib(REF_LIB)
+    L.ffref_hevc_sao_restore_fn.restype = C.c_void_p
+    return L
+
+
+def RefCheck():
+    return cl.RefCheck(REF_DIGESTS, REF_LIB)
 
 
 def orc():
@@ -56,64 +55,6 @@ def orc():
                                          vp, C.c_int64, C.c_int, C.c_int, vp]
         L._sao_types = True
     return L
-
-
-_digests = None
-_blocks = {}
-
-
-def _write_digests():
-    with open(REF_DIGESTS, "w") as f:
-        json.dump(_digests, f, indent=0, sort_keys=True)
-        f.write("\n")
-
-
-class RefCheck:
-    """with RefCheck() as rc: assert rc.same(ours, lambda: theirs) -- hevcdbklib.RefCheck's scheme with this path's own digest file:
-    live comparison (and a check of the stored digest) where libffref_hevcsao.so is built, the stored digest of `ours` elsewhere;
-    FFDSP_RECORD_REF=1 with the reference built rewrites the digests at exit."""
-
-    def __enter__(self):
-        global _digests
-        nodeid = os.environ.get("PYTEST_CURRENT_TEST", "?").rsplit(" (", 1)[0]
-        path, _, name = nodeid.partition("::")
-        test = f"{os.path.basename(path)}::{name}"
-        k = _blocks[test] = _blocks.get(test, -1) + 1
-        self.key, self.h = f"{test}#{k}", hashlib.sha256()
-        self.live, self.record = have_ref(), have_ref() and os.environ.get("FFDSP_RECORD_REF") == "1"
-        if _digests is None:
-            _digests = json.load(open(REF_DIGESTS)) if os.path.exists(REF_DIGESTS) else {}
-            if self.record:
-                import atexit
-                atexit.register(_write_digests)
-        assert self.live or self.key in _digests, f"no stored reference result for {self.key} ({REF_DIGESTS})"
-        return self
-
-    def _add(self, v):
-        for x in (v if isinstance(v, (list, tuple)) else [v]):
-            x = np.asarray(x)
-            self.h.update(f"{x.dtype.str}{x.shape}".encode())
-            self.h.update(np.ascontiguousarray(x).tobytes())
-
-    def same(self, ours, ref_fn):
-        if not self.live:
-            self._add(ours)
-            return True
-        theirs = ref_fn()
-        self._add(theirs)
-        if isinstance(ours, (list, tuple)):
-            return len(ours) == len(theirs) and all(np.array_equal(a, b) for a, b in zip(ours, theirs))
-        return bool(np.array_equal(ours, theirs))
-
-    def __exit__(self, typ, *_):
-        if typ is not None:
-            return False
-        if self.record:
-            _digests[self.key] = self.h.hexdigest()[:32]
-        else:
-            assert self.key in _digests, f"no stored reference result for {self.key} ({REF_DIGESTS})"
-            assert self.h.hexdigest()[:32] == _digests[self.key], f"differs from the stored reference results ({self.key})"
-        return False
 
 
 def sdtype(depth):

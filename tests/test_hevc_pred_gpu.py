@@ -7,6 +7,7 @@ ops lie beyond 2^31 bytes.  Only committed fixtures and the checker are read."""
 import numpy as np
 import pytest
 
+import cpulibs as cl
 import hevcpredlib as hl
 
 pytestmark = pytest.mark.gpu
@@ -84,7 +85,7 @@ def test_strong_threshold(dev, depth):
     p = hl.strong_case(40 + depth, depth)
     got = on_device(dev, p)[0]
     assert np.array_equal(got, hl.orc_plane(p))
-    assert hl.digest_like_refcheck([got]) == hl.stored_digest(f"test_hevc_pred.py::test_emu_strong_threshold[{depth}]#0")
+    assert cl.ref_digest([got]) == cl.stored_digest(hl.REF_DIGESTS, f"test_hevc_pred.py::test_emu_strong_threshold[{depth}]#0")
 
 
 @pytest.mark.parametrize("depth", hl.DEPTHS)
@@ -104,9 +105,9 @@ def test_members_vs_reference(dev, depth):
     from ffmpeg_b200 import hevcdsp
     ctx = hevcdsp.ff_hevc_pred_init(depth)
     ours = [hl.ctx_member(ctx, depth, c) for c in hl.member_cases(700 + depth, depth)]
-    assert hl.digest_like_refcheck(ours) == hl.stored_digest(f"test_hevc_pred.py::test_emu_every_member[{depth}]#0")
+    assert cl.ref_digest(ours) == cl.stored_digest(hl.REF_DIGESTS, f"test_hevc_pred.py::test_emu_every_member[{depth}]#0")
     ours = [a for k, c in enumerate(hl.filter_cases(800 + depth, depth)) for a in hl.ctx_filters(ctx, depth, c, k % 3)]
-    assert hl.digest_like_refcheck(ours) == hl.stored_digest(f"test_hevc_pred.py::test_emu_every_member[{depth}]#1")
+    assert cl.ref_digest(ours) == cl.stored_digest(hl.REF_DIGESTS, f"test_hevc_pred.py::test_emu_every_member[{depth}]#1")
 
 
 def test_out_of_range_ops_change_nothing(dev):

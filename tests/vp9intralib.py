@@ -2,7 +2,7 @@
 a decoder-shaped frame generator (random partition trees per 64x64 superblock in decode_sb's order, intra and inter blocks, per-4x4
 modes, skip, lossless frames, tile columns, every chroma format, odd sizes) with the op list built the way intra_recon's loops clip it,
 runners of the checker (oracle/liboracle.so: orc_vp9_intra_pred, orc_vp9_intra_frame) and of the compiled reference
-(oracle/_ref/libffref_vp9intra.so, built by oracle/ref/vp9intra.mk).  The reference's results are kept as digests in
+(oracle/_ref/libffref_vp9intra.so, built by oracle/ref/Makefile).  The reference's results are kept as digests in
 tests/golden/vp9intra_ref_digests.json (cpulibs.RefCheck) for machines without the reference."""
 import ctypes as C
 import hashlib
@@ -14,7 +14,7 @@ import cpulibs as cl
 from ffmpeg_b200.vp9dsp import INTRA_DTYPE, INTRA_HAVE_LEFT, INTRA_HAVE_RIGHT, INTRA_LOSSLESS
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_SO = os.path.join(ROOT, "oracle", "_ref", "libffref_vp9intra.so")
+REF_LIB = "libffref_vp9intra"
 REF_DIGESTS = os.path.join(ROOT, "tests", "golden", "vp9intra_ref_digests.json")
 FIXTURE = os.path.join(ROOT, "tests", "golden", "vp9intra_hashes.txt")
 DEPTHS = (8, 10, 12)
@@ -23,25 +23,22 @@ MARGIN = 8           # sentinel samples around every plane's area
 # ff_vp9_bwh_tab[1] (vp9data.c): block size in 8x8 units, and [0] in 4x4 units, by BlockSize
 BWH8 = ((8, 8), (8, 4), (4, 8), (4, 4), (4, 2), (2, 4), (2, 2), (2, 1), (1, 2), (1, 1), (1, 1), (1, 1), (1, 1))
 BWH4 = ((16, 16), (16, 8), (8, 16), (8, 8), (8, 4), (4, 8), (4, 4), (4, 2), (2, 4), (2, 2), (2, 1), (1, 2), (1, 1))
-_ref = None
 
 
 def have_ref():
-    return os.path.exists(REF_SO) and cl.have_ref()
+    return cl.have_ref(REF_LIB)
 
 
 def ref():
-    global _ref
-    if _ref is None:
-        _ref = C.CDLL(REF_SO)
-        _ref.ffref_vp9_intra_pred.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_void_p]
-        _ref.ffref_vp9_intra_frame.argtypes = [C.c_int] * 5 + [C.c_void_p, C.c_ssize_t, C.c_ssize_t, C.c_int, C.c_int, C.c_void_p,
-                                                               C.c_void_p, C.c_void_p]
-    return _ref
+    L = cl.ref_lib(REF_LIB)
+    L.ffref_vp9_intra_pred.argtypes = [C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_void_p]
+    L.ffref_vp9_intra_frame.argtypes = [C.c_int] * 5 + [C.c_void_p, C.c_ssize_t, C.c_ssize_t, C.c_int, C.c_int, C.c_void_p,
+                                                        C.c_void_p, C.c_void_p]
+    return L
 
 
 def RefCheck():
-    return cl.RefCheck(REF_DIGESTS)
+    return cl.RefCheck(REF_DIGESTS, REF_LIB)
 
 
 def sdtype(depth):

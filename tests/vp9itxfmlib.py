@@ -1,6 +1,6 @@
 """Test infrastructure for VP9 inverse transforms (the itxfm_add members of VP9DSPContext and b200_vp9_itxfm_add_batch_device): the
 seeded case generators, runners of the checker (oracle/liboracle.so: orc_vp9_itxfm, orc_vp9_itxfm_batch) and of the compiled reference
-(oracle/_ref/libffref_vp9itxfm.so, built by oracle/ref/vp9itxfm.mk).  The reference's results are kept as digests in
+(oracle/_ref/libffref_vp9itxfm.so, built by oracle/ref/Makefile).  The reference's results are kept as digests in
 tests/golden/vp9itxfm_ref_digests.json (cpulibs.RefCheck) for machines without the reference."""
 import ctypes as C
 import hashlib
@@ -12,27 +12,23 @@ import cpulibs as cl
 from ffmpeg_b200.vp9dsp import TX_DTYPE
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_SO = os.path.join(ROOT, "oracle", "_ref", "libffref_vp9itxfm.so")
+REF_LIB = "libffref_vp9itxfm"
 REF_DIGESTS = os.path.join(ROOT, "tests", "golden", "vp9itxfm_ref_digests.json")
 FIXTURE = os.path.join(ROOT, "tests", "golden", "vp9itxfm_hashes.txt")
 DEPTHS = (8, 10, 12)
 CLASSES = ("decoder", "noise", "extremes", "dcmix")
-_ref = None
 
 
 def have_ref():
-    return os.path.exists(REF_SO) and cl.have_ref()
+    return cl.have_ref(REF_LIB)
 
 
 def ref():
-    global _ref
-    if _ref is None:
-        _ref = C.CDLL(REF_SO)
-    return _ref
+    return cl.ref_lib(REF_LIB)
 
 
 def RefCheck():
-    return cl.RefCheck(REF_DIGESTS)
+    return cl.RefCheck(REF_DIGESTS, REF_LIB)
 
 
 def size(tx):

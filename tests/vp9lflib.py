@@ -1,7 +1,7 @@
 """Test infrastructure for the VP9 loop filter (the loop-filter members of VP9DSPContext and b200_vp9_loopfilter_frame_device): seeded
 frames with decoder-shaped loop-filter records (mask_edges, vp9block.c:1142-1262, restated on random partitions, transform sizes, skip
 flags and levels) or arbitrary masks, member calls, and runners of the checker (oracle/liboracle.so: orc_vp9_lf_member, orc_vp9_lf_frame)
-and of the compiled reference (oracle/_ref/libffref_vp9lf.so, built by oracle/ref/vp9lf.mk).  The reference's results are kept as
+and of the compiled reference (oracle/_ref/libffref_vp9lf.so, built by oracle/ref/Makefile).  The reference's results are kept as
 digests in tests/golden/vp9lf_ref_digests.json (cpulibs.RefCheck) for machines without the reference."""
 import ctypes as C
 import hashlib
@@ -13,28 +13,24 @@ import cpulibs as cl
 from ffmpeg_b200.vp9dsp import LF_DTYPE
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_SO = os.path.join(ROOT, "oracle", "_ref", "libffref_vp9lf.so")
+REF_LIB = "libffref_vp9lf"
 REF_DIGESTS = os.path.join(ROOT, "tests", "golden", "vp9lf_ref_digests.json")
 FIXTURE = os.path.join(ROOT, "tests", "golden", "vp9lf_hashes.txt")
 DEPTHS = (8, 10, 12)
 FORMATS = {"420": (1, 1), "422": (1, 0), "440": (0, 1), "444": (0, 0)}     # (ss_h, ss_v)
 MARGIN = 8           # sentinel samples around every plane's area
-_ref = None
 
 
 def have_ref():
-    return os.path.exists(REF_SO) and cl.have_ref()
+    return cl.have_ref(REF_LIB)
 
 
 def ref():
-    global _ref
-    if _ref is None:
-        _ref = C.CDLL(REF_SO)
-    return _ref
+    return cl.ref_lib(REF_LIB)
 
 
 def RefCheck():
-    return cl.RefCheck(REF_DIGESTS)
+    return cl.RefCheck(REF_DIGESTS, REF_LIB)
 
 
 def sdtype(depth):

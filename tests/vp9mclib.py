@@ -1,6 +1,6 @@
 """Test infrastructure for VP9 motion compensation (the mc / smc tables of VP9DSPContext and b200_vp9_mc_batch_device): the seeded case
 generators, runners of the checker (oracle/liboracle.so: orc_vp9_mc, orc_vp9_smc, orc_vp9_mc_batch) and of the compiled reference
-(oracle/_ref/libffref_vp9dsp.so, built by oracle/ref/vp9dsp.mk).  The reference's results are kept as digests in
+(oracle/_ref/libffref_vp9dsp.so, built by oracle/ref/Makefile).  The reference's results are kept as digests in
 tests/golden/vp9mc_ref_digests.json (cpulibs.RefCheck) for machines without the reference."""
 import ctypes as C
 import hashlib
@@ -13,29 +13,25 @@ from ffmpeg_b200._lib import Vp9McRef
 from ffmpeg_b200.vp9dsp import OP_DTYPE, SINGLE, COMPOUND
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_SO = os.path.join(ROOT, "oracle", "_ref", "libffref_vp9dsp.so")
+REF_LIB = "libffref_vp9dsp"
 REF_DIGESTS = os.path.join(ROOT, "tests", "golden", "vp9mc_ref_digests.json")
 FIXTURE = os.path.join(ROOT, "tests", "golden", "vp9mc_hashes.txt")
 DEPTHS = (8, 10, 12)
 WIDTHS = (64, 32, 16, 8, 4)                             # table index 0..4
 BANKS = ("smooth", "regular", "sharp", "bilinear")      # FilterMode order
 STEPS = (1, 5, 8, 15, 16, 17, 20, 31, 32)
-_ref = None
 
 
 def have_ref():
-    return os.path.exists(REF_SO) and cl.have_ref()
+    return cl.have_ref(REF_LIB)
 
 
 def ref():
-    global _ref
-    if _ref is None:
-        _ref = C.CDLL(REF_SO)
-    return _ref
+    return cl.ref_lib(REF_LIB)
 
 
 def RefCheck():
-    return cl.RefCheck(REF_DIGESTS)
+    return cl.RefCheck(REF_DIGESTS, REF_LIB)
 
 
 def sdtype(depth):

@@ -253,6 +253,36 @@ class Vp9IntraOp(C.Structure):
                 ("mode", C.c_uint8), ("flags", C.c_uint8), ("reserved", C.c_uint8 * 10)]
 
 
+VP8_MC_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_ssize_t, C.c_int, C.c_int, C.c_int)
+VP8_WHT_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p)
+VP8_IDCT_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t)
+
+
+class VP8DSPContext(C.Structure):
+    """libavcodec/vp8dsp.h:37-82 (same member order; the loop-filter members, which this library does not fill, are plain pointers)"""
+    _fields_ = [("vp8_luma_dc_wht", VP8_WHT_FUNC), ("vp8_luma_dc_wht_dc", VP8_WHT_FUNC), ("vp8_idct_add", VP8_IDCT_FUNC),
+                ("vp8_idct_dc_add", VP8_IDCT_FUNC), ("vp8_idct_dc_add4y", VP8_IDCT_FUNC), ("vp8_idct_dc_add4uv", VP8_IDCT_FUNC),
+                ("loop_filter", vp * 10), ("put_vp8_epel_pixels_tab", VP8_MC_FUNC * 3 * 3 * 3),
+                ("put_vp8_bilinear_pixels_tab", VP8_MC_FUNC * 3 * 3 * 3)]
+
+
+class Vp8McRef(C.Structure):
+    """B200Vp8McRef (include/b200dsp.h), 40 bytes"""
+    _fields_ = [("y", C.c_void_p), ("u", C.c_void_p), ("v", C.c_void_p), ("ls_y", C.c_ssize_t), ("ls_uv", C.c_ssize_t)]
+
+
+class Vp8McOp(C.Structure):
+    """B200Vp8McOp (include/b200dsp.h), 24 bytes"""
+    _fields_ = [("src_x", C.c_int32), ("src_y", C.c_int32), ("dst_x", C.c_int32), ("dst_y", C.c_int32), ("plane", C.c_uint8), ("w", C.c_uint8),
+                ("h", C.c_uint8), ("ref", C.c_uint8), ("mx", C.c_uint8), ("my", C.c_uint8), ("reserved", C.c_uint8 * 2)]
+
+
+class Vp8ResidualOp(C.Structure):
+    """B200Vp8ResidualOp (include/b200dsp.h), 48 bytes"""
+    _fields_ = [("coef_off", C.c_int64), ("mb_x", C.c_int32), ("mb_y", C.c_int32), ("nnz", C.c_uint8 * 4 * 6), ("y2_nnz", C.c_uint8),
+                ("flags", C.c_uint8), ("reserved", C.c_uint8 * 6)]
+
+
 class ProresDSPContext(C.Structure):
     """libavcodec/proresdsp.h:28-35"""
     _fields_ = [("idct_permutation_type", C.c_int), ("idct_permutation", C.c_uint8 * 64),
@@ -388,6 +418,9 @@ PROTOTYPES = {
     "b200_vp9_intra_recon_frame_device": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_ssize_t, C.c_ssize_t, C.c_int64,
                                                     vp, vp]),
     "b200_vp9_intra_timeouts": (C.c_int, [vp, vp]),
+    "b200_vp8_dsp_init": (C.c_int, [vp, C.c_int]),
+    "b200_vp8_mc_frame_device": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_int64, vp, vp, C.c_ssize_t, C.c_ssize_t]),
+    "b200_vp8_residual_frame_device": (C.c_int, [vp, C.c_int, C.c_int64, vp, vp, vp, C.c_ssize_t, C.c_ssize_t]),
     "b200_proresdsp_init": (C.c_int, [vp, C.c_int]),
     "b200_prores_idct_put_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, vp, vp, vp, C.c_int]),
     "b200_float_dsp_init": (C.c_int, [vp]),

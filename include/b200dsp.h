@@ -943,6 +943,124 @@ int  b200_vp9_intra_recon_frame_device(B200Device *dev, int bit_depth, int ss_h,
  * b200_vp9_loopfilter_timeouts).  0; B200_EINVAL for count == NULL; B200_ENODEV; B200_EEXTERNAL. */
 int  b200_vp9_intra_timeouts(B200Device *dev, int64_t *count);
 
+/* VP8 / VP7 motion compensation and residual: VP8DSPContext (libavcodec/vp8dsp.h:37-82) in the reference's member order and types.
+ * b200_vp8_dsp_init() fills what ff_vp78dsp_init and ff_vp8dsp_init (is_vp7 = 0) / ff_vp7dsp_init (is_vp7 = 1) fill (vp8dsp.c:663-760)
+ * except the ten loop-filter members, which stay NULL:
+ *   vp8_luma_dc_wht, _wht_dc, vp8_idct_add, _dc_add, _dc_add4y, _dc_add4uv   the VP8 or the VP7 arithmetic
+ *   put_vp8_epel_pixels_tab[size][v][h]       size 0..2 = 16, 8, 4 columns; v / h: 0 none, 1 4-tap, 2 6-tap; [0][1][*] and [0][*][1]
+ *                                             NULL, as in the reference
+ *   put_vp8_bilinear_pixels_tab[size][v][h]   v / h: 0 none, 1 and 2 bilinear
+ * Shared as in the reference: [i][0][0] is one function in both tables; in the bilinear table [i][0][1] / [i][0][2] are one function,
+ * [i][1][0] / [i][2][0] are one, and the four 2-D positions are one.  HOST pointers, the reference's signatures; MC source and
+ * destination are uint8, strides in bytes.
+ *   6-tap     clip((F0 s[-2] - F1 s[-1] + F2 s[0] + F3 s[1] - F4 s[2] + F5 s[3] + 64) >> 7), F = subpel_filters[phase - 1] (vp8dsp.c:459-490)
+ *   4-tap     clip((- F1 s[-1] + F2 s[0] + F3 s[1] - F4 s[2] + 64) >> 7) of the same row, whatever the phase's parity
+ *   bilinear  ((8 - m) s[0] + m s[1] + 4) >> 3
+ *   2-D       the horizontal pass, clipped to uint8, over rows -2 .. h + 2 (6-tap vertical) or -1 .. h + 1 (4-tap) / 0 .. h (bilinear),
+ *             then the vertical pass over it
+ * A member reads exactly the samples its reference function reads.  It writes nothing and records the reason (b200_last_error()) for h
+ * outside 1 .. 2 * width (the reference's tmp_array), a phase above 7, or an epel member handed phase 0 in a direction it filters (the
+ * reference indexes subpel_filters[-1] there).
+ *   wht        VP8: column pass into int16 dc[], then (x + 3) >> 3 into block[i][j][0] (vp8dsp.c:152-180); VP7: row pass with the
+ *              products in unsigned, (int) >> 14 into int16, then the column pass (+ 0x20000) >> 18 (:56-84); clears dc[0..15]
+ *   wht_dc     VP8 (dc[0] + 3) >> 3, VP7 (23170 * (23170 * dc[0] >> 14) + 0x20000) >> 18 into all 16 block[i][j][0]; clears dc[0]
+ *   idct_add   VP8: column pass with MUL_20091 / MUL_35468 into int16, row pass (+ 4) >> 3 added and clipped (:195-231); VP7 as wht with
+ *              the add (:99-131); clears block[0..15]
+ *   dc_add     VP8 (block[0] + 4) >> 3, VP7 as wht_dc, added to the 4x4 block; reads and clears block[0] only
+ *   dc_add4y   dc_add on the four blocks at dst + 0, 4, 8, 12;  dc_add4uv: at dst, dst + 4, dst + 4 stride, dst + 4 stride + 4
+ * 0; B200_EINVAL for c == NULL or is_vp7 not 0 / 1; B200_ENODEV. */
+typedef void (*b200_vp8_mc_func)(uint8_t *dst, ptrdiff_t dst_stride, const uint8_t *src, ptrdiff_t src_stride, int h, int mx, int my);
+typedef struct B200VP8DSPContext {
+    void (*vp8_luma_dc_wht)(int16_t block[4][4][16], int16_t dc[16]);
+    void (*vp8_luma_dc_wht_dc)(int16_t block[4][4][16], int16_t dc[16]);
+    void (*vp8_idct_add)(uint8_t *dst, int16_t block[16], ptrdiff_t stride);
+    void (*vp8_idct_dc_add)(uint8_t *dst, int16_t block[16], ptrdiff_t stride);
+    void (*vp8_idct_dc_add4y)(uint8_t *dst, int16_t block[4][16], ptrdiff_t stride);
+    void (*vp8_idct_dc_add4uv)(uint8_t *dst, int16_t block[4][16], ptrdiff_t stride);
+    void (*vp8_v_loop_filter16y)(uint8_t *dst, ptrdiff_t stride, int flim_E, int flim_I, int hev_thresh);
+    void (*vp8_h_loop_filter16y)(uint8_t *dst, ptrdiff_t stride, int flim_E, int flim_I, int hev_thresh);
+    void (*vp8_v_loop_filter8uv)(uint8_t *dstU, uint8_t *dstV, ptrdiff_t stride, int flim_E, int flim_I, int hev_thresh);
+    void (*vp8_h_loop_filter8uv)(uint8_t *dstU, uint8_t *dstV, ptrdiff_t stride, int flim_E, int flim_I, int hev_thresh);
+    void (*vp8_v_loop_filter16y_inner)(uint8_t *dst, ptrdiff_t stride, int flim_E, int flim_I, int hev_thresh);
+    void (*vp8_h_loop_filter16y_inner)(uint8_t *dst, ptrdiff_t stride, int flim_E, int flim_I, int hev_thresh);
+    void (*vp8_v_loop_filter8uv_inner)(uint8_t *dstU, uint8_t *dstV, ptrdiff_t stride, int flim_E, int flim_I, int hev_thresh);
+    void (*vp8_h_loop_filter8uv_inner)(uint8_t *dstU, uint8_t *dstV, ptrdiff_t stride, int flim_E, int flim_I, int hev_thresh);
+    void (*vp8_v_loop_filter_simple)(uint8_t *dst, ptrdiff_t stride, int flim);
+    void (*vp8_h_loop_filter_simple)(uint8_t *dst, ptrdiff_t stride, int flim);
+    b200_vp8_mc_func put_vp8_epel_pixels_tab[3][3][3];
+    b200_vp8_mc_func put_vp8_bilinear_pixels_tab[3][3][3];
+} B200VP8DSPContext;
+int  b200_vp8_dsp_init(B200VP8DSPContext *c, int is_vp7);
+
+/* One reference frame of b200_vp8_mc_frame_device: DEVICE addresses of sample (0, 0) of its three planes, line sizes in bytes. */
+typedef struct B200Vp8McRef {
+    const uint8_t *y, *u, *v;
+    ptrdiff_t ls_y, ls_uv;
+} B200Vp8McRef;
+/* One inter block of b200_vp8_mc_frame_device.  plane LUMA writes a w x h block of Y at (dst_x, dst_y); CHROMA writes the same block
+ * of U and of V, as vp8_mc_chroma does.  (src_x, src_y) is the integer source position and mx / my the eighth-sample phase (0..7), as
+ * the decoder has them after its motion-vector arithmetic: x_off + (mv >> 2) with phase (mv * 2) & 7 for luma, x_off + (mv >> 3) with
+ * mv & 7 for chroma (vp8.c:1844-1848, :1900-1904).  Split-MV chroma averaging, profile-3 full-pel chroma and MV clamping stay with the
+ * caller. */
+enum { B200_VP8_MC_LUMA = 0, B200_VP8_MC_CHROMA = 1 };
+typedef struct B200Vp8McOp {
+    int32_t src_x, src_y;   /* any value */
+    int32_t dst_x, dst_y;   /* top-left sample of the block in its plane; dst_x a multiple of 4 */
+    uint8_t plane;          /* B200_VP8_MC_LUMA / B200_VP8_MC_CHROMA */
+    uint8_t w, h;           /* w 16, 8 or 4; h 1..16 */
+    uint8_t ref;            /* index into the call's refs */
+    uint8_t mx, my;         /* 0..7 */
+    uint8_t reserved[2];
+} B200Vp8McOp;
+#ifdef __cplusplus
+static_assert(sizeof(B200Vp8McOp) == 24, "B200Vp8McOp is 24 bytes");
+#else
+_Static_assert(sizeof(B200Vp8McOp) == 24, "B200Vp8McOp is 24 bytes");
+#endif
+/* Inter prediction of a whole VP8 / VP7 frame in one call: `refs` is a HOST array of 1 <= nrefs <= 3 frames (copied into the launch),
+ * `ops` and the dst[0..2] planes are DEVICE pointers; asynchronous on the device's stream.  bilinear selects
+ * put_vp8_bilinear_pixels_tab, else put_vp8_epel_pixels_tab (the decoder's put_pixels_tab: epel for VP7 and for VP8 profile 0,
+ * vp8.c:601, :757-762).  Each op's result is put_pixels_tab[size of w][subpel_idx[0][my]][subpel_idx[0][mx]] (odd phase 4-tap, even
+ * non-zero phase 6-tap, vp8.c:1809-1814), its source samples read through coordinates clamped to the plane: 16 mb_width x 16 mb_height
+ * for luma, 8 mb_width x 8 mb_height for chroma.  That is what the decoder's emulated_edge_mc windows give, and where the decoder does
+ * not emulate its own test (vp8.c:1853-1854, :1910-1911) keeps every read inside the plane, so no edge emulation pass is needed.
+ * The caller guarantees that the ops of one call write disjoint blocks and that no op reads what another op of the call writes.
+ * An op writes nothing if its plane class or width is undefined, h is outside 1..16, a phase is above 7, ref >= nrefs, it is a
+ * 16-wide epel op with an odd phase (the reference table is NULL there), dst_x is not a multiple of 4, or its block is not inside the
+ * plane.  Offsets are 64-bit; more ops than one launch takes are split inside the entry.
+ * Returns 0, or B200_EINVAL (launching nothing) for NULL pointers, nops < 0, nrefs outside 1..3, mb_width or mb_height outside
+ * 1..65536, ops not aligned to 4 bytes, or a dst plane or line size that is not a multiple of 4; nops == 0 returns 0. */
+int  b200_vp8_mc_frame_device(B200Device *dev, int bilinear, int mb_width, int mb_height, int nrefs, const B200Vp8McRef *refs, int64_t nops,
+                              const B200Vp8McOp *ops, uint8_t *const dst[3], ptrdiff_t ls_y, ptrdiff_t ls_uv);
+
+/* One macroblock of b200_vp8_residual_frame_device: the state decode_mb_coeffs leaves for idct_mb (vp8.c:1493-1566, :2085-2146). */
+enum { B200_VP8_RESIDUAL_LUMA = 1 };    /* flags: the luma residual is present (mode != MODE_I4x4) */
+typedef struct B200Vp8ResidualOp {
+    int64_t coef_off;       /* element offset in coef of the MB's 400 int16: td->block[6][4][16], then block_dc[16]; a multiple of 8 */
+    int32_t mb_x, mb_y;     /* >= 0 */
+    uint8_t nnz[6][4];      /* td->non_zero_count_cache */
+    uint8_t y2_nnz;         /* 0 none, 1 vp8_luma_dc_wht_dc, > 1 vp8_luma_dc_wht */
+    uint8_t flags;          /* B200_VP8_RESIDUAL_* */
+    uint8_t reserved[6];
+} B200Vp8ResidualOp;
+#ifdef __cplusplus
+static_assert(sizeof(B200Vp8ResidualOp) == 48, "B200Vp8ResidualOp is 48 bytes");
+#else
+_Static_assert(sizeof(B200Vp8ResidualOp) == 48, "B200Vp8ResidualOp is 48 bytes");
+#endif
+/* The residual of every macroblock of a VP8 / VP7 frame in one call, DEVICE pointers (ops, coef, dst[0..2]), asynchronous on the
+ * device's stream.  Per op: with y2_nnz > 0 the WHT (or WHT_DC) of block_dc replaces coefficient 0 of the 16 luma blocks, then idct_mb
+ * with idct_mb's own decisions: in a luma row (and a chroma plane) whose four nnz bytes are all <= 1 and not all 0, dc_add4y (dc_add4uv)
+ * adds the DC of all four blocks, nnz-0 blocks included; otherwise each block alone: nnz 1 dc_add (reads coefficient 0 only), nnz > 1
+ * idct_add, 0 nothing.  Luma only with B200_VP8_RESIDUAL_LUMA.  is_vp7 selects the VP7 arithmetic.  Every int16 value is accepted.
+ * `coef` is read only: clearing it stays with the decoder.  The ops of one call write disjoint macroblocks.  An op with a negative
+ * mb_x / mb_y or coef_off, or coef_off not a multiple of 8, writes nothing.  Offsets are 64-bit; more ops than one launch takes are
+ * split inside the entry.
+ * Returns 0, or B200_EINVAL (launching nothing) for NULL pointers, nops < 0, is_vp7 not 0 / 1, ops not aligned to 8 bytes, coef not
+ * aligned to 16 bytes, or a dst plane or line size that is not a multiple of 4; nops == 0 returns 0. */
+int  b200_vp8_residual_frame_device(B200Device *dev, int is_vp7, int64_t nops, const B200Vp8ResidualOp *ops, const int16_t *coef,
+                                    uint8_t *const dst[3], ptrdiff_t ls_y, ptrdiff_t ls_uv);
+
 /* mpegvideo inverse quantisers: the members of MPVUnquantDSPContext (libavcodec/mpegvideo_unquantize.h:31-44) as
  * ff_mpv_unquantize_init() installs them (libavcodec/mpegvideo_unquantize.c:50-290), i.e. what runs in front of the IDCT in
  * mpv_reconstruct_mb's put_dct / add_dequant_dct (libavcodec/mpegvideo_dec.c).  The reference functions take the whole

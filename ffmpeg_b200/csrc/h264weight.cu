@@ -166,6 +166,7 @@ B200_API int b200_h264_weight_hbd_batch_device(B200Device *dev, int bit_depth, i
     if (!dev || n < 0 || !params || !dst || !dst_off || (src && !src_off)) return B200_EINVAL;
     if (bit_depth != 9 && bit_depth != 10 && bit_depth != 12 && bit_depth != 14) return B200_ENOSYS;
     if ((stride & 1) || ((reinterpret_cast<uintptr_t>(dst) | reinterpret_cast<uintptr_t>(src)) & 1)) return B200_EINVAL;
+    if ((uintptr_t)params & 3) return B200_EINVAL;                     // the kernel reads params as int32
     if (n == 0) return 0;
     B200_CUDA_OK(cudaSetDevice(dev->ordinal));
     return launch(dev->stream, bit_depth, n, params, dst, dst_off, src, src_off, (long long)stride);

@@ -41,7 +41,8 @@ struct HbWin {
     }
 };
 
-// op byte as in b200_h264qpel_batch_device: bit0 avg, bits1-2 size index, bits3-6 position x + 4 y; offsets and stride in BYTES.
+// op byte as in b200_h264qpel_batch_device: bit0 avg, bits1-2 size index (3 writes nothing), bits3-6 position x + 4 y; offsets and
+// stride in BYTES.
 // A warp per operation, a lane per pixel (size^2 / 32 rounds); the taps come straight from the reference picture (the window of a
 // block stays in L1 for its 8 rounds): no shared memory, no synchronisation, every thread is independent.
 // (tests/test_cuda_emu.py runs this whole file, host code included, on the CPU against the checker)
@@ -52,7 +53,9 @@ qpel_hbd_kernel(long long n, const uint8_t *__restrict__ op, uint8_t *dst, const
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long st = stride / 2;
     for (long long i = (long long)blockIdx.x * HB_WARPS + warp; i < n; i += (long long)gridDim.x * HB_WARPS) {
-        const int o = op[i], avg = o & 1, ls = 4 - ((o >> 1) & 3), size = 1 << ls, qx = (o >> 3) & 3, qy = (o >> 5) & 3;
+        const int o = op[i];
+        if (((o >> 1) & 3) == 3) continue;                         // size index 3: a NULL entry of the reference's table, writes nothing
+        const int avg = o & 1, ls = 4 - ((o >> 1) & 3), size = 1 << ls, qx = (o >> 3) & 3, qy = (o >> 5) & 3;
         unsigned short *dp = reinterpret_cast<unsigned short *>(dst + dst_off[i]);
         const HbWin W{ reinterpret_cast<const unsigned short *>(src + src_off[i]), st, (1 << depth) - 1 };
         for (int p = lane; p < size * size; p += 32) {
@@ -85,7 +88,7 @@ int hbd_launch(cudaStream_t st, int depth, long long n, const uint8_t *op, uint8
 // h264chroma for 16-bit samples (h264chroma_template.c:27-176 with BIT_DEPTH 16, what ff_h264chroma_init installs for every depth above 8,
 // h264chroma.c:45-50): bilinear eighth-pel (A p00 + B p01 + C p10 + D p11 + 32) >> 6 with A = (8-x)(8-y), B = x(8-y), C = (8-x)y, D = xy;
 // like the reference the D == 0 / B + C == 0 forms do not read the unused row / column.  op byte: bit0 avg, bits1-2 width index
-// (0: 8, 1: 4, 2: 2); h[i] rows; xy[i] = x | y << 3; offsets and stride in BYTES.  A warp per block, a lane per pixel.
+// (0: 8, 1: 4, 2: 2; 3 writes nothing); h[i] rows; xy[i] = x | y << 3; offsets and stride in BYTES.  A warp per block, a lane per pixel.
 __global__ void __launch_bounds__(32 * HB_WARPS)
 chroma_hbd_kernel(long long n, const uint8_t *__restrict__ op, const uint8_t *__restrict__ hh, const uint8_t *__restrict__ xy, uint8_t *dst,
                   const long long *__restrict__ dst_off, const uint8_t *src, const long long *__restrict__ src_off, long long stride)
@@ -93,7 +96,9 @@ chroma_hbd_kernel(long long n, const uint8_t *__restrict__ op, const uint8_t *__
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long st = stride / 2;
     for (long long i = (long long)blockIdx.x * HB_WARPS + warp; i < n; i += (long long)gridDim.x * HB_WARPS) {
-        const int o = op[i], avg = o & 1, lw = 3 - ((o >> 1) & 3), w = 1 << lw, h = hh[i], x = xy[i] & 7, y = (xy[i] >> 3) & 7;
+        const int o = op[i];
+        if (((o >> 1) & 3) == 3) continue;                         // width index 3: the reference's NULL entry, writes nothing
+        const int avg = o & 1, lw = 3 - ((o >> 1) & 3), w = 1 << lw, h = hh[i], x = xy[i] & 7, y = (xy[i] >> 3) & 7;
         const int A = (8 - x) * (8 - y), B = x * (8 - y), C = (8 - x) * y, D = x * y, E = B + C;
         const unsigned short *sp = reinterpret_cast<const unsigned short *>(src + src_off[i]);
         unsigned short *dp = reinterpret_cast<unsigned short *>(dst + dst_off[i]);

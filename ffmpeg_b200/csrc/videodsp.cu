@@ -119,6 +119,7 @@ B200_API int b200_emulated_edge_mc_hbd_batch_device(B200Device *dev, int64_t n, 
 {
     if (!dev || n < 0 || !buf || !buf_off || !src || !origin || !geom || w < 0 || h < 0) return B200_EINVAL;
     if (((buf_linesize | src_linesize) & 1) || ((reinterpret_cast<uintptr_t>(buf) | reinterpret_cast<uintptr_t>(src)) & 1)) return B200_EINVAL;
+    if ((uintptr_t)geom & 3) return B200_EINVAL;                   // the kernel reads geom as int32
     if (n == 0 || !w || !h) return 0;
     B200_CUDA_OK(cudaSetDevice(dev->ordinal));
     return launch<uint16_t>(dev->stream, n, buf, buf_off, buf_linesize, src, origin, src_linesize, geom, w, h);

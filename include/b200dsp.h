@@ -1181,7 +1181,8 @@ int  b200_h264_weight_init(B200H264WeightContext *c, int bit_depth);            
  * Destination blocks of one call must not overlap each other, and no op may read samples that another op of the same call writes. */
 int  b200_h264_weight_batch_device(B200Device *dev, int64_t n, const int32_t *params, uint8_t *dst, const int64_t *dst_off,
                                    const uint8_t *src, const int64_t *src_off, ptrdiff_t stride);
-/* the same for 9 / 10 / 12 / 14 bit samples (uint16): offsets and stride in BYTES (even) */
+/* the same for 9 / 10 / 12 / 14 bit samples (uint16): offsets and stride in BYTES (even); params must be 4-byte aligned (B200_EINVAL
+ * otherwise) */
 int  b200_h264_weight_hbd_batch_device(B200Device *dev, int bit_depth, int64_t n, const int32_t *params, uint8_t *dst, const int64_t *dst_off,
                                        const uint8_t *src, const int64_t *src_off, ptrdiff_t stride);
 
@@ -1308,7 +1309,8 @@ int  b200_hpeldsp_init(B200HpelDSPContext *c, int flags);
  * result): keep the planes edge-padded by 3 pixels / rows, as H.264 reference frames are (h264_mb.c mc_dir_part). */
 int  b200_h264qpel_batch_device(B200Device *dev, int64_t n, const uint8_t *op, uint8_t *dst, const int64_t *dst_off,
                                 const uint8_t *src, const int64_t *src_off, ptrdiff_t stride);
-/* the same for 9 / 10 / 12 / 14 bit samples (uint16, native endian): op bytes as above, offsets and stride in BYTES (even) */
+/* the same for 9 / 10 / 12 / 14 bit samples (uint16, native endian): op bytes as above (size index 3 writes nothing), offsets and stride
+ * in BYTES (even) */
 int  b200_h264qpel_hbd_batch_device(B200Device *dev, int bit_depth, int64_t n, const uint8_t *op, uint8_t *dst, const int64_t *dst_off,
                                     const uint8_t *src, const int64_t *src_off, ptrdiff_t stride);
 int  b200_hpel_batch_device(B200Device *dev, int64_t n, const uint8_t *op, const uint8_t *h, uint8_t *dst,
@@ -1336,7 +1338,7 @@ int  b200_h264chroma_init(B200H264ChromaContext *c, int bit_depth);   /* 9 ... 1
 int  b200_h264chroma_batch_device(B200Device *dev, int64_t n, const uint8_t *op, const uint8_t *h, const uint8_t *xy,
                                   uint8_t *dst, const int64_t *dst_off, const uint8_t *src, const int64_t *src_off,
                                   ptrdiff_t stride);
-/* the same for 16-bit samples (any depth above 8): offsets and stride in BYTES (even) */
+/* the same for 16-bit samples (any depth above 8): op bytes as above (width index 3 writes nothing), offsets and stride in BYTES (even) */
 int  b200_h264chroma_hbd_batch_device(B200Device *dev, int64_t n, const uint8_t *op, const uint8_t *h, const uint8_t *xy,
                                       uint8_t *dst, const int64_t *dst_off, const uint8_t *src, const int64_t *src_off,
                                       ptrdiff_t stride);
@@ -1358,7 +1360,8 @@ int  b200_videodsp_init(B200VideoDSPContext *c, int bpc);             /* bpc <= 
 int  b200_emulated_edge_mc_batch_device(B200Device *dev, int64_t n, uint8_t *buf, const int64_t *buf_off,
                                         ptrdiff_t buf_linesize, const uint8_t *src, const int64_t *origin,
                                         ptrdiff_t src_linesize, const int32_t *geom, int w, int h);
-/* the same for 16-bit samples: geom in pixels; buf_off, origin and the line sizes in BYTES (even) */
+/* the same for 16-bit samples: geom in pixels; buf_off, origin and the line sizes in BYTES (even); geom must be 4-byte aligned
+ * (B200_EINVAL otherwise) */
 int  b200_emulated_edge_mc_hbd_batch_device(B200Device *dev, int64_t n, uint8_t *buf, const int64_t *buf_off,
                                             ptrdiff_t buf_linesize, const uint8_t *src, const int64_t *origin,
                                             ptrdiff_t src_linesize, const int32_t *geom, int w, int h);

@@ -386,80 +386,94 @@ def esa_expected(lib_fn, row, curbuf, refbuf, workers=None):
     return mv, cost
 
 
-# ---------------------------------------------------------------- 8-bit motion compensation (csrc/pel.cu, csrc/h264weight.cu)
-# Plane layouts of tests/test_pel_paths_gpu.py and tests/test_oracle_pel_layouts.py.  A case's source and destination pictures have
-# the same width and share one stride, like a decoder's reference and current pictures.  Each plane has an allocation of its own with
-# PEL_SLACK bytes before its first and after its last sample: the kernels load the aligned 16-byte (qpel) or 8-byte (chroma) words
-# around the bytes they need, so those words stay inside the allocation whatever the alignment of the base.
-#   A  stride a multiple of 64, plane bases 64-byte aligned, block offsets as a decoder makes them (x a multiple of the block width)
-#   B  odd stride (width + 37 or + 38): the rows of one block all have different alignments; source base at +3, destination base at
-#      +10, destination x jittered by 0..15, so that 8- and 16-wide qpel blocks take both the 8-byte and the byte store path
+# ---------------------------------------------------------------- motion compensation (csrc/pel.cu, csrc/pel_hbd.cu, csrc/h264weight.cu)
+# Plane layouts of tests/test_pel_paths_gpu.py, tests/test_h264_hbd_paths_gpu.py and the checkers' pins on the reference.  A case's source
+# and destination pictures have the same width and share one stride, like a decoder's reference and current pictures.  Each plane has an
+# allocation of its own with PEL_SLACK bytes before its first and after its last sample: the kernels load the aligned 16-byte (qpel) or
+# 8-byte (chroma) words around the bytes they need, so those words stay inside the allocation whatever the alignment of the base.
+# Samples are bytes (bps = 1) or native-endian uint16 (bps = 2, depths 9 to 14); strides and offsets count bytes either way.
+#   A  stride a multiple of 64 bytes (128 at bps 2), plane bases 64-byte aligned, block offsets as a decoder makes them (x a multiple of
+#      the block width)
+#   B  stride an odd number of samples (width + 37 or + 38): the rows of one block all have different alignments (at bps 2 they cycle
+#      through 2, 4, 8 and 16 bytes); source base at +3 bytes (+2 at bps 2), destination base at +10, destination x jittered by 0..15
+#      samples, so that 8- and 16-wide blocks take both the word and the sample store paths
 #   C  the picture of A stored bottom-up: negative stride, the base (picture row 0) is the last row in memory and the offsets
-#      y * stride + x are negative
+#      y * stride + x * bps are negative
 PEL_SLACK = 64
 PEL_LAYOUTS = ("A", "B", "C")
 
 
 class PelPlane:
     """One w x h picture in a layout.  buf: the whole allocation (uint8, seeded noise outside the picture); base: offset of sample
-    (0, 0) in buf; stride: bytes from one picture row to the next (negative in layout C).  Offsets handed to the kernels are relative
-    to base: off(x, y) = y * stride + x."""
+    (0, 0) in buf; stride: bytes from one picture row to the next (negative in layout C); bps: bytes per sample (1, or 2 for uint16
+    samples).  Offsets handed to the kernels are relative to base: off(x, y) = y * stride + x * bps.  `pitch` / `mis` (bytes) replace
+    the layout's row pitch / base misalignment."""
 
-    def __init__(self, layout, w, h, role, seed):
+    def __init__(self, layout, w, h, role, seed, bps=1, pitch=None, mis=None):
         if layout == "B":
-            pitch, mis = (w + 37 if (w + 37) % 2 else w + 38), (3 if role == "src" else 10)
+            lp, lm = (w + 37 if (w + 37) % 2 else w + 38) * bps, ((3 if bps == 1 else 2) if role == "src" else 10)
         else:
-            pitch, mis = (w + 63) // 64 * 64, 0
-        self.layout, self.w, self.h = layout, w, h
+            lp, lm = (w * bps + 64 * bps - 1) // (64 * bps) * 64 * bps, 0
+        pitch, mis = lp if pitch is None else pitch, lm if mis is None else mis
+        self.layout, self.w, self.h, self.bps = layout, w, h, bps
+        self.dtype = np.uint8 if bps == 1 else np.uint16
         self.stride = -pitch if layout == "C" else pitch
         self.base = PEL_SLACK + mis + ((h - 1) * pitch if layout == "C" else 0)
-        size = PEL_SLACK + mis + (h - 1) * pitch + w + PEL_SLACK
+        size = PEL_SLACK + mis + (h - 1) * pitch + w * bps + PEL_SLACK
         self.buf = np.random.default_rng(seed).integers(0, 256, (size + 15) // 16 * 16, dtype=np.uint8)
 
     def off(self, x, y):
-        return y * self.stride + x
+        return y * self.stride + x * self.bps
+
+    def row(self, buf, y):
+        """picture row y of the allocation `buf` (a copy of self.buf), as samples"""
+        o = self.base + y * self.stride
+        return buf[o:o + self.w * self.bps].view(self.dtype)
 
     def fill(self, pic):
         for y in range(self.h):
-            o = self.base + y * self.stride
-            self.buf[o:o + self.w] = pic[y]
+            self.row(self.buf, y)[:] = pic[y]
         return self
 
     def picture(self):
-        return np.stack([self.buf[self.base + y * self.stride:][:self.w] for y in range(self.h)])
+        return np.stack([self.row(self.buf, y).copy() for y in range(self.h)])
 
 
-def pel_picture(kind, h, w, seed):
-    """'random', or 'extremes': 0 / 255 patterns in 24 x 24 tiles, cycling through vertical and horizontal stripes of periods 2, 3
-    and 6, a checkerboard, flat 0 and flat 255 -- they drive the 6-tap sums, the centre sample and the weighted sums to both clip
-    limits"""
+def pel_picture(kind, h, w, seed, depth=8):
+    """'random', or 'extremes': 0 / max patterns in 24 x 24 tiles, cycling through vertical and horizontal stripes of periods 2, 3
+    and 6, a checkerboard, flat 0 and flat max -- they drive the 6-tap sums, the centre sample and the weighted sums to both clip
+    limits.  max = (1 << depth) - 1; uint8 samples at depth 8, uint16 above."""
+    dt, mx = (np.uint8, 255) if depth == 8 else (np.uint16, (1 << depth) - 1)
     if kind == "random":
-        return np.random.default_rng(seed).integers(0, 256, (h, w), dtype=np.uint8)
+        return np.random.default_rng(seed).integers(0, mx + 1, (h, w), dtype=dt)
     yy, xx = np.mgrid[0:h, 0:w]
     pats = [xx % p < p // 2 for p in (2, 3, 6)] + [yy % p < p // 2 for p in (2, 3, 6)] + [(xx + yy) % 2 == 0, xx < 0, xx >= 0]
     tile = ((yy // 24) * 5 + xx // 24 + seed) % len(pats)
-    return (np.select([tile == i for i in range(len(pats))], pats) * 255).astype(np.uint8)
+    return (np.select([tile == i for i in range(len(pats))], pats) * mx).astype(dt)
 
 
-def pel_layout_case(layout, kind, blocks, seed, src_h=96, margin=(0, 0), cell=(16, 16), phases=None, cols=64):
+def pel_layout_case(layout, kind, blocks, seed, src_h=96, margin=(0, 0), cell=(16, 16), phases=None, cols=64, depth=8):
     """Source and destination planes and per-op offsets for a list of (block width, block height).  Op i reads its block at a seeded
     position of the source picture, `margin` = (samples before, samples after) it may read around the block staying inside the
-    picture; with `phases`, the address of its sample (0, 0) is phases[i] mod 16.  It writes a block of its own cell
-    (cell = (width, height)) of the destination picture, `cols` cells per row, at an x jitter the layout allows.
+    picture; with `phases`, the address of its sample (0, 0) is phases[i] mod 16 (bytes; even above depth 8).  It writes a block of
+    its own cell (cell = (width, height)) of the destination picture, `cols` cells per row, at an x jitter the layout allows.
+    depth 8: uint8 samples; 9 to 14: uint16 samples, offsets still in bytes.
     Returns dict(src=PelPlane, dst=PelPlane, soff=int64[n], doff=int64[n])."""
     rng = np.random.default_rng(seed)
+    bps = 1 if depth == 8 else 2
     n = len(blocks)
     bw, bh = (np.array([b[k] for b in blocks], np.int64).reshape(n) for k in (0, 1))
     cw, ch = cell
     w = cols * cw
     rows = max(1, (n + cols - 1) // cols)
-    src = PelPlane(layout, w, src_h, "src", seed + 1).fill(pel_picture(kind, src_h, w, seed + 2))
-    dst = PelPlane(layout, w, rows * ch, "dst", seed + 3).fill(pel_picture("random", rows * ch, w, seed + 4))
+    src = PelPlane(layout, w, src_h, "src", seed + 1, bps).fill(pel_picture(kind, src_h, w, seed + 2, depth))
+    dst = PelPlane(layout, w, rows * ch, "dst", seed + 3, bps).fill(pel_picture("random", rows * ch, w, seed + 4, depth))
     lo, hi = margin
     sy = rng.integers(lo, src_h - bh - hi + 1)
     sx = rng.integers(lo, w - bw - hi - 15 + 1)
     if phases is not None:
-        sx = sx + (np.asarray(phases, np.int64) - (src.base + src.off(sx, sy))) % 16
+        assert bps == 1 or not (np.asarray(phases) % 2).any(), "uint16 samples sit at even byte phases"
+        sx = sx + (np.asarray(phases, np.int64) - (src.base + src.off(sx, sy))) % 16 // bps
     if layout == "B":
         jx = rng.integers(0, np.minimum(15, cw - bw) + 1)
     else:

@@ -683,6 +683,75 @@ def h264lf_case(seed, n, cols=16):
     return pic, kinds, off.astype(np.int64), alpha, beta, tc0
 
 
+LF_SHAPES = [(0, 0, 1, 4), (0, 0, 0, 4), (0, 0, 0, 2), (1, 0, 1, 4), (1, 0, 0, 4), (1, 0, 0, 2), (0, 1, 1, 2), (0, 1, 0, 2), (0, 1, 0, 1),
+             (1, 1, 1, 2), (1, 1, 0, 2), (1, 1, 0, 1), (0, 1, 0, 4), (0, 1, 0, 2), (1, 1, 0, 4), (1, 1, 0, 2)]   # kind -> intra, chroma, vert, lines / 4
+# what one line of a threshold case puts at a threshold: "a" |p0 - q0| vs alpha, "b1" |p1 - p0|, "b2" |q1 - q0|, "b3" |p2 - p0|, "b4" |q2 - q0|
+# vs beta, "ai" |p0 - q0| vs (alpha >> 2) + 2 (luma intra), each at threshold - 1 and at threshold; "clip" lines put p0 and q0 at 0 or the
+# maximum with p1 or q1 beta - 1 inside, so that p0 + delta or q0 - delta leaves the sample range
+LF_LINE_MODES = [(t, s) for t in ("a", "b1", "b2", "b3", "b4", "ai") for s in (0, 1)] + [("clip", 0), ("clip", 1)]
+
+
+def h264lf_threshold_case(seed, n, depth, cols=16):
+    """(pic [rows*32, cols*32] uint8 at depth 8 / uint16 above, kinds, off (bytes), alpha, beta, tc0) in h264lf_case's layout, each line
+    across each edge built from the edge's alpha and beta after the depth scaling so that one comparison of the filters' decisions lands
+    exactly on one side of its strict '<' (LF_LINE_MODES, cycling over the lines and edges) and every other comparison passes.  Edge e is
+    of kind e % 16; alpha cycles through 0, 1, 255 and a random value every 16 edges, beta through 0, 1, 18 and a random value every 64;
+    the tc0 entries of half the edges are -1, 0, 1 and 25 in rotation, of the other half random in -1..25.  A line's samples are shifted
+    to 0 or the maximum one time in three."""
+    rng = np.random.default_rng(seed)
+    sh, mx = depth - 8, (1 << depth) - 1
+    dt = np.uint8 if depth == 8 else np.uint16
+    rows = (n + cols - 1) // cols
+    pic = rng.integers(0, mx + 1, (rows * LF_CELL, cols * LF_CELL)).astype(dt)
+    e = np.arange(n)
+    kinds = (e % 16).astype(np.uint8)
+    alpha = np.where(e // 16 % 4 < 3, np.array([0, 1, 255])[np.minimum(e // 16 % 4, 2)], rng.integers(2, 255, n)).astype(np.uint8)
+    beta = np.where(e // 64 % 4 < 3, np.array([0, 1, 18])[np.minimum(e // 64 % 4, 2)], rng.integers(2, 18, n)).astype(np.uint8)
+    tc0 = np.where((e // 256 % 2 == 0)[:, None], np.array([-1, 0, 1, 25])[(np.arange(4)[None, :] + e[:, None]) % 4],
+                   rng.integers(-1, 26, (n, 4))).astype(np.int8)
+    k = 0
+    for i in range(n):
+        intra, chroma, vert, iters = LF_SHAPES[kinds[i]]
+        A, B = int(alpha[i]) << sh, int(beta[i]) << sh
+        thr = {"a": A, "ai": (A >> 2) + 2, "b1": B, "b2": B, "b3": B, "b4": B}
+        y0, x0 = (i // cols) * LF_CELL + 8, (i % cols) * LF_CELL + 8
+        for line in range(4 * iters):
+            mode, side = LF_LINE_MODES[k % len(LF_LINE_MODES)]
+            k += 1
+            ok = lambda t: int(rng.integers(0, thr[t])) if thr[t] > 0 else 0      # a difference that passes comparison t (0 if none does)
+            if mode == "clip":                                                      # side 0: at 0, 1: at the maximum
+                d = dict(a=0, b1=0, b2=0, b3=ok("b3"), b4=ok("b4"))
+                d["b1" if rng.integers(0, 2) else "b2"] = max(B - 1, 0)
+            else:
+                d = dict(a=ok("a"), b1=ok("b1"), b2=ok("b2"), b3=ok("b3"), b4=ok("b4"))
+                d["a" if mode == "ai" else mode] = max(thr[mode] - 1 + side, 0)
+            s0 = 1 if rng.integers(0, 2) else -1                                    # q0 above or below p0
+            for attempt in range(2):
+                # p3 p2 p1 p0 q0 q1 q2 q3 relative to p0: random directions first, then all pointing inwards (the smallest span)
+                if mode == "clip":
+                    sg = np.full(4, -1 if side else 1)
+                else:
+                    sg = rng.choice([-1, 1], 4) if attempt == 0 else np.array([s0, s0, -s0, -s0])
+                p0, q0 = 0, s0 * d["a"]
+                p1, p2, q1, q2 = p0 + sg[0] * d["b1"], p0 + sg[1] * d["b3"], q0 + sg[2] * d["b2"], q0 + sg[3] * d["b4"]
+                jit = rng.integers(-B, B + 1, 2) if attempt == 0 and B and mode != "clip" else (0, 0)
+                v = np.array([p2 + jit[0], p2, p1, p0, q0, q1, q2, q2 + jit[1]], np.int64)
+                if v.max() - v.min() <= mx:
+                    break
+            lo, hi = -int(v.min()), mx - int(v.max())
+            r = int(rng.integers(0, 6))
+            if mode == "clip":
+                r = side
+            v += lo if r == 0 else hi if r == 1 else int(rng.integers(lo, hi + 1))
+            for j in range(8):
+                if vert:
+                    pic[y0 - 4 + j, x0 + line] = v[j]
+                else:
+                    pic[y0 + line, x0 - 4 + j] = v[j]
+    off = (((e // cols) * LF_CELL + 8) * pic.strides[0] + ((e % cols) * LF_CELL + 8) * pic.itemsize).astype(np.int64)
+    return pic, kinds, off, alpha, beta, tc0
+
+
 def h264lf_hbd_case(seed, n, depth, cols=16):
     """the same layout for 9 / 10 / 12 / 14 bit samples: pic uint16, off in BYTES; the content of the 8-bit case scaled to the depth with
     fresh low bits, so the scaled thresholds see the same mix of branches"""

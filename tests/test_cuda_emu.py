@@ -1335,6 +1335,65 @@ def test_host_h264qpel_hbd(emuhost):
     assert L.emu_host_qpel_hbd_tab(8, 0, 0, 0, got.ctypes.data, img.ctypes.data, Wd * 2) == -38
 
 
+def test_host_hbd_null_table_ops_and_int32_alignment(emuhost):
+    """pel_hbd.cu: a qpel op at size index 3 and a chroma op at width index 3 name entries the reference leaves NULL and write nothing,
+    between valid ops of the same call.  h264weight.cu / videodsp.cu: the 16-bit weight and edge entries read params / geom as int32 and
+    refuse an array that is not 4-byte aligned."""
+    L, O = emuhost, cl.oracle()
+    L.b200_h264qpel_hbd_batch_device.argtypes = [C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_ssize_t]
+    L.b200_h264chroma_hbd_batch_device.argtypes = [C.c_void_p, C.c_int64] + [C.c_void_p] * 7 + [C.c_ssize_t]
+    L.b200_h264_weight_hbd_batch_device.argtypes = [C.c_void_p, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_ssize_t]
+    L.b200_emulated_edge_mc_hbd_batch_device.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_int, C.c_int]
+    O.orc_h264qpel_hbd_batch.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_ssize_t]
+    O.orc_h264chroma_hbd.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_int, C.c_int, C.c_int]
+    dev = C.c_void_p()
+    assert L.b200_device_open(C.byref(dev), 0, None) == 0
+    rng = np.random.default_rng(31)
+    Wd, Hd = 96, 80
+    img = rng.integers(0, 1024, (Hd, Wd)).astype(np.uint16)
+    # 24 ops on a 4 x 6 grid of 16 x 16 cells, every third one at size / width index 3
+    k = np.arange(24)
+    doff = ((k % 4) * 16 * Wd + (k // 4) * 16).astype(np.int64) * 2
+    soff = (rng.integers(3, Hd - 19, 24) * Wd + rng.integers(3, Wd - 19, 24)).astype(np.int64) * 2
+    ops = np.array([(i & 1) | ((3 if i % 3 == 1 else i % 3) << 1) | (int(rng.integers(0, 16)) << 3) for i in range(24)], np.uint8)
+    ok = ((ops >> 1) & 3) != 3
+    got = np.full((Hd, Wd), 0x5A5A, np.uint16)
+    exp = got.copy()
+    assert L.b200_h264qpel_hbd_batch_device(dev, 10, 24, ops.ctypes.data, got.ctypes.data, doff.ctypes.data, img.ctypes.data, soff.ctypes.data, Wd * 2) == 0
+    o, d, s = ops[ok].copy(), doff[ok].copy(), soff[ok].copy()
+    O.orc_h264qpel_hbd_batch(10, len(o), o.ctypes.data, exp.ctypes.data, d.ctypes.data, img.ctypes.data, s.ctypes.data, Wd * 2)
+    assert np.array_equal(got, exp), "qpel size index 3"
+    cop = np.array([(i & 1) | ((3 if i % 3 == 1 else i % 3) << 1) for i in range(24)], np.uint8)
+    hs = rng.choice(np.array([1, 2, 7, 16], np.uint8), 24)
+    xy = rng.integers(0, 64, 24).astype(np.uint8)
+    got = np.full((Hd, Wd), 0x5A5A, np.uint16)
+    exp = got.copy()
+    assert L.b200_h264chroma_hbd_batch_device(dev, 24, cop.ctypes.data, hs.ctypes.data, xy.ctypes.data, got.ctypes.data, doff.ctypes.data,
+                                              img.ctypes.data, soff.ctypes.data, Wd * 2) == 0
+    for j in range(24):
+        if (cop[j] >> 1) & 3 != 3:
+            O.orc_h264chroma_hbd(int(cop[j]) & 1, int(cop[j]) >> 1, exp.ctypes.data + int(doff[j]), img.ctypes.data + int(soff[j]), Wd * 2,
+                                 int(hs[j]), int(xy[j]) & 7, int(xy[j]) >> 3)
+    assert np.array_equal(got, exp), "chroma width index 3"
+    # int32 arrays at 2 bytes past a 16-byte boundary: refused, nothing written
+    raw = _aligned((64,))
+    raw.view(np.int32)[:] = [0 | 16 << 8, 1, 1, 0] * 4
+    dst = np.full((Hd, Wd), 0x5A5A, np.uint16)
+    off = np.zeros(2, np.int64)
+    assert L.b200_h264_weight_hbd_batch_device(dev, 10, 1, raw.ctypes.data + 2, dst.ctypes.data, off.ctypes.data, None, None, Wd * 2) == -22
+    assert L.b200_h264_weight_hbd_batch_device(dev, 10, 1, raw.ctypes.data + 2, dst.ctypes.data, off.ctypes.data, img.ctypes.data,
+                                               off.ctypes.data, Wd * 2) == -22
+    raw.view(np.int32)[:] = [4, 4, 0, 0] * 4
+    assert L.b200_emulated_edge_mc_hbd_batch_device(dev, 1, dst.ctypes.data, off.ctypes.data, Wd * 2, img.ctypes.data, off.ctypes.data, Wd * 2,
+                                                    raw.ctypes.data + 2, Wd, Hd) == -22
+    assert (dst == 0x5A5A).all()
+    # 4-byte aligned but not 16-byte aligned: accepted
+    raw.view(np.int32)[1:5] = [4, 4, 0, 0]
+    assert L.b200_emulated_edge_mc_hbd_batch_device(dev, 1, dst.ctypes.data, off.ctypes.data, Wd * 2, img.ctypes.data, off.ctypes.data, Wd * 2,
+                                                    raw.ctypes.data + 4, Wd, Hd) == 0
+    assert np.array_equal(dst[:4, :4], img[:4, :4])
+
+
 def test_host_chroma_and_edge_hbd(emuhost):
     """pel_hbd.cu: h264chroma for 16-bit samples, and videodsp.cu: emulated_edge_mc for 16-bit and 8-bit samples; batched device entries and
     drop-in table functions on the stand-in runtime against the checker (every eighth-pel phase, put / avg, widths 8 / 4 / 2; windows on and

@@ -820,15 +820,12 @@ def test_pixelutils_sad(device):
 # ---------------------------------------------------------------------------------------------- h264qpel, 9 / 10 / 12 / 14 bit samples
 def test_h264qpel_hbd(device):
     """ff_h264qpel_init(c, depth) for depth 9 / 10 / 12 / 14: the drop-in table functions (host pointers) against the hashes of the compiled
-    reference's outputs, and a macroblock stream through the batched device entry against the oracle"""
+    reference's outputs (the batched device entry: tests/test_h264_hbd_paths_gpu.py)"""
     import ctypes as C
     import hashlib
-    import torch
     import ffmpeg_b200 as fb
     from ffmpeg_b200 import pel
     from ffmpeg_b200._lib import u8p
-    O = cl.oracle()
-    O.orc_h264qpel_hbd_batch.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_ssize_t]
     tabs, pics, n = {}, {}, 0
     for k, line in enumerate(open(os.path.join(G, "pel_hbd_hashes.txt"))):
         if k % 3:
@@ -849,28 +846,6 @@ def test_h264qpel_hbd(device):
     assert n == 256
     with pytest.raises(fb.B200Error):
         pel.ff_h264qpel_init(11)
-    rng = np.random.default_rng(14)
-    W, H = 640, 368
-    for depth in (9, 10, 12, 14):
-        ref_ = rng.integers(0, 1 << depth, (H, W)).astype(np.uint16)
-        dst0 = rng.integers(0, 1 << depth, (H, W)).astype(np.uint16)
-        ops, doffs, soffs = [], [], []
-        for by in range(1, H // 16 - 1):
-            for bx in range(1, W // 16 - 1):
-                ops.append(pel.qpel_op(int(rng.integers(0, 2)), int(rng.integers(0, 3)), int(rng.integers(0, 16))))
-                dx, dy = (int(v) for v in rng.integers(-10, 11, 2))
-                doffs.append((by * 16 * W + bx * 16) * 2); soffs.append(((by * 16 + dy) * W + bx * 16 + dx) * 2)
-        cnt = len(ops)
-        ops_a, do_a, so_a = np.array(ops, np.uint8), np.array(doffs, np.int64), np.array(soffs, np.int64)
-        exp = dst0.copy()
-        O.orc_h264qpel_hbd_batch(depth, cnt, ops_a.ctypes.data, exp.ctypes.data, do_a.ctypes.data, ref_.ctypes.data, so_a.ctypes.data, W * 2)
-        with on_stream(device):
-            d_ops, d_do, d_so = torch.from_numpy(ops_a).cuda(), torch.from_numpy(do_a).cuda(), torch.from_numpy(so_a).cuda()
-            d_dst, d_src = torch.from_numpy(dst0.view(np.int16)).cuda(), torch.from_numpy(ref_.view(np.int16)).cuda()
-            pel.h264qpel_hbd_batch_device(device, depth, cnt, d_ops, d_dst, d_do, d_src, d_so, W * 2)
-            device.sync()
-            got = d_dst.cpu().numpy().view(np.uint16)
-        assert np.array_equal(got, exp), (depth, int((got != exp).sum()))
 
 
 # ---------------------------------------------------------------------------------------------- swscale: same-size packed RGB -> packed RGB
@@ -959,16 +934,12 @@ def test_sws_yuv_matrix_cascade(device):
 # ---------------------------------------------------------------------------------------------- h264chroma + emulated_edge_mc, 16-bit samples
 def test_h264chroma_and_edge_hbd(device):
     """ff_h264chroma_init(c, depth > 8) and ff_videodsp_init(ctx, bpc > 8): drop-in table functions against the hashes of the compiled
-    reference's outputs; batched device entries against the oracle"""
+    reference's outputs (the batched device entries: tests/test_h264_hbd_paths_gpu.py)"""
     import ctypes as C
     import hashlib
-    import torch
     from ffmpeg_b200 import pel
     from ffmpeg_b200._lib import u8p
     from test_oracle_more import hbd_chroma_rows
-    O = cl.oracle()
-    O.orc_h264chroma_hbd.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_int, C.c_int, C.c_int]
-    O.orc_emulated_edge_mc_hbd.argtypes = [C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_ssize_t] + [C.c_int] * 6
     tabs, pics = {}, {}
     vd = pel.ff_videodsp_init(10)
     for k, row in enumerate(hbd_chroma_rows()):
@@ -989,61 +960,18 @@ def test_h264chroma_and_edge_hbd(device):
             vd.emulated_edge_mc(C.cast(out.ctypes.data, u8p), C.cast(pic.ctypes.data + sy * pic.strides[0] + sx * 2, u8p), out.strides[0], pic.strides[0], bw, bh, sx, sy, 64, 48)
             assert hashlib.sha256(out.tobytes()).hexdigest() == hsh, row[:5]
     assert not tabs[10].put_h264_chroma_pixels_tab[3]
-    rng = np.random.default_rng(23)
-    W, H = 640, 368
-    ref_ = rng.integers(0, 1 << 10, (H, W)).astype(np.uint16)
-    dst0 = rng.integers(0, 1 << 10, (H, W)).astype(np.uint16)
-    ops, hs, xys, doffs, soffs = [], [], [], [], []
-    for by in range(1, H // 16 - 1):
-        for bx in range(1, W // 8 - 1):
-            idx = int(rng.integers(0, 3))
-            ops.append(pel.chroma_op(int(rng.integers(0, 2)), idx)); hs.append(int(rng.choice([2, 4, 8, 16]))); xys.append(int(rng.integers(0, 64)))
-            dx, dy = (int(v) for v in rng.integers(-6, 7, 2))
-            doffs.append((by * 16 * W + bx * 8) * 2); soffs.append(((by * 16 + dy) * W + bx * 8 + dx) * 2)
-    n = len(ops)
-    a = [np.array(v, t) for v, t in ((ops, np.uint8), (hs, np.uint8), (xys, np.uint8), (doffs, np.int64), (soffs, np.int64))]
-    exp = dst0.copy()
-    for j in range(n):
-        O.orc_h264chroma_hbd(ops[j] & 1, ops[j] >> 1, exp.ctypes.data + doffs[j], ref_.ctypes.data + soffs[j], W * 2, hs[j], xys[j] & 7, xys[j] >> 3)
-    with on_stream(device):
-        d = [torch.from_numpy(v).cuda() for v in a]
-        d_dst, d_src = torch.from_numpy(dst0.view(np.int16)).cuda(), torch.from_numpy(ref_.view(np.int16)).cuda()
-        pel.h264chroma_hbd_batch_device(device, n, d[0], d[1], d[2], d_dst, d[3], d_src, d[4], W * 2)
-        device.sync()
-        got = d_dst.cpu().numpy().view(np.uint16)
-    assert np.array_equal(got, exp), int((got != exp).sum())
-    # edge emulation: windows all around a 64 x 48 picture, one call
-    pic, _ = cl.hbd_picture(10, 0)
-    geoms = [(int(rng.integers(1, 25)), int(rng.integers(1, 25)), int(rng.integers(-30, 80)), int(rng.integers(-30, 70))) for _ in range(500)]
-    BW = 32
-    g = np.array(geoms, np.int32); og = np.zeros(500, np.int64); bo = (np.arange(500, dtype=np.int64) * 25 * BW * 2)
-    with on_stream(device):
-        d_pic = torch.from_numpy(pic.view(np.int16)).cuda()
-        d_buf = torch.zeros((500 * 25, BW), dtype=torch.int16, device="cuda")
-        d_g, d_og, d_bo = torch.from_numpy(g).cuda(), torch.from_numpy(og).cuda(), torch.from_numpy(bo).cuda()
-        pel.emulated_edge_mc_hbd_batch_device(device, 500, d_buf, d_bo, BW * 2, d_pic, d_og, pic.strides[0], d_g, 64, 48)
-        device.sync()
-        buf = d_buf.cpu().numpy().view(np.uint16)
-    for it, (bw, bh, sx, sy) in enumerate(geoms):
-        e = np.zeros((bh, bw), np.uint16)
-        O.orc_emulated_edge_mc_hbd(e.ctypes.data, pic.ctypes.data + sy * pic.strides[0] + sx * 2, e.strides[0], pic.strides[0], bw, bh, sx, sy, 64, 48)
-        assert np.array_equal(buf[it * 25:it * 25 + bh, :bw], e), ("edge", it)
 
 
 # ---------------------------------------------------------------------------------------------- H.264 weighted prediction, 16-bit samples
 def test_h264_weight_hbd(device):
     """ff_h264dsp_init(c, 9 / 10 / 12 / 14) weight / biweight tables: table functions against the hashes of the compiled reference's
-    outputs, batched device entry against the oracle"""
+    outputs (the batched device entry: tests/test_h264_hbd_paths_gpu.py)"""
     import ctypes as C
     import hashlib
-    import torch
     import ffmpeg_b200 as fb
     from ffmpeg_b200 import pel
     from ffmpeg_b200._lib import u8p
     from test_oracle_more import run_weight_hbd_case, weight_hbd_hashes
-    O = cl.oracle()
-    O.orc_h264_weight_hbd.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_ssize_t] + [C.c_int] * 4
-    O.orc_h264_biweight_hbd.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_ssize_t] + [C.c_int] * 5
     hs = weight_hbd_hashes()
     for depth in (9, 10, 12, 14):
         t = pel.ff_h264dsp_weight_init(depth)
@@ -1055,47 +983,16 @@ def test_h264_weight_hbd(device):
             assert hashlib.sha256(run_weight_hbd_case(wf, bf, depth, case).tobytes()).hexdigest() == hs[(depth, k)], (depth, case)
     with pytest.raises(fb.B200Error):
         pel.ff_h264dsp_weight_init(11)
-    rng = np.random.default_rng(29)
-    W, H, depth = 640, 368, 10
-    # one spare row: the last block shifted by a sample ends a sample into it
-    ref_ = rng.integers(0, 1 << depth, (H + 1, W)).astype(np.uint16)
-    dst0 = rng.integers(0, 1 << depth, (H + 1, W)).astype(np.uint16)
-    for bi in (0, 1):
-        prm, doffs = [], []
-        for by in range(H // 16):
-            for bx in range(W // 16):
-                idx, h, d = int(rng.integers(0, 4)), int(rng.choice([2, 4, 8, 16])), int(rng.integers(0, 8))
-                prm.append([idx | (h << 8) | (d << 16), int(rng.integers(-128, 128)), int(rng.integers(-128, 128)), int(rng.integers(-128, 128))])
-                doffs.append((by * 16 * W + bx * 16) * 2)
-        for shift in (0, 2):                                        # 32-byte-aligned blocks (word accesses), then one sample further
-            prm_a, do_a = np.array(prm, np.int32), np.array(doffs, np.int64) + shift
-            exp = dst0.copy()
-            for p_, o_ in zip(prm, do_a.tolist()):
-                if bi:
-                    O.orc_h264_biweight_hbd(depth, p_[0] & 3, exp.ctypes.data + o_, ref_.ctypes.data + o_, W * 2, (p_[0] >> 8) & 255, p_[0] >> 16, p_[1], p_[2], p_[3])
-                else:
-                    O.orc_h264_weight_hbd(depth, p_[0] & 3, exp.ctypes.data + o_, W * 2, (p_[0] >> 8) & 255, p_[0] >> 16, p_[1], p_[3])
-            with on_stream(device):
-                d_p, d_o = torch.from_numpy(prm_a).cuda(), torch.from_numpy(do_a).cuda()
-                d_dst, d_src = torch.from_numpy(dst0.view(np.int16)).cuda(), torch.from_numpy(ref_.view(np.int16)).cuda()
-                pel.h264_weight_hbd_batch_device(device, depth, len(prm), d_p, d_dst, d_o, d_src if bi else None, d_o if bi else None, W * 2)
-                device.sync()
-                got = d_dst.cpu().numpy().view(np.uint16)
-            assert np.array_equal(got, exp), (bi, shift, int((got != exp).sum()))
 
 
 # ---------------------------------------------------------------------------------------------- H.264 residual adds, 16-bit samples
 def test_h264_idct_hbd(device):
     """ff_h264dsp_init(c, 9 / 10 / 12 / 14) idct_add / idct8_add / idct_dc_add / idct8_dc_add (int32 coefficients): member functions against
-    the hashes of the compiled reference's outputs, batched device entry against the oracle"""
+    the hashes of the compiled reference's outputs (the batched device entry: tests/test_h264_hbd_paths_gpu.py)"""
     import ctypes as C
-    import torch
-    import ffmpeg_b200 as fb
     from ffmpeg_b200 import idctdsp
-    from ffmpeg_b200._lib import lib, vp, check, H264IDCTContext
+    from ffmpeg_b200._lib import lib, check, H264IDCTContext
     from test_oracle_more import h264_idct_hbd_hashes, run_h264_idct_hbd_case
-    O = cl.oracle()
-    O.orc_h264_idct_hbd.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_ssize_t]
     hs = h264_idct_hbd_hashes()
     for depth in (9, 10, 12, 14):
         c = H264IDCTContext()
@@ -1108,27 +1005,6 @@ def test_h264_idct_hbd(device):
                     assert run_h264_idct_hbd_case(fn, depth, kind, case) == hs[(depth, kind, k)], (depth, kind, k)
     c = H264IDCTContext()
     assert lib().b200_h264_idct_init(C.byref(c), 11, 1) < 0
-    rng = np.random.default_rng(37)
-    W, H, depth = 640, 368, 10
-    for kind in range(4):
-        N, B = (64, 8) if kind & 1 else (16, 4)
-        nb = (W // B) * (H // B)
-        blocks = rng.integers(-3000, 3000, (nb, N)).astype(np.int32)
-        # one spare row: the last block shifted by a sample ends a sample into it
-        pic = rng.integers(0, 1 << depth, (H + 1, W)).astype(np.uint16)
-        boff = np.arange(nb, dtype=np.int64) * N
-        for shift in (0, 2):                                        # aligned rows (one access per row), then one sample further
-            doff = np.array([((k // (W // B)) * B * W + (k % (W // B)) * B) * 2 + shift for k in range(nb)], np.int64)
-            exp, eb = pic.copy(), blocks.copy()
-            for k in range(nb):
-                O.orc_h264_idct_hbd(depth, kind, exp.ctypes.data + int(doff[k]), eb.ctypes.data + 4 * int(boff[k]), W * 2)
-            with on_stream(device):
-                d_b, d_bo, d_do = torch.from_numpy(blocks).cuda(), torch.from_numpy(boff).cuda(), torch.from_numpy(doff).cuda()
-                d_p = torch.from_numpy(pic.view(np.int16)).cuda()
-                check(lib().b200_h264_idct_hbd_batch_device(device.handle, depth, kind, nb, vp(d_b.data_ptr()), vp(d_bo.data_ptr()), vp(d_p.data_ptr()), vp(d_do.data_ptr()), W * 2), "h264_idct_hbd_batch")
-                device.sync()
-                got, gb = d_p.cpu().numpy().view(np.uint16), d_b.cpu().numpy()
-            assert np.array_equal(got, exp) and np.array_equal(gb, eb), (kind, shift)
 
 
 # ---------------------------------------------------------------------------------------------- H.264 deblocking, 16-bit samples

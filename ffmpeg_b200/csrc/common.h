@@ -4,6 +4,7 @@
 #include <cstdint>
 #include <cstddef>
 #include <cstdio>
+#include <cstdlib>
 #include <atomic>
 #include <mutex>
 #include "b200dsp.h"
@@ -46,6 +47,54 @@ void *b200_pinned(B200Device *dev, size_t bytes);        // pinned host scratch
     } while (0)
 
 #define B200_LAUNCHED() (g_b200_launches.fetch_add(1, std::memory_order_relaxed))
+
+// The device a batch entry runs on: the caller's, or the default device when `dev` is NULL; made current for the calling thread.
+static inline int b200_use_device(B200Device *&dev)
+{
+    if (!dev) dev = b200_default_device();
+    if (!dev) return B200_ENODEV;
+    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    return 0;
+}
+
+// One host-pointer function-table call's trip through the device (`dev` NULL: the default device).  Such a member returns void, so a
+// failure cannot be reported: it aborts rather than hand back a wrong picture (DESIGN.md §2).  The device lock is held for the
+// object's lifetime, from before `scratch` is obtained until the stream has synchronised, because scratch and stream are per device
+// and the reference functions the members replace are called from many threads at once.
+struct B200HostCall {
+    const char *feature;
+    B200Device *dev;
+    std::lock_guard<std::recursive_mutex> lock;
+    uint8_t *scratch;
+    cudaStream_t stream;
+
+    B200HostCall(const char *feature_, B200Device *dev_, size_t scratch_bytes)
+        : feature(feature_), dev(current(feature_, dev_)), lock(dev->mu), scratch((uint8_t *)b200_scratch(dev, scratch_bytes)),
+          stream(dev->stream)
+    {
+        if (!scratch) fail("scratch");
+    }
+    // also for a member that refuses its arguments before any device work
+    [[noreturn]] static void fail(const char *feature, const char *step)
+    {
+        fprintf(stderr, "libb200dsp: %s failed: %s (%s)\n", feature, step, b200_last_error());
+        abort();
+    }
+    [[noreturn]] void fail(const char *step) const { fail(feature, step); }
+    void check(cudaError_t e, const char *step) const { if (e != cudaSuccess) fail(step); }
+    // after a <<<...>>> launch, or with the return code of a function that launched
+    void launched(int ret = 0) const { if (ret < 0 || cudaGetLastError() != cudaSuccess) fail("launch"); }
+    void sync() const { check(cudaStreamSynchronize(stream), "sync"); }
+
+private:
+    static B200Device *current(const char *feature, B200Device *dev)
+    {
+        if (!dev) dev = b200_default_device();
+        if (!dev) fail(feature, "no device");
+        if (cudaSetDevice(dev->ordinal) != cudaSuccess) fail(feature, "cudaSetDevice");
+        return dev;
+    }
+};
 
 static inline int b200_ceil_div(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
 

@@ -51,18 +51,14 @@ int kind_of(int dct_algo, int bits_per_raw_sample)
 template <int KIND>
 void host_fdct(int16_t *block)
 {
-    auto fail = [](const char *what) { fprintf(stderr, "libb200dsp: fdct failed: %s (%s)\n", what, b200_last_error()); abort(); };
-    B200Device *dev = b200_default_device();
-    if (!dev) fail("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) fail("cudaSetDevice");
-    B200_LOCK_DEVICE(dev);                                        // scratch + stream are per device: one host-pointer call at a time
-    int16_t *scr = (int16_t *)b200_scratch(dev, 128);
-    if (!scr) fail("scratch");
-    cudaStream_t st = dev->stream;
-    if (cudaMemcpyAsync(scr, block, 128, cudaMemcpyHostToDevice, st) != cudaSuccess) fail("h2d");
-    fdct_kernel<<<1, 32, 0, st>>>(KIND, scr, 1);
+    B200HostCall call("fdct", nullptr, 128);
+    int16_t *scr = (int16_t *)call.scratch;
+    call.check(cudaMemcpyAsync(scr, block, 128, cudaMemcpyHostToDevice, call.stream), "h2d");
+    fdct_kernel<<<1, 32, 0, call.stream>>>(KIND, scr, 1);
     B200_LAUNCHED();
-    if (cudaMemcpyAsync(block, scr, 128, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) fail("d2h");
+    call.launched();
+    call.check(cudaMemcpyAsync(block, scr, 128, cudaMemcpyDeviceToHost, call.stream), "d2h");
+    call.sync();
 }
 
 } // namespace
@@ -81,13 +77,11 @@ B200_API int b200_fdctdsp_init(B200FDCTDSPContext *c, int dct_algo, int bits_per
 
 B200_API int b200_fdct_batch_device(B200Device *dev, int dct_algo, int bits_per_raw_sample, int is248, int16_t *blocks, int64_t n)
 {
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
+    if (int r = b200_use_device(dev)) return r;
     if (!blocks || n < 0 || ((uintptr_t)blocks & 15)) return B200_EINVAL;
     const int kind = kind_of(dct_algo, bits_per_raw_sample);
     if (kind < 0) { b200_set_error("fdctdsp: FF_DCT_FAAN is not implemented"); return B200_ENOSYS; }
     if (n == 0) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
     const long long ctas = (n + 31) / 32;                          // 256 threads = 32 blocks of 8 lanes
     if (ctas > 0x7fffffffLL) return B200_EINVAL;
     fdct_kernel<<<(unsigned)ctas, 256, 0, dev->stream>>>(kind | (is248 ? 4 : 0), blocks, n);

@@ -115,47 +115,38 @@ bool uses_src1(int op)
 }
 bool uses_src2(int op) { return op == B200_FDSP_VECTOR_FMUL_WINDOW || op == B200_FDSP_VECTOR_FMUL_ADD; }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: float_dsp failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
+constexpr const char *kFeature = "float_dsp";
 
 // drop-in: one call through the device (host pointers); returns the scalar product for the two reducing ops
 double host_op(int op, void *dst, const void *src0, const void *src1, const void *src2, double mul, int len)
 {
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (len < 0) die("negative length");
+    if (len < 0) B200HostCall::fail(kFeature, "negative length");
     if (len == 0) return 0.0;
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
     const size_t es = is_double(op) ? 8 : 4;
     const bool dot = op == B200_FDSP_SCALARPRODUCT_FLOAT || op == B200_FDSP_SCALARPRODUCT_DOUBLE;
     const size_t nd = dot ? 1 : op == B200_FDSP_VECTOR_FMUL_WINDOW ? 2 * (size_t)len : (size_t)len;
     const size_t n2 = op == B200_FDSP_VECTOR_FMUL_WINDOW ? 2 * (size_t)len : (size_t)len;
     const size_t seg = ((n2 * es) + 255) & ~(size_t)255;
-    B200_LOCK_DEVICE(dev);      // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, 4 * seg);
-    if (!scr) die("scratch");
-    cudaStream_t st = dev->stream;
+    B200HostCall call(kFeature, nullptr, 4 * seg);
+    uint8_t *scr = call.scratch;
+    cudaStream_t st = call.stream;
     Operands o = { scr, scr + seg, scr + 2 * seg, scr + 3 * seg, 0, 0, 0, 0 };
     const bool dst_in = op == B200_FDSP_VECTOR_FMAC_SCALAR || op == B200_FDSP_VECTOR_DMAC_SCALAR || op == B200_FDSP_BUTTERFLIES_FLOAT;
-    if (dst_in && cudaMemcpyAsync(scr, dst, nd * es, cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d dst");
-    if (cudaMemcpyAsync(scr + seg, src0, (size_t)len * es, cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d src0");
-    if (uses_src1(op) && cudaMemcpyAsync(scr + 2 * seg, src1, (size_t)len * es, cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d src1");
-    if (uses_src2(op) && cudaMemcpyAsync(scr + 3 * seg, src2, n2 * es, cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d src2");
-    if (run(dev, st, op, 1, len, o, mul) < 0 || cudaGetLastError() != cudaSuccess) die("launch");
+    if (dst_in) call.check(cudaMemcpyAsync(scr, dst, nd * es, cudaMemcpyHostToDevice, st), "h2d dst");
+    call.check(cudaMemcpyAsync(scr + seg, src0, (size_t)len * es, cudaMemcpyHostToDevice, st), "h2d src0");
+    if (uses_src1(op)) call.check(cudaMemcpyAsync(scr + 2 * seg, src1, (size_t)len * es, cudaMemcpyHostToDevice, st), "h2d src1");
+    if (uses_src2(op)) call.check(cudaMemcpyAsync(scr + 3 * seg, src2, n2 * es, cudaMemcpyHostToDevice, st), "h2d src2");
+    call.launched(run(call.dev, st, op, 1, len, o, mul));
     double ret = 0.0;
     if (dot) {
         union { float f; double d; } r;
-        if (cudaMemcpyAsync(&r, scr, es, cudaMemcpyDeviceToHost, st) != cudaSuccess) die("d2h");
-        if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+        call.check(cudaMemcpyAsync(&r, scr, es, cudaMemcpyDeviceToHost, st), "d2h");
+        call.sync();
         return es == 4 ? (double)r.f : r.d;
     }
-    if (cudaMemcpyAsync(dst, scr, nd * es, cudaMemcpyDeviceToHost, st) != cudaSuccess) die("d2h dst");
-    if (op == B200_FDSP_BUTTERFLIES_FLOAT &&
-        cudaMemcpyAsync(const_cast<void *>(src0), scr + seg, (size_t)len * es, cudaMemcpyDeviceToHost, st) != cudaSuccess) die("d2h v2");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.check(cudaMemcpyAsync(dst, scr, nd * es, cudaMemcpyDeviceToHost, st), "d2h dst");
+    if (op == B200_FDSP_BUTTERFLIES_FLOAT) call.check(cudaMemcpyAsync(const_cast<void *>(src0), scr + seg, (size_t)len * es, cudaMemcpyDeviceToHost, st), "d2h v2");
+    call.sync();
     return ret;
 }
 
@@ -172,7 +163,7 @@ float t_scalarproduct_float(const float *a, const float *b, int n) { return (flo
 void t_vector_dmul(double *d, const double *a, const double *b, int n) { host_op(B200_FDSP_VECTOR_DMUL, d, a, b, nullptr, 0, n); }
 double t_scalarproduct_double(const double *a, const double *b, size_t n)
 {
-    if (n > 0x7fffffff) die("length");
+    if (n > 0x7fffffff) B200HostCall::fail(kFeature, "length");
     return host_op(B200_FDSP_SCALARPRODUCT_DOUBLE, nullptr, a, b, nullptr, 0, (int)n);
 }
 
@@ -194,15 +185,13 @@ B200_API int b200_float_dsp_batch_device(B200Device *dev, int op, int64_t nvec, 
                                          const void *src0, int64_t src0_stride, const void *src1, int64_t src1_stride,
                                          const void *src2, int64_t src2_stride, double mul)
 {
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
+    if (int r = b200_use_device(dev)) return r;
     if (op < 0 || op > B200_FDSP_SCALARPRODUCT_DOUBLE || nvec < 0 || len < 0) return B200_EINVAL;
     if (nvec == 0 || len == 0) return 0;
     if (!dst || !src0 || (uses_src1(op) && !src1) || (uses_src2(op) && !src2)) return B200_EINVAL;
     const uintptr_t am = is_double(op) ? 7 : 3;
     if ((reinterpret_cast<uintptr_t>(dst) | reinterpret_cast<uintptr_t>(src0) | reinterpret_cast<uintptr_t>(src1) |
          reinterpret_cast<uintptr_t>(src2)) & am) return B200_EINVAL;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
     Operands o = { dst, src0, src1 ? src1 : src0, src2 ? src2 : src0, dst_stride, src0_stride, src1_stride, src2_stride };
     const int ret = run(dev, dev->stream, op, nvec, len, o, mul);
     if (ret < 0) return ret;

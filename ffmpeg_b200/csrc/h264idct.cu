@@ -176,12 +176,6 @@ h264_idct_kernel(long long n, dctcoef<P> *blocks, const int64_t *blk_off, uint8_
     store_rows(res);
 }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: h264 idct failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 template <typename P>
 int launch(cudaStream_t st, int kind, int depth, long long n, dctcoef<P> *blocks, const int64_t *blk_off, uint8_t *dst, const int64_t *dst_off,
            long long stride)
@@ -207,24 +201,20 @@ void host_fn(uint8_t *dst, int16_t *block16, ptrdiff_t stride)
     using P = std::conditional_t<DEPTH == 8, uint8_t, uint16_t>;
     constexpr int N = (KIND & 1) ? 8 : 4, NC = N * N;
     dctcoef<P> *block = reinterpret_cast<dctcoef<P> *>(block16);
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
-    B200_LOCK_DEVICE(dev);      // scratch + stream are per device: one host-pointer call at a time (released on return)
     constexpr size_t CB = 64 * sizeof(dctcoef<P>);                // coefficients of an 8x8 block
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, CB + 256);
-    if (!scr) die("scratch");
+    B200HostCall call("h264 idct", nullptr, CB + 256);
+    uint8_t *scr = call.scratch;
     dctcoef<P> *dblk = (dctcoef<P> *)scr;
     uint8_t *dpix = scr + CB;                                      // N rows, pitch 16 bytes
     int64_t *meta = (int64_t *)(scr + CB + 128);
-    cudaStream_t st = dev->stream;
+    cudaStream_t st = call.stream;
     const int64_t m[2] = { 0, 0 };
-    if (cudaMemcpyAsync(dblk, block, (KIND >= 2 ? 1 : NC) * sizeof(dctcoef<P>), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d block");
-    if (b200_h2d_rows(dpix, 16, dst, stride, N * sizeof(P), N, st) != cudaSuccess) die("h2d dst");
-    if (cudaMemcpyAsync(meta, m, sizeof(m), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d meta");
-    if (launch<P>(st, KIND, DEPTH, 1, dblk, meta, dpix, meta + 1, 16) < 0) die("launch");
-    if (b200_d2h_rows(dst, stride, dpix, 16, N * sizeof(P), N, st) != cudaSuccess) die("d2h");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.check(cudaMemcpyAsync(dblk, block, (KIND >= 2 ? 1 : NC) * sizeof(dctcoef<P>), cudaMemcpyHostToDevice, st), "h2d block");
+    call.check(b200_h2d_rows(dpix, 16, dst, stride, N * sizeof(P), N, st), "h2d dst");
+    call.check(cudaMemcpyAsync(meta, m, sizeof(m), cudaMemcpyHostToDevice, st), "h2d meta");
+    call.launched(launch<P>(st, KIND, DEPTH, 1, dblk, meta, dpix, meta + 1, 16));
+    call.check(b200_d2h_rows(dst, stride, dpix, 16, N * sizeof(P), N, st), "d2h");
+    call.sync();
     if (KIND >= 2) block[0] = 0; else memset(block, 0, NC * sizeof(dctcoef<P>));     // what the reference leaves behind
 }
 
@@ -257,7 +247,7 @@ B200_API int b200_h264_idct_batch_device(B200Device *dev, int kind, int64_t n, i
     if (!dev || n < 0 || !blocks || !blk_off || !dst || !dst_off || kind < 0 || kind > 3) return B200_EINVAL;
     if (((uintptr_t)blocks & 15) || ((uintptr_t)dst & ((kind & 1) ? 7 : 3)) || (stride & ((kind & 1) ? 7 : 3))) return B200_EINVAL;
     if (n == 0) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     return launch<uint8_t>(dev->stream, kind, 8, n, blocks, blk_off, dst, dst_off, (long long)stride);
 }
 
@@ -268,6 +258,6 @@ B200_API int b200_h264_idct_hbd_batch_device(B200Device *dev, int bit_depth, int
     if (bit_depth != 9 && bit_depth != 10 && bit_depth != 12 && bit_depth != 14) return B200_ENOSYS;
     if (((uintptr_t)blocks & 3) || ((uintptr_t)dst & 1) || (stride & 1)) return B200_EINVAL;
     if (n == 0) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     return launch<uint16_t>(dev->stream, kind, bit_depth, n, blocks, blk_off, dst, dst_off, (long long)stride);
 }

@@ -115,39 +115,28 @@ int launch(cudaStream_t st, int depth, long long nedges, const uint8_t *kinds, u
     return 0;
 }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: h264 loop filter failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 // drop-in: one edge through the device (host pointers).  The touched window is 4 samples either side of the edge, 16 lines at most.
 template <int DEPTH>
 void host_op(int kind, uint8_t *pix, ptrdiff_t stride, int alpha, int beta, const int8_t *tc0)
 {
     constexpr int BPS = DEPTH > 8 ? 2 : 1;                                // bytes per sample
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
     const LfShape S = lf_shape(kind);
     const int lines = 4 * S.iters;                                        // the lines this edge has (4 per tc0 entry / iteration group)
     const int w = S.vert ? lines : 8, h = S.vert ? 8 : lines;             // window in samples: vert: `lines` columns x rows -4..3; else columns -4..3 x `lines` rows
     uint8_t *origin = S.vert ? pix - 4 * stride : pix - 4 * BPS;
     const size_t pitch = 16 * BPS;
-    B200_LOCK_DEVICE(dev);      // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, pitch * 16 + 64);
-    if (!scr) die("scratch");
-    uint8_t *win = scr, *meta = scr + pitch * 16;
-    cudaStream_t st = dev->stream;
-    if (b200_h2d_rows(win, pitch, origin, stride, (size_t)w * BPS, (size_t)h, st) != cudaSuccess) die("h2d");
+    B200HostCall call("h264 loop filter", nullptr, pitch * 16 + 64);
+    uint8_t *win = call.scratch, *meta = call.scratch + pitch * 16;
+    cudaStream_t st = call.stream;
+    call.check(b200_h2d_rows(win, pitch, origin, stride, (size_t)w * BPS, (size_t)h, st), "h2d");
     struct { int64_t off; int8_t tc[4]; uint8_t kind, alpha, beta, pad; } m;
     m.off = S.vert ? 4 * (int64_t)pitch : 4 * BPS;
     for (int i = 0; i < 4; i++) m.tc[i] = tc0 ? tc0[i] : 0;
     m.kind = (uint8_t)kind; m.alpha = (uint8_t)alpha; m.beta = (uint8_t)beta; m.pad = 0;
-    if (cudaMemcpyAsync(meta, &m, sizeof(m), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d meta");
-    if (launch(st, DEPTH, 1, meta + 12, win, (const int64_t *)meta, (long long)pitch, meta + 13, meta + 14, (const int8_t *)(meta + 8)) < 0) die("launch");
-    if (b200_d2h_rows(origin, stride, win, pitch, (size_t)w * BPS, (size_t)h, st) != cudaSuccess) die("d2h");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.check(cudaMemcpyAsync(meta, &m, sizeof(m), cudaMemcpyHostToDevice, st), "h2d meta");
+    call.launched(launch(st, DEPTH, 1, meta + 12, win, (const int64_t *)meta, (long long)pitch, meta + 13, meta + 14, (const int8_t *)(meta + 8)));
+    call.check(b200_d2h_rows(origin, stride, win, pitch, (size_t)w * BPS, (size_t)h, st), "d2h");
+    call.sync();
 }
 
 template <int DEPTH, int KIND> void tab_tc(uint8_t *pix, ptrdiff_t stride, int alpha, int beta, int8_t *tc0) { host_op<DEPTH>(KIND, pix, stride, alpha, beta, tc0); }
@@ -186,24 +175,20 @@ B200_API int b200_h264_loop_filter_init(B200H264LoopFilterContext *c, int bit_de
 B200_API int b200_h264_loop_filter_batch_device(B200Device *dev, int64_t nedges, const uint8_t *kinds, uint8_t *pix, const int64_t *pix_off,
                                                 ptrdiff_t stride, const uint8_t *alpha, const uint8_t *beta, const int8_t *tc0)
 {
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
+    if (int r = b200_use_device(dev)) return r;
     if (nedges < 0 || stride < 0) return B200_EINVAL;
     if (nedges == 0) return 0;
     if (!kinds || !pix || !pix_off || !alpha || !beta || !tc0) return B200_EINVAL;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
     return launch(dev->stream, 8, nedges, kinds, pix, pix_off, (long long)stride, alpha, beta, tc0);
 }
 
 B200_API int b200_h264_loop_filter_hbd_batch_device(B200Device *dev, int bit_depth, int64_t nedges, const uint8_t *kinds, uint8_t *pix,
                                                     const int64_t *pix_off, ptrdiff_t stride, const uint8_t *alpha, const uint8_t *beta, const int8_t *tc0)
 {
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
+    if (int r = b200_use_device(dev)) return r;
     if (nedges < 0 || stride < 0 || (stride & 1)) return B200_EINVAL;
     if (bit_depth != 9 && bit_depth != 10 && bit_depth != 12 && bit_depth != 14) return B200_ENOSYS;
     if (nedges == 0) return 0;
     if (!kinds || !pix || !pix_off || !alpha || !beta || !tc0 || ((uintptr_t)pix & 1)) return B200_EINVAL;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
     return launch(dev->stream, bit_depth, nedges, kinds, pix, pix_off, (long long)stride, alpha, beta, tc0);
 }

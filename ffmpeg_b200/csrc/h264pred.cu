@@ -398,51 +398,31 @@ cudaError_t launch_add(int depth, long long nops, const uint8_t *kinds, const ui
     return cudaSuccess;
 }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: h264 intra prediction failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 // ---- drop-in members (host pointers).  The window on the device: row 0 = the picture row above the block, rows 1.. the block; block
 // column 0 at byte 16 of a row (the left neighbour just before it, the top-right samples after it).
 constexpr size_t kPitch = 64, kX0 = 16, kRows = 17;
 constexpr size_t kMeta = kPitch * kRows;                                 // kinds, flags, offsets, coefficients follow the window
-
-// the device the drop-in members run on; its scratch and stream are used under B200_LOCK_DEVICE
-B200Device *host_device()
-{
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
-    return dev;
-}
-
-struct Staging {
-    uint8_t *scr;
-    cudaStream_t st;
-};
+constexpr const char *kFeature = "h264 intra prediction";
 
 // copy the neighbours `need` names (NT: W top samples, + ntr top-right ones; NL: H left; NC: the corner) from the host picture
 template <int BPS>
-void h2d_neighbours(const Staging &s, const uint8_t *src, ptrdiff_t stride, int need, int W, int H, int ntr, const uint8_t *topright)
+void h2d_neighbours(const B200HostCall &call, const uint8_t *src, ptrdiff_t stride, int need, int W, int H, int ntr, const uint8_t *topright)
 {
-    uint8_t *win = s.scr + kPitch + kX0;                                 // the block's top-left sample in the window
-    if ((need & NT) && cudaMemcpyAsync(win - kPitch, src - stride, (size_t)W * BPS, cudaMemcpyHostToDevice, s.st) != cudaSuccess) die("h2d top");
-    if (ntr && cudaMemcpyAsync(win - kPitch + W * BPS, topright ? topright : src - stride + W * BPS, (size_t)ntr * BPS, cudaMemcpyHostToDevice, s.st) != cudaSuccess)
-        die("h2d top-right");
-    if ((need & NL) && b200_h2d_rows(win - BPS, kPitch, src - BPS, stride, BPS, (size_t)H, s.st) != cudaSuccess) die("h2d left");
-    if ((need & NC) && cudaMemcpyAsync(win - kPitch - BPS, src - stride - BPS, BPS, cudaMemcpyHostToDevice, s.st) != cudaSuccess) die("h2d corner");
+    uint8_t *win = call.scratch + kPitch + kX0;                          // the block's top-left sample in the window
+    cudaStream_t st = call.stream;
+    if (need & NT) call.check(cudaMemcpyAsync(win - kPitch, src - stride, (size_t)W * BPS, cudaMemcpyHostToDevice, st), "h2d top");
+    if (ntr)
+        call.check(cudaMemcpyAsync(win - kPitch + W * BPS, topright ? topright : src - stride + W * BPS, (size_t)ntr * BPS, cudaMemcpyHostToDevice, st),
+                   "h2d top-right");
+    if (need & NL) call.check(b200_h2d_rows(win - BPS, kPitch, src - BPS, stride, BPS, (size_t)H, st), "h2d left");
+    if (need & NC) call.check(cudaMemcpyAsync(win - kPitch - BPS, src - stride - BPS, BPS, cudaMemcpyHostToDevice, st), "h2d corner");
 }
 
 template <int DEPTH>
 void pred_host(int t, int m, int fl, uint8_t *src, ptrdiff_t stride, const uint8_t *topright)
 {
     constexpr int BPS = DEPTH > 8 ? 2 : 1;
-    B200Device *dev = host_device();
-    B200_LOCK_DEVICE(dev);       // scratch + stream are per device: one host-pointer call at a time (released on return)
-    Staging s = { (uint8_t *)b200_scratch(dev, kMeta + 256), dev->stream };
-    if (!s.scr) die("scratch");
+    B200HostCall call(kFeature, nullptr, kMeta + 256);
     const int W = pred_w(t), H = pred_h(t), need = pred_needs(t, m);
     int ntr = 0, nd = need;
     if (t == P4 && (need & NTR)) ntr = 4;                                // from `topright`, wherever it points (h264_mb.c:676-691)
@@ -450,18 +430,17 @@ void pred_host(int t, int m, int fl, uint8_t *src, ptrdiff_t stride, const uint8
         if ((fl & 2) && (need & NT)) ntr = (need & NTR) ? 8 : 1;
         if ((fl & 1) && (need & (NT | NL))) nd |= NC;
     }
-    h2d_neighbours<BPS>(s, src, stride, nd, W, H, ntr, t == P4 ? topright : nullptr);
-    uint8_t *meta = s.scr + kMeta;
+    h2d_neighbours<BPS>(call, src, stride, nd, W, H, ntr, t == P4 ? topright : nullptr);
+    uint8_t *meta = call.scratch + kMeta;
     struct { long long off; uint8_t kind, flags, pad[6]; } h;
     h.off = (long long)(kPitch + kX0);
     h.kind = (uint8_t)(t << 4 | m);
     h.flags = (uint8_t)(t == P4 ? (ntr ? 2 : 0) : fl);                   // pred4x4: the four samples are in the window's top row
     memset(h.pad, 0, sizeof(h.pad));
-    if (cudaMemcpyAsync(meta, &h, sizeof(h), cudaMemcpyHostToDevice, s.st) != cudaSuccess) die("h2d meta");
-    if (launch_pred(DEPTH, 1, meta + 8, meta + 9, s.scr, (const long long *)meta, (long long)kPitch, s.st) != cudaSuccess)
-        die("launch");
-    if (b200_d2h_rows(src, stride, s.scr + kPitch + kX0, kPitch, (size_t)W * BPS, (size_t)H, s.st) != cudaSuccess) die("d2h");
-    if (cudaStreamSynchronize(s.st) != cudaSuccess) die("sync");
+    call.check(cudaMemcpyAsync(meta, &h, sizeof(h), cudaMemcpyHostToDevice, call.stream), "h2d meta");
+    call.check(launch_pred(DEPTH, 1, meta + 8, meta + 9, call.scratch, (const long long *)meta, (long long)kPitch, call.stream), "launch");
+    call.check(b200_d2h_rows(src, stride, call.scratch + kPitch + kX0, kPitch, (size_t)W * BPS, (size_t)H, call.stream), "d2h");
+    call.sync();
 }
 
 // pred4x4_add / pred8x8l_add / pred8x8l_filter_add through the device: the edge the function starts from, the coefficients, and back
@@ -470,31 +449,29 @@ void add_host(int t, int m, int fl, uint8_t *pix, int16_t *block, ptrdiff_t stri
 {
     constexpr int BPS = DEPTH > 8 ? 2 : 1;
     using C = typename std::conditional<(DEPTH > 8), int32_t, int16_t>::type;
-    B200Device *dev = host_device();
-    B200_LOCK_DEVICE(dev);
     const int N = t == A4 ? 4 : 8;
     const size_t cbytes = (size_t)N * N * sizeof(C);
-    Staging s = { (uint8_t *)b200_scratch(dev, kMeta + 256 + cbytes), dev->stream };
-    if (!s.scr) die("scratch");
+    B200HostCall call(kFeature, nullptr, kMeta + 256 + cbytes);
     const bool vert = m == 0;
     int need = vert ? NT : NL, ntr = 0;
     if (t == A8LF && (fl & 1)) need |= NC;                               // PREDICT_8x8_LOAD_TOP / _LEFT read the corner when has_topleft
     if (t == A8LF && (fl & 2) && vert) ntr = 1;                          // and SRC(8, -1) when has_topright
-    h2d_neighbours<BPS>(s, pix, stride, need, N, N, ntr, nullptr);
-    uint8_t *meta = s.scr + kMeta, *dcoef = meta + 256;
+    h2d_neighbours<BPS>(call, pix, stride, need, N, N, ntr, nullptr);
+    uint8_t *meta = call.scratch + kMeta, *dcoef = meta + 256;
     struct { long long off, coff; uint8_t kind, flags, pad[6]; } h;
     h.off = (long long)(kPitch + kX0);
     h.coff = 0;
     h.kind = (uint8_t)(t << 4 | m);
     h.flags = (uint8_t)fl;
     memset(h.pad, 0, sizeof(h.pad));
-    if (cudaMemcpyAsync(meta, &h, sizeof(h), cudaMemcpyHostToDevice, s.st) != cudaSuccess) die("h2d meta");
-    if (cudaMemcpyAsync(dcoef, block, cbytes, cudaMemcpyHostToDevice, s.st) != cudaSuccess) die("h2d coefficients");
-    if (launch_add(DEPTH, 1, meta + 16, meta + 17, s.scr, (const long long *)meta, (long long)kPitch, dcoef, (const long long *)(meta + 8), s.st) != cudaSuccess)
-        die("launch");
-    if (b200_d2h_rows(pix, stride, s.scr + kPitch + kX0, kPitch, (size_t)N * BPS, (size_t)N, s.st) != cudaSuccess) die("d2h");
-    if (cudaMemcpyAsync(block, dcoef, cbytes, cudaMemcpyDeviceToHost, s.st) != cudaSuccess) die("d2h coefficients");
-    if (cudaStreamSynchronize(s.st) != cudaSuccess) die("sync");
+    cudaStream_t st = call.stream;
+    call.check(cudaMemcpyAsync(meta, &h, sizeof(h), cudaMemcpyHostToDevice, st), "h2d meta");
+    call.check(cudaMemcpyAsync(dcoef, block, cbytes, cudaMemcpyHostToDevice, st), "h2d coefficients");
+    call.check(launch_add(DEPTH, 1, meta + 16, meta + 17, call.scratch, (const long long *)meta, (long long)kPitch, dcoef, (const long long *)(meta + 8), st),
+               "launch");
+    call.check(b200_d2h_rows(pix, stride, call.scratch + kPitch + kX0, kPitch, (size_t)N * BPS, (size_t)N, st), "d2h");
+    call.check(cudaMemcpyAsync(block, dcoef, cbytes, cudaMemcpyDeviceToHost, st), "d2h coefficients");
+    call.sync();
 }
 
 // pred8x8_add / pred16x16_add through the device with the caller's block_offset table, in table order (template :1275-1330; the 8x16
@@ -505,7 +482,7 @@ void add_table_host(int t, int m, uint8_t *pix, const int *block_offset, int16_t
 {
     constexpr int BPS = DEPTH > 8 ? 2 : 1;
     using C = typename std::conditional<(DEPTH > 8), int32_t, int16_t>::type;
-    if (stride == 0) die("zero stride");
+    if (stride == 0) B200HostCall::fail(kFeature, "zero stride");
     const int nsub = t == A16 ? 16 : t == A816 ? 8 : 4;
     const bool vert = m == 2;
     long long dx[16], dy[16], minx = 0, maxx = 0, miny = 0, maxy = 0;
@@ -521,29 +498,27 @@ void add_table_host(int t, int m, uint8_t *pix, const int *block_offset, int16_t
     const long long x0 = minx - (vert ? 0 : BPS), y0 = miny - (vert ? 1 : 0), x1 = maxx + 4 * BPS, y1 = maxy + 4;
     const size_t wbytes = (size_t)(x1 - x0), rows = (size_t)(y1 - y0), pitch = (wbytes + 15) & ~(size_t)15;
     const size_t cbytes = (size_t)nsub * 16 * sizeof(C), wsize = pitch * rows;
-    B200Device *dev = host_device();
-    B200_LOCK_DEVICE(dev);
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, wsize + 16 * sizeof(long long) + cbytes + 64);
-    if (!scr) die("scratch");
-    cudaStream_t st = dev->stream;
+    B200HostCall call(kFeature, nullptr, wsize + 16 * sizeof(long long) + cbytes + 64);
+    uint8_t *scr = call.scratch;
+    cudaStream_t st = call.stream;
     uint8_t *doffs = scr + ((wsize + 15) & ~(size_t)15), *dcoef = doffs + 16 * sizeof(long long);
     long long offs[16];
     for (int k = 0; k < nsub; k++) offs[k] = (dy[k] - y0) * (long long)pitch + (dx[k] - x0);
     const uint8_t *org = pix + x0 + y0 * (long long)stride;
-    if (b200_h2d_rows(scr, pitch, org, stride, wbytes, rows, st) != cudaSuccess) die("h2d window");
-    if (cudaMemcpyAsync(doffs, offs, sizeof(offs), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d offsets");
-    if (cudaMemcpyAsync(dcoef, block, cbytes, cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d coefficients");
+    call.check(b200_h2d_rows(scr, pitch, org, stride, wbytes, rows, st), "h2d window");
+    call.check(cudaMemcpyAsync(doffs, offs, sizeof(offs), cudaMemcpyHostToDevice, st), "h2d offsets");
+    call.check(cudaMemcpyAsync(dcoef, block, cbytes, cudaMemcpyHostToDevice, st), "h2d coefficients");
     using P = typename std::conditional<(DEPTH > 8), uint16_t, uint8_t>::type;
     h264_pred_add_table_kernel<P, C><<<1, 32, 0, st>>>(scr, (const long long *)doffs, nsub, vert, (long long)pitch, (C *)dcoef);
     B200_LAUNCHED();
-    if (cudaGetLastError() != cudaSuccess) die("launch");
+    call.launched();
     // back: the sub-blocks' rectangle (without the row above / the column to the left)
     const long long bx0 = minx, by0 = miny;
-    if (b200_d2h_rows(pix + bx0 + by0 * (long long)stride, stride, scr + (by0 - y0) * (long long)pitch + (bx0 - x0), pitch, (size_t)(x1 - bx0),
-                      (size_t)(y1 - by0), st) != cudaSuccess)
-        die("d2h");
-    if (cudaMemcpyAsync(block, dcoef, cbytes, cudaMemcpyDeviceToHost, st) != cudaSuccess) die("d2h coefficients");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.check(b200_d2h_rows(pix + bx0 + by0 * (long long)stride, stride, scr + (by0 - y0) * (long long)pitch + (bx0 - x0), pitch, (size_t)(x1 - bx0),
+                             (size_t)(y1 - by0), st),
+               "d2h");
+    call.check(cudaMemcpyAsync(block, dcoef, cbytes, cudaMemcpyDeviceToHost, st), "d2h coefficients");
+    call.sync();
 }
 
 template <int D, int M> void tab4(uint8_t *src, const uint8_t *topright, ptrdiff_t stride) { pred_host<D>(P4, M, 0, src, stride, topright); }
@@ -619,9 +594,7 @@ B200_API int b200_h264_pred_batch_device(B200Device *dev, int bit_depth, int64_t
         b200_set_error("h264 pred batch: NULL or misaligned pointer");
         return B200_EINVAL;
     }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     B200_CUDA_OK(launch_pred(bit_depth, nops, kinds, flags, pix, (const long long *)pix_off, (long long)stride, dev->stream));
     return 0;
 }
@@ -635,9 +608,7 @@ B200_API int b200_h264_pred_add_batch_device(B200Device *dev, int bit_depth, int
         b200_set_error("h264 pred add batch: NULL or misaligned pointer");
         return B200_EINVAL;
     }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     B200_CUDA_OK(launch_add(bit_depth, nops, kinds, flags, pix, (const long long *)pix_off, (long long)stride, coef, (const long long *)coef_off, dev->stream));
     return 0;
 }

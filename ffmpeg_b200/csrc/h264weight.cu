@@ -83,36 +83,27 @@ int launch(cudaStream_t st, int depth, long long n, const int32_t *params, uint8
     return 0;
 }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: h264 weighted prediction failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 // drop-in: one block through the device (host pointers)
 template <int DEPTH>
 void host_op(bool bi, int idx, uint8_t *dst, const uint8_t *src, ptrdiff_t stride, int height, int log2_denom, int wd, int ws, int offset)
 {
     constexpr int BPS = DEPTH > 8 ? 2 : 1;                                // bytes per sample
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (height < 0 || height > 255 || log2_denom < 0 || log2_denom > 7) die("unsupported height / log2_denom");
+    const char *feature = "h264 weighted prediction";
+    if (height < 0 || height > 255 || log2_denom < 0 || log2_denom > 7) B200HostCall::fail(feature, "unsupported height / log2_denom");
     if (height == 0) return;
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
     const size_t wb = (size_t)(16 >> idx) * BPS, pitch = 16 * BPS;      // row bytes of the block, of the staging copy
-    B200_LOCK_DEVICE(dev);      // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, 2 * pitch * 256 + 256);
-    if (!scr) die("scratch");
+    B200HostCall call(feature, nullptr, 2 * pitch * 256 + 256);
+    uint8_t *scr = call.scratch;
     uint8_t *ddst = scr, *dsrc = scr + pitch * 256, *meta = scr + 2 * pitch * 256;
-    cudaStream_t st = dev->stream;
-    if (b200_h2d_rows(ddst, pitch, dst, stride, wb, (size_t)height, st) != cudaSuccess) die("h2d dst");
-    if (bi && b200_h2d_rows(dsrc, pitch, src, stride, wb, (size_t)height, st) != cudaSuccess) die("h2d src");
+    cudaStream_t st = call.stream;
+    call.check(b200_h2d_rows(ddst, pitch, dst, stride, wb, (size_t)height, st), "h2d dst");
+    if (bi) call.check(b200_h2d_rows(dsrc, pitch, src, stride, wb, (size_t)height, st), "h2d src");
     struct { int32_t p[4]; int64_t doff, soff; } m = { { idx | (height << 8) | (log2_denom << 16), wd, ws, offset }, 0, 0 };
-    if (cudaMemcpyAsync(meta, &m, sizeof(m), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d meta");
+    call.check(cudaMemcpyAsync(meta, &m, sizeof(m), cudaMemcpyHostToDevice, st), "h2d meta");
     const int64_t *doff = (const int64_t *)(meta + 16), *soff = doff + 1;
-    if (launch(st, DEPTH, 1, (const int32_t *)meta, ddst, doff, bi ? dsrc : nullptr, soff, (long long)pitch) < 0) die("launch");
-    if (b200_d2h_rows(dst, stride, ddst, pitch, wb, (size_t)height, st) != cudaSuccess) die("d2h");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.launched(launch(st, DEPTH, 1, (const int32_t *)meta, ddst, doff, bi ? dsrc : nullptr, soff, (long long)pitch));
+    call.check(b200_d2h_rows(dst, stride, ddst, pitch, wb, (size_t)height, st), "d2h");
+    call.sync();
 }
 
 template <int DEPTH, int IDX>
@@ -156,7 +147,7 @@ B200_API int b200_h264_weight_batch_device(B200Device *dev, int64_t n, const int
     if (!dev || n < 0 || !params || !dst || !dst_off || (src && !src_off)) return B200_EINVAL;
     if ((uintptr_t)params & 15) return B200_EINVAL;
     if (n == 0) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     return launch(dev->stream, 8, n, params, dst, dst_off, src, src_off, (long long)stride);
 }
 
@@ -168,6 +159,6 @@ B200_API int b200_h264_weight_hbd_batch_device(B200Device *dev, int bit_depth, i
     if ((stride & 1) || ((reinterpret_cast<uintptr_t>(dst) | reinterpret_cast<uintptr_t>(src)) & 1)) return B200_EINVAL;
     if ((uintptr_t)params & 3) return B200_EINVAL;                     // the kernel reads params as int32
     if (n == 0) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     return launch(dev->stream, bit_depth, n, params, dst, dst_off, src, src_off, (long long)stride);
 }

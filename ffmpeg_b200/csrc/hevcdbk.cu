@@ -156,12 +156,6 @@ cudaError_t launch(const DbkArgs &a0, bool chroma, cudaStream_t st)
     return cudaGetLastError();
 }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: hevc deblocking failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 // ---- drop-in members (host pointers): the edge is staged into a 16 x 16 scratch plane with Q0 of line 0 at (8, 0) (vertical edge)
 // or (0, 8) (horizontal edge) and run through the plane kernel with its two segments in the grids.  Per segment j with tc[j] > 0 (the
 // reference does nothing for the others), the lines 4j..4j+3 of P3..Q3 (luma) or P1..Q1 (chroma) go up, and P2..Q2 / P0..Q0 (what the
@@ -172,13 +166,9 @@ void member_host(int depth, bool chroma, bool horiz, uint8_t *pix, ptrdiff_t str
     if (tc[0] <= 0 && tc[1] <= 0) return;
     const int bps = depth > 8 ? 2 : 1, reach = chroma ? 2 : 4, wr = chroma ? 1 : 3;
     const size_t dpitch = 16 * (size_t)bps;
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
-    B200_LOCK_DEVICE(dev);            // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, 256 + 16 * dpitch);
-    if (!scr) die("scratch");
-    cudaStream_t st = dev->stream;
+    B200HostCall call("hevc deblocking", nullptr, 256 + 16 * dpitch);
+    uint8_t *scr = call.scratch;
+    cudaStream_t st = call.stream;
     B200HevcDbkSeg seg[64];
     memset(seg, 0, sizeof(seg));
     B200HevcDbkSeg *vs = seg, *hs = seg + 32;                // vertical: 16 x 8 plane, vseg 2 x 2; horizontal: 8 x 16 plane, hseg 2 x 2
@@ -193,22 +183,22 @@ void member_host(int depth, bool chroma, bool horiz, uint8_t *pix, ptrdiff_t str
     // host sample (column c, line r) of the edge <-> device plane sample
     auto hp = [&](int c, int r) { return pix + (ptrdiff_t)r * stride + (ptrdiff_t)c * bps; };
     auto dp = [&](int c, int r) { return plane + (size_t)(r + (horiz ? 8 : 0)) * dpitch + (size_t)(c + (horiz ? 0 : 8)) * bps; };
-    if (cudaMemcpyAsync(scr, seg, sizeof(seg), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d segments");
+    call.check(cudaMemcpyAsync(scr, seg, sizeof(seg), cudaMemcpyHostToDevice, st), "h2d segments");
     for (int j = 0; j < 2; j++) {
         if (tc[j] <= 0) continue;
         cudaError_t e = horiz ? b200_h2d_rows(dp(4 * j, -reach), dpitch, hp(4 * j, -reach), stride, 4 * (size_t)bps, 2 * (size_t)reach, st)
                               : b200_h2d_rows(dp(-reach, 4 * j), dpitch, hp(-reach, 4 * j), stride, 2 * (size_t)reach * bps, 4, st);
-        if (e != cudaSuccess) die("h2d edge");
+        call.check(e, "h2d edge");
     }
     DbkArgs a = { plane, (long long)dpitch, dseg, dseg + 32, 2, 2, horiz ? 8 : 16, horiz ? 16 : 8, depth, 0 };
-    if (launch(a, chroma, st) != cudaSuccess) die("launch");
+    call.check(launch(a, chroma, st), "launch");
     for (int j = 0; j < 2; j++) {
         if (tc[j] <= 0) continue;
         cudaError_t e = horiz ? b200_d2h_rows(hp(4 * j, -wr), stride, dp(4 * j, -wr), dpitch, 4 * (size_t)bps, 2 * (size_t)wr, st)
                               : b200_d2h_rows(hp(-wr, 4 * j), stride, dp(-wr, 4 * j), dpitch, 2 * (size_t)wr * bps, 4, st);
-        if (e != cudaSuccess) die("d2h edge");
+        call.check(e, "d2h edge");
     }
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.sync();
 }
 
 // for a vertical edge the member's `pix` is Q0 of line 0 and lines run down the rows; for a horizontal one lines run along the row
@@ -278,9 +268,7 @@ B200_API int b200_hevc_deblock_plane_device(B200Device *dev, int bit_depth, int 
         b200_set_error("hevc deblock plane: grid stride shorter than the grid row");
         return B200_EINVAL;
     }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     const DbkArgs a = { pix, (long long)stride, vseg, hseg, (long long)vseg_stride, (long long)hseg_stride, width, height, bit_depth, 0 };
     B200_CUDA_OK(launch(a, chroma != 0, dev->stream));
     return 0;

@@ -180,25 +180,15 @@ cudaError_t launch(TuArgs a, cudaStream_t st)
     return cudaSuccess;
 }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: hevc transform failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 // ---- drop-in members (host pointers): one op through the device scratch.  res != nullptr: the members that work in place on the
 // coefficients (the kernel's int16 result is copied back over them); else add_residual (the block of dst is staged and copied back).
 void member_host(int depth, int log2, int kind, int flags, int col_limit, int16_t *coeffs, const int16_t *res, uint8_t *dst, ptrdiff_t stride)
 {
     const int N = 1 << log2, bps = depth > 8 ? 2 : 1;
     const size_t cbytes = (size_t)N * N * sizeof(int16_t), dpitch = (size_t)N * bps;
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
-    B200_LOCK_DEVICE(dev);            // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, 256 + 3 * 2048);
-    if (!scr) die("scratch");
-    cudaStream_t st = dev->stream;
+    B200HostCall call("hevc transform", nullptr, 256 + 3 * 2048);
+    uint8_t *scr = call.scratch;
+    cudaStream_t st = call.stream;
     uint8_t *dop = scr, *dcoef = scr + 256, *dres = dcoef + 2048, *ddst = dres + 2048;
     B200HevcTuOp op;
     memset(&op, 0, sizeof(op));
@@ -206,17 +196,14 @@ void member_host(int depth, int log2, int kind, int flags, int col_limit, int16_
     op.kind = (uint8_t)kind;
     op.flags = (uint8_t)flags;
     op.col_limit = col_limit;
-    if (cudaMemcpyAsync(dop, &op, sizeof(op), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d op");
-    if (cudaMemcpyAsync(dcoef, coeffs ? coeffs : res, cbytes, cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d coefficients");
-    if (!coeffs && b200_h2d_rows(ddst, dpitch, dst, stride, dpitch, (size_t)N, st) != cudaSuccess) die("h2d block");
+    call.check(cudaMemcpyAsync(dop, &op, sizeof(op), cudaMemcpyHostToDevice, st), "h2d op");
+    call.check(cudaMemcpyAsync(dcoef, coeffs ? coeffs : res, cbytes, cudaMemcpyHostToDevice, st), "h2d coefficients");
+    if (!coeffs) call.check(b200_h2d_rows(ddst, dpitch, dst, stride, dpitch, (size_t)N, st), "h2d block");
     TuArgs a = { (const B200HevcTuOp *)dop, 1, (const int16_t *)dcoef, ddst, (long long)dpitch, coeffs ? (int16_t *)dres : nullptr, depth, 1 };
-    if (launch(a, st) != cudaSuccess) die("launch");
-    if (coeffs) {
-        if (cudaMemcpyAsync(coeffs, dres, cbytes, cudaMemcpyDeviceToHost, st) != cudaSuccess) die("d2h coefficients");
-    } else if (b200_d2h_rows(dst, stride, ddst, dpitch, dpitch, (size_t)N, st) != cudaSuccess) {
-        die("d2h block");
-    }
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.check(launch(a, st), "launch");
+    if (coeffs) call.check(cudaMemcpyAsync(coeffs, dres, cbytes, cudaMemcpyDeviceToHost, st), "d2h coefficients");
+    else call.check(b200_d2h_rows(dst, stride, ddst, dpitch, dpitch, (size_t)N, st), "d2h block");
+    call.sync();
 }
 
 bool log2_ok(int log2, const char *who)
@@ -294,9 +281,7 @@ B200_API int b200_hevc_transform_add_batch_device(B200Device *dev, int bit_depth
         b200_set_error("hevc transform batch: NULL or misaligned pointer");
         return B200_EINVAL;
     }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     TuArgs a = { ops, (long long)nops, coef, dst, (long long)dst_stride, nullptr, bit_depth, 1 };
     B200_CUDA_OK(launch(a, dev->stream));
     return 0;

@@ -203,9 +203,7 @@ B200_API int b200_hevc_intra_recon_picture_device(B200Device *dev, int bit_depth
         b200_set_error("hevc intra picture: ops / coef NULL or not aligned to 16 bytes");
         return B200_EINVAL;
     }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     B200_LOCK_DEVICE(dev);
     int *timeouts = b200_wait_timeouts_word(dev->ordinal, B200_WAIT_HEVC_INTRA, true);
     if (!timeouts) { b200_set_error("hevc intra picture: no timeout counter for device %d", dev->ordinal); return B200_ENOMEM; }
@@ -256,9 +254,7 @@ B200_API int b200_hevc_intra_recon_picture_device(B200Device *dev, int bit_depth
 B200_API int b200_hevc_intra_timeouts(B200Device *dev, int64_t *count)
 {
     if (!count) { b200_set_error("hevc intra timeouts: NULL pointer"); return B200_EINVAL; }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     B200_CUDA_OK(cudaStreamSynchronize(dev->stream));
     int v = 0;
     int *w = b200_wait_timeouts_word(dev->ordinal, B200_WAIT_HEVC_INTRA, false);

@@ -203,12 +203,6 @@ cudaError_t launch(McArgs a, int epel, cudaStream_t st)
     return cudaSuccess;
 }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: hevc motion compensation failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 // ---- drop-in members (host pointers).  The samples the reference function reads are copied into a dense device window that is the
 // op's whole "picture" (so the clamped reads never clamp), src2 next to it, one op, and the block back.
 enum { F_PLAIN, F_UNI, F_UNI_W, F_BI, F_BI_W };
@@ -217,24 +211,22 @@ void member_host(int depth, int epel, int form, int vdir, int hdir, uint8_t *dst
                  const int16_t *src2, int height, int denom, int wx0, int wx1, int ox, intptr_t mx, intptr_t my, int width)
 {
     const int maxp = epel ? 7 : 3, zero = maxp + 1, B = epel ? 1 : 3, A = epel ? 2 : 4, bps = depth > 8 ? 2 : 1;
-    if (width < 1 || width > kMaxPb || height < 1 || height > kMaxPb) die("width / height outside 1..64");
-    if ((hdir && (mx < 0 || mx > maxp)) || (vdir && (my < 0 || my > maxp))) die("phase outside the filter table");
-    if ((form == F_UNI_W || form == F_BI_W) && (denom < 0 || denom > 7)) die("denom outside 0..7");
+    const char *feature = "hevc motion compensation";
+    if (width < 1 || width > kMaxPb || height < 1 || height > kMaxPb) B200HostCall::fail(feature, "width / height outside 1..64");
+    if ((hdir && (mx < 0 || mx > maxp)) || (vdir && (my < 0 || my > maxp))) B200HostCall::fail(feature, "phase outside the filter table");
+    if ((form == F_UNI_W || form == F_BI_W) && (denom < 0 || denom > 7)) B200HostCall::fail(feature, "denom outside 0..7");
     const int x0 = hdir ? B : 0, y0 = vdir ? B : 0, wc = width + (hdir ? B + A : 0), wr = height + (vdir ? B + A : 0);
     const size_t wpitch = ((size_t)wc * bps + 15) & ~(size_t)15, wbytes = (wpitch * wr + 255) & ~(size_t)255;
     const size_t s2bytes = (size_t)kMaxPb * kMaxPb * sizeof(int16_t), dpitch = form == F_PLAIN ? kMaxPb * sizeof(int16_t) : wpitch;
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
-    B200_LOCK_DEVICE(dev);            // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, wbytes + s2bytes + 256 + dpitch * kMaxPb);
-    if (!scr) die("scratch");
-    cudaStream_t st = dev->stream;
+    B200HostCall call(feature, nullptr, wbytes + s2bytes + 256 + dpitch * kMaxPb);
+    uint8_t *scr = call.scratch;
+    cudaStream_t st = call.stream;
     uint8_t *dwin = scr, *ds2 = scr + wbytes, *dop = ds2 + s2bytes, *ddst = dop + 256;
-    if (b200_h2d_rows(dwin, wpitch, src - y0 * srcstride - x0 * bps, srcstride, (size_t)wc * bps, (size_t)wr, st) != cudaSuccess) die("h2d window");
+    call.check(b200_h2d_rows(dwin, wpitch, src - y0 * srcstride - x0 * bps, srcstride, (size_t)wc * bps, (size_t)wr, st), "h2d window");
     const bool bi = form == F_BI || form == F_BI_W;
-    if (bi && b200_h2d_rows(ds2, kMaxPb * sizeof(int16_t), src2, kMaxPb * sizeof(int16_t), (size_t)width * sizeof(int16_t), (size_t)height, st) != cudaSuccess)
-        die("h2d src2");
+    if (bi)
+        call.check(b200_h2d_rows(ds2, kMaxPb * sizeof(int16_t), src2, kMaxPb * sizeof(int16_t), (size_t)width * sizeof(int16_t), (size_t)height, st),
+                   "h2d src2");
     B200HevcMcOp op;
     memset(&op, 0, sizeof(op));
     const int r = bi ? 1 : 0;
@@ -249,16 +241,13 @@ void member_host(int depth, int epel, int form, int vdir, int hdir, uint8_t *dst
     op.wx0 = wx0;
     op.wx1 = wx1;
     op.ox = ox;
-    if (cudaMemcpyAsync(dop, &op, sizeof(op), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d op");
+    call.check(cudaMemcpyAsync(dop, &op, sizeof(op), cudaMemcpyHostToDevice, st), "h2d op");
     McArgs a = { (const B200HevcMcOp *)dop, 1, ddst, (long long)dpitch, dwin, (long long)wpitch, wc, wr, depth, 1, zero, kPlain,
                  bi ? (const int16_t *)ds2 : nullptr };
-    if (launch(a, epel, st) != cudaSuccess) die("launch");
-    if (form == F_PLAIN) {
-        if (b200_d2h_rows(dst, kMaxPb * sizeof(int16_t), ddst, dpitch, (size_t)width * sizeof(int16_t), (size_t)height, st) != cudaSuccess) die("d2h");
-    } else if (b200_d2h_rows(dst, dststride, ddst, dpitch, (size_t)width * bps, (size_t)height, st) != cudaSuccess) {
-        die("d2h");
-    }
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.check(launch(a, epel, st), "launch");
+    if (form == F_PLAIN) call.check(b200_d2h_rows(dst, kMaxPb * sizeof(int16_t), ddst, dpitch, (size_t)width * sizeof(int16_t), (size_t)height, st), "d2h");
+    else call.check(b200_d2h_rows(dst, dststride, ddst, dpitch, (size_t)width * bps, (size_t)height, st), "d2h");
+    call.sync();
 }
 
 template <int D, int E, int V, int H>
@@ -349,9 +338,7 @@ B200_API int b200_hevc_mc_batch_device(B200Device *dev, int bit_depth, int epel,
         b200_set_error("hevc mc batch: NULL or misaligned pointer");
         return B200_EINVAL;
     }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     McArgs a = { ops, (long long)nops, dst, (long long)dst_stride, ref, (long long)ref_stride, pic_w, pic_h, bit_depth, 1,
                  epel ? 7 : 3, B200_HEVC_MC_BI_W, nullptr };
     B200_CUDA_OK(launch(a, epel, dev->stream));

@@ -84,12 +84,6 @@ cudaError_t launch_batch(IntraArgs a, cudaStream_t st)
     return cudaSuccess;
 }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: hevc intra prediction failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 // ---- prediction members (host pointers): top[t0..t1) and left[t0..t1) staged (index -1 = the corner), the block predicted into a
 // scratch block and copied back.  `stride` is in samples, as intra_pred passes it (linesize / sizeof(pixel)).
 template <int D>
@@ -104,21 +98,17 @@ void member_run(uint8_t *dst, ptrdiff_t stride, const uint8_t *top_, const uint8
         staged[kPad + 1 + i] = left[i];
         staged[kArr + kPad + 1 + i] = top[i];
     }
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
-    B200_LOCK_DEVICE(dev);            // scratch + stream are per device: one host-pointer call at a time (released on return)
     const size_t blk = (size_t)size * size * sizeof(P);
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, sizeof(staged) + blk);
-    if (!scr) die("scratch");
-    cudaStream_t st = dev->stream;
-    if (cudaMemcpyAsync(scr, staged, sizeof(staged), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d edges");
+    B200HostCall call("hevc intra prediction", nullptr, sizeof(staged) + blk);
+    uint8_t *scr = call.scratch;
+    cudaStream_t st = call.stream;
+    call.check(cudaMemcpyAsync(scr, staged, sizeof(staged), cudaMemcpyHostToDevice, st), "h2d edges");
     P *sdst = reinterpret_cast<P *>(scr + sizeof(staged));
     hevc_pred_member_kernel<P><<<1, 32, (2 * kArr + kRef) * sizeof(int), st>>>((const int *)scr, sdst, size, log2, mode, c_idx == 0, D);
     B200_LAUNCHED();
-    if (cudaGetLastError() != cudaSuccess) die("launch");
-    if (b200_d2h_rows(dst, stride * (ptrdiff_t)sizeof(P), sdst, (size_t)size * sizeof(P), (size_t)size * sizeof(P), (size_t)size, st) != cudaSuccess) die("d2h block");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.launched();
+    call.check(b200_d2h_rows(dst, stride * (ptrdiff_t)sizeof(P), sdst, (size_t)size * sizeof(P), (size_t)size * sizeof(P), (size_t)size, st), "d2h block");
+    call.sync();
 }
 
 template <int D, int L2>
@@ -226,9 +216,7 @@ B200_API int b200_hevc_intra_pred_batch_device(B200Device *dev, int bit_depth, u
         b200_set_error("hevc intra batch: NULL pix / ops, pix not aligned to a sample or ops not aligned to 16 bytes");
         return B200_EINVAL;
     }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     IntraArgs a;
     a.pix = pix; a.stride = (long long)stride; a.ops = ops; a.nops = nops;
     PredPlane &g = a.g;

@@ -228,12 +228,6 @@ SaoArgs plane_args(int depth, uint8_t *dst, long long dstride, const uint8_t *sr
     return a;
 }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: hevc sao failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 // ---- band and edge members (host pointers): the block is staged into a scratch plane and run through the plane kernel with
 // 64-sample CTBs, so the filter arithmetic exists once.  Band: a w x h plane, one BAND CTB.  Edge: a (w + 2) x (h + 2) plane with
 // the block at (1, 1), every CTB EDGE with no flags: the block's samples are never on a CTB's picture border, so all of them take
@@ -246,13 +240,9 @@ void member_run(int depth, bool band, uint8_t *dst, ptrdiff_t dst_stride, const 
 {
     const int bps = depth > 8 ? 2 : 1;
     const size_t pitch = (size_t)kPitch * bps, plane = pitch * kPitch;
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
-    B200_LOCK_DEVICE(dev);            // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, kRec + 2 * plane);
-    if (!scr) die("scratch");
-    cudaStream_t st = dev->stream;
+    B200HostCall call("hevc sao", nullptr, kRec + 2 * plane);
+    uint8_t *scr = call.scratch;
+    cudaStream_t st = call.stream;
     uint8_t *ssrc = scr + kRec, *sdst = scr + kRec + plane;
     B200HevcSaoCtb rec[4];
     memset(rec, 0, sizeof(rec));
@@ -261,20 +251,19 @@ void member_run(int depth, bool band, uint8_t *dst, ptrdiff_t dst_stride, const 
         rec[k].type = band ? B200_HEVC_SAO_BAND : B200_HEVC_SAO_EDGE;
         rec[k].cls = (uint8_t)(band ? cls & 31 : cls);
     }
-    if (cudaMemcpyAsync(scr, rec, sizeof(rec), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d records");
+    call.check(cudaMemcpyAsync(scr, rec, sizeof(rec), cudaMemcpyHostToDevice, st), "h2d records");
     const int pw = band ? w : w + 2, ph = band ? h : h + 2, o = band ? 0 : 1;
     // rows / columns of the host block staged: edge classes read only their neighbours' ring
     const int r0 = band || cls == 0 ? 0 : -1, r1 = band || cls == 0 ? h : h + 1;
     const int c0 = band || cls == 1 ? 0 : -1, c1 = band || cls == 1 ? w : w + 1;
-    if (b200_h2d_rows(ssrc + (size_t)(r0 + o) * pitch + (size_t)(c0 + o) * bps, pitch, src + (ptrdiff_t)r0 * src_stride + (ptrdiff_t)c0 * bps,
-                      src_stride, (size_t)(c1 - c0) * bps, (size_t)(r1 - r0), st) != cudaSuccess)
-        die("h2d block");
+    call.check(b200_h2d_rows(ssrc + (size_t)(r0 + o) * pitch + (size_t)(c0 + o) * bps, pitch, src + (ptrdiff_t)r0 * src_stride + (ptrdiff_t)c0 * bps,
+                             src_stride, (size_t)(c1 - c0) * bps, (size_t)(r1 - r0), st),
+               "h2d block");
     const SaoArgs a = plane_args(depth, sdst, (long long)pitch, ssrc, (long long)pitch, pw, ph, 6, 0, 0, (const B200HevcSaoCtb *)scr, 2,
                                  nullptr, 0, 2);
-    if (launch(a, st) != cudaSuccess) die("launch");
-    if (b200_d2h_rows(dst, dst_stride, sdst + (size_t)o * pitch + (size_t)o * bps, pitch, (size_t)w * bps, (size_t)h, st) != cudaSuccess)
-        die("d2h block");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.check(launch(a, st), "launch");
+    call.check(b200_d2h_rows(dst, dst_stride, sdst + (size_t)o * pitch + (size_t)o * bps, pitch, (size_t)w * bps, (size_t)h, st), "d2h block");
+    call.sync();
 }
 
 template <int D>
@@ -383,9 +372,7 @@ B200_API int b200_hevc_sao_plane_device(B200Device *dev, int bit_depth, uint8_t 
     const uintptr_t d0 = (uintptr_t)dst, d1 = d0 + (uintptr_t)((height - 1) * (int64_t)dst_stride + row);
     const uintptr_t s0 = (uintptr_t)src, s1 = s0 + (uintptr_t)((height - 1) * (int64_t)src_stride + row);
     if (d0 < s1 && s0 < d1) { b200_set_error("hevc sao plane: dst and src overlap (the entry works out of place)"); return B200_EINVAL; }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     const SaoArgs a = plane_args(bit_depth, dst, (long long)dst_stride, src, (long long)src_stride, width, height, log2_ctb_size, hshift,
                                  vshift, ctb, (long long)ctb_stride, keep, (long long)keep_stride, log2_min_pu_size);
     B200_CUDA_OK(launch(a, dev->stream));

@@ -545,7 +545,7 @@ B200_API int b200_mpv_unquant_idct_mb420_device(B200Device *dev, int variant, co
     FusedUnquant U;
     if (!mpv_unquant_params(p, &U)) { b200_set_error("b200_mpv_unquant_idct: permutated[] is not a permutation of 0..63"); return B200_EINVAL; }
     U.qscale = qscale; U.last_index = last_index;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     Mb420Geom g{};
     g.mb_w = mb_w; g.mb_h = mb_h;
     for (int i = 0; i < 3; i++) { g.plane[i] = planes[i]; g.linesize[i] = linesize[i]; g.frame_stride[i] = frame_stride[i]; }
@@ -567,7 +567,7 @@ B200_API int b200_idct_batch_device(B200Device *dev, int kind, int16_t *blocks, 
     if (!dev || !blocks || nblocks < 0) return B200_EINVAL;
     if (kind != B200_IDCT && (!dest || !dest_off)) return B200_EINVAL;
     if (((uintptr_t)blocks) & 15) { b200_set_error("idct: coefficient blocks must be 16-byte aligned"); return B200_EINVAL; }
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     Mb420Geom g{};
     return dispatch(dev->stream, kind, false, blocks, blocks, nblocks, dest, dest_off, line_size, uniform_line_size, g);
 }
@@ -578,7 +578,7 @@ B200_API int b200_idct_mb420_device(B200Device *dev, int kind, const int16_t *bl
     if (!dev || !blocks || !planes || !linesize || !frame_stride || mb_w <= 0 || mb_h <= 0 || nframes < 0) return B200_EINVAL;
     if (kind != B200_IDCT_PUT && kind != B200_IDCT_ADD) return B200_EINVAL;
     if (((uintptr_t)blocks) & 15) return B200_EINVAL;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     Mb420Geom g{};
     g.mb_w = mb_w; g.mb_h = mb_h;
     for (int i = 0; i < 3; i++) { g.plane[i] = planes[i]; g.linesize[i] = linesize[i]; g.frame_stride[i] = frame_stride[i]; }
@@ -640,65 +640,43 @@ B200_API int b200_idct_mb420_host(B200Device *dev, int kind, const int16_t *bloc
 // batched entry points above are the fast path.
 namespace {
 
-int one_block(int kind, uint8_t *dest, ptrdiff_t line_size, int16_t *block)
+void one_block(const char *feature, int kind, uint8_t *dest, ptrdiff_t line_size, int16_t *block)
 {
-    B200Device *dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) return B200_EEXTERNAL;
-    B200_LOCK_DEVICE(dev);      // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, 256);
-    if (!scr) return B200_ENOMEM;
-    int16_t *dblk = (int16_t *)scr;
-    uint8_t *dpix = scr + 128;               // packed 8x8, line size 8
-    int64_t *doff = (int64_t *)(scr + 192);
-    cudaStream_t st = dev->stream;
-    B200_CUDA_OK(cudaMemcpyAsync(dblk, block, 128, cudaMemcpyHostToDevice, st));
-    if (kind == B200_IDCT_ADD)
-        B200_CUDA_OK(b200_h2d_rows(dpix, 8, dest, line_size, 8, 8, st));
-    B200_CUDA_OK(cudaMemsetAsync(doff, 0, 8, st));
+    B200HostCall call(feature, nullptr, 256);
+    int16_t *dblk = (int16_t *)call.scratch;
+    uint8_t *dpix = call.scratch + 128;      // packed 8x8, line size 8
+    int64_t *doff = (int64_t *)(call.scratch + 192);
+    cudaStream_t st = call.stream;
+    call.check(cudaMemcpyAsync(dblk, block, 128, cudaMemcpyHostToDevice, st), "h2d block");
+    if (kind == B200_IDCT_ADD) call.check(b200_h2d_rows(dpix, 8, dest, line_size, 8, 8, st), "h2d dest");
+    call.check(cudaMemsetAsync(doff, 0, 8, st), "memset");
     Mb420Geom g{};
-    int ret = dispatch(st, kind, false, dblk, dblk, 1, dpix, doff, nullptr, 8, g);
-    if (ret < 0) return ret;
-    if (kind == B200_IDCT)
-        B200_CUDA_OK(cudaMemcpyAsync(block, dblk, 128, cudaMemcpyDeviceToHost, st));
-    else
-        B200_CUDA_OK(b200_d2h_rows(dest, line_size, dpix, 8, 8, 8, st));
-    B200_CUDA_OK(cudaStreamSynchronize(st));
-    return 0;
+    call.launched(dispatch(st, kind, false, dblk, dblk, 1, dpix, doff, nullptr, 8, g));
+    if (kind == B200_IDCT) call.check(cudaMemcpyAsync(block, dblk, 128, cudaMemcpyDeviceToHost, st), "d2h block");
+    else call.check(b200_d2h_rows(dest, line_size, dpix, 8, 8, 8, st), "d2h dest");
+    call.sync();
 }
 
-int one_clamp(int kind, const int16_t *block, uint8_t *pixels, ptrdiff_t line_size)
+void one_clamp(const char *feature, int kind, const int16_t *block, uint8_t *pixels, ptrdiff_t line_size)
 {
-    B200Device *dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) return B200_EEXTERNAL;
-    B200_LOCK_DEVICE(dev);      // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, 256);
-    if (!scr) return B200_ENOMEM;
-    cudaStream_t st = dev->stream;
-    B200_CUDA_OK(cudaMemcpyAsync(scr, block, 128, cudaMemcpyHostToDevice, st));
-    if (kind == 2) B200_CUDA_OK(b200_h2d_rows(scr + 128, 8, pixels, line_size, 8, 8, st));
+    B200HostCall call(feature, nullptr, 256);
+    uint8_t *scr = call.scratch;
+    cudaStream_t st = call.stream;
+    call.check(cudaMemcpyAsync(scr, block, 128, cudaMemcpyHostToDevice, st), "h2d block");
+    if (kind == 2) call.check(b200_h2d_rows(scr + 128, 8, pixels, line_size, 8, 8, st), "h2d pixels");
     pixels_clamped_kernel<<<1, 64, 0, st>>>(kind, (const int16_t *)scr, scr + 128);
     B200_LAUNCHED();
-    B200_CUDA_OK(b200_d2h_rows(pixels, line_size, scr + 128, 8, 8, 8, st));
-    B200_CUDA_OK(cudaStreamSynchronize(st));
-    return 0;
+    call.launched();
+    call.check(b200_d2h_rows(pixels, line_size, scr + 128, 8, 8, 8, st), "d2h pixels");
+    call.sync();
 }
 
-void die_if(int ret, const char *what)
-{
-    if (ret < 0) {   // the reference's entry points return void: a silent wrong picture is worse than stopping
-        fprintf(stderr, "libb200dsp: %s failed (%d): %s\n", what, ret, b200_last_error());
-        abort();
-    }
-}
-
-void tab_idct(int16_t *block) { die_if(one_block(B200_IDCT, nullptr, 0, block), "idct"); }
-void tab_idct_put(uint8_t *dest, ptrdiff_t ls, int16_t *block) { die_if(one_block(B200_IDCT_PUT, dest, ls, block), "idct_put"); }
-void tab_idct_add(uint8_t *dest, ptrdiff_t ls, int16_t *block) { die_if(one_block(B200_IDCT_ADD, dest, ls, block), "idct_add"); }
-void tab_put_clamped(const int16_t *b, uint8_t *p, ptrdiff_t ls) { die_if(one_clamp(0, b, p, ls), "put_pixels_clamped"); }
-void tab_put_signed_clamped(const int16_t *b, uint8_t *p, ptrdiff_t ls) { die_if(one_clamp(1, b, p, ls), "put_signed_pixels_clamped"); }
-void tab_add_clamped(const int16_t *b, uint8_t *p, ptrdiff_t ls) { die_if(one_clamp(2, b, p, ls), "add_pixels_clamped"); }
+void tab_idct(int16_t *block) { one_block("idct", B200_IDCT, nullptr, 0, block); }
+void tab_idct_put(uint8_t *dest, ptrdiff_t ls, int16_t *block) { one_block("idct_put", B200_IDCT_PUT, dest, ls, block); }
+void tab_idct_add(uint8_t *dest, ptrdiff_t ls, int16_t *block) { one_block("idct_add", B200_IDCT_ADD, dest, ls, block); }
+void tab_put_clamped(const int16_t *b, uint8_t *p, ptrdiff_t ls) { one_clamp("put_pixels_clamped", 0, b, p, ls); }
+void tab_put_signed_clamped(const int16_t *b, uint8_t *p, ptrdiff_t ls) { one_clamp("put_signed_pixels_clamped", 1, b, p, ls); }
+void tab_add_clamped(const int16_t *b, uint8_t *p, ptrdiff_t ls) { one_clamp("add_pixels_clamped", 2, b, p, ls); }
 
 } // namespace
 

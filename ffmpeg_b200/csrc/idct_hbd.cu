@@ -138,38 +138,31 @@ int launch(cudaStream_t st, int kind, int16_t *blocks, long long n, uint8_t *des
     return 0;
 }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: high-bit-depth idct failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
+constexpr const char *kFeature = "high-bit-depth idct";
 
 // drop-in: one block through the device (host pointers); put / add leave the caller's coefficient block as it was (the
 // reference uses it as scratch; no caller reads it afterwards)
 template <int DEPTH>
 void host_op(int kind, uint8_t *dest, ptrdiff_t line_size, int16_t *block)
 {
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (kind != B200_IDCT && ((line_size > -16 && line_size < 16) || (line_size & 1))) die("|line_size| must be even and >= 16 bytes");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
-    B200_LOCK_DEVICE(dev);      // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, 128 + 8 * 16 + 16);
-    if (!scr) die("scratch");
+    if (kind != B200_IDCT && ((line_size > -16 && line_size < 16) || (line_size & 1)))
+        B200HostCall::fail(kFeature, "|line_size| must be even and >= 16 bytes");
+    B200HostCall call(kFeature, nullptr, 128 + 8 * 16 + 16);
+    uint8_t *scr = call.scratch;
     int16_t *dblk = (int16_t *)scr;
     uint8_t *ddst = scr + 128;
     int64_t *doff = (int64_t *)(scr + 128 + 128);
-    cudaStream_t st = dev->stream;
+    cudaStream_t st = call.stream;
     const int64_t zero = 0;
-    if (cudaMemcpyAsync(dblk, block, 128, cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d block");
+    call.check(cudaMemcpyAsync(dblk, block, 128, cudaMemcpyHostToDevice, st), "h2d block");
     if (kind != B200_IDCT) {
-        if (kind == B200_IDCT_ADD && b200_h2d_rows(ddst, 16, dest, line_size, 16, 8, st) != cudaSuccess) die("h2d dest");
-        if (cudaMemcpyAsync(doff, &zero, 8, cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d off");
+        if (kind == B200_IDCT_ADD) call.check(b200_h2d_rows(ddst, 16, dest, line_size, 16, 8, st), "h2d dest");
+        call.check(cudaMemcpyAsync(doff, &zero, 8, cudaMemcpyHostToDevice, st), "h2d off");
     }
-    if (launch<DEPTH>(st, kind, dblk, 1, ddst, doff, nullptr, 16) < 0 || cudaGetLastError() != cudaSuccess) die("launch");
-    if (kind == B200_IDCT) { if (cudaMemcpyAsync(block, dblk, 128, cudaMemcpyDeviceToHost, st) != cudaSuccess) die("d2h block"); }
-    else if (b200_d2h_rows(dest, line_size, ddst, 16, 16, 8, st) != cudaSuccess) die("d2h dest");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.launched(launch<DEPTH>(st, kind, dblk, 1, ddst, doff, nullptr, 16));
+    if (kind == B200_IDCT) call.check(cudaMemcpyAsync(block, dblk, 128, cudaMemcpyDeviceToHost, st), "d2h block");
+    else call.check(b200_d2h_rows(dest, line_size, ddst, 16, 16, 8, st), "d2h dest");
+    call.sync();
 }
 
 template <int DEPTH> void tab_idct(int16_t *b) { host_op<DEPTH>(B200_IDCT, nullptr, 0, b); }
@@ -194,15 +187,13 @@ B200_API int b200_idctdsp_init_hbd(B200IDCTDSPContext *c, int idct_algo, int bit
 B200_API int b200_idct_hbd_batch_device(B200Device *dev, int depth, int kind, int16_t *blocks, int64_t nblocks, uint8_t *dest,
                                         const int64_t *dest_off, const int32_t *line_size, int uniform_line_size)
 {
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
+    if (int r = b200_use_device(dev)) return r;
     if (depth == 9) depth = 10;
     if ((depth != 10 && depth != 12) || kind < B200_IDCT || kind > B200_IDCT_ADD || nblocks < 0) return B200_EINVAL;
     if (nblocks == 0) return 0;
     if (!blocks || (reinterpret_cast<uintptr_t>(blocks) & 15)) return B200_EINVAL;
     if (kind != B200_IDCT && (!dest || !dest_off || (reinterpret_cast<uintptr_t>(dest) & 1) || (!line_size && (uniform_line_size & 1))))
         return B200_EINVAL;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
     const int ret = depth == 10 ? launch<10>(dev->stream, kind, blocks, nblocks, dest, dest_off, line_size, uniform_line_size)
                                 : launch<12>(dev->stream, kind, blocks, nblocks, dest, dest_off, line_size, uniform_line_size);
     if (ret < 0) return ret;
@@ -227,24 +218,20 @@ int launch_prores(cudaStream_t st, int bits, const int16_t *blocks, long long n,
 template <int BITS>
 void prores_tab_put(uint16_t *out, ptrdiff_t linesize, int16_t *block, const int16_t *qmat)
 {
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if ((linesize > -16 && linesize < 16) || (linesize & 1)) die("|line size| must be even and >= 16 bytes");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
-    B200_LOCK_DEVICE(dev);      // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, 128 + 128 + 128 + 16);
-    if (!scr) die("scratch");
+    if ((linesize > -16 && linesize < 16) || (linesize & 1)) B200HostCall::fail(kFeature, "|line size| must be even and >= 16 bytes");
+    B200HostCall call(kFeature, nullptr, 128 + 128 + 128 + 16);
+    uint8_t *scr = call.scratch;
     int16_t *dblk = (int16_t *)scr, *dq = (int16_t *)(scr + 128);
     uint8_t *ddst = scr + 256;
     int64_t *doff = (int64_t *)(scr + 384);
-    cudaStream_t st = dev->stream;
+    cudaStream_t st = call.stream;
     const int64_t zero = 0;
-    if (cudaMemcpyAsync(dblk, block, 128, cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d block");
-    if (cudaMemcpyAsync(dq, qmat, 128, cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d qmat");
-    if (cudaMemcpyAsync(doff, &zero, 8, cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d off");
-    if (launch_prores(st, BITS, dblk, 1, dq, ddst, doff, nullptr, 16) < 0 || cudaGetLastError() != cudaSuccess) die("launch");
-    if (b200_d2h_rows(out, linesize, ddst, 16, 16, 8, st) != cudaSuccess) die("d2h");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.check(cudaMemcpyAsync(dblk, block, 128, cudaMemcpyHostToDevice, st), "h2d block");
+    call.check(cudaMemcpyAsync(dq, qmat, 128, cudaMemcpyHostToDevice, st), "h2d qmat");
+    call.check(cudaMemcpyAsync(doff, &zero, 8, cudaMemcpyHostToDevice, st), "h2d off");
+    call.launched(launch_prores(st, BITS, dblk, 1, dq, ddst, doff, nullptr, 16));
+    call.check(b200_d2h_rows(out, linesize, ddst, 16, 16, 8, st), "d2h");
+    call.sync();
 }
 
 } // namespace
@@ -265,12 +252,10 @@ B200_API int b200_proresdsp_init(B200ProresDSPContext *c, int bits_per_raw_sampl
 B200_API int b200_prores_idct_put_batch_device(B200Device *dev, int bits, const int16_t *blocks, int64_t nblocks, const int16_t *qmat,
                                                uint8_t *dest, const int64_t *dest_off, const int32_t *line_size, int uniform_line_size)
 {
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
+    if (int r = b200_use_device(dev)) return r;
     if ((bits != 10 && bits != 12) || nblocks < 0) return B200_EINVAL;
     if (nblocks == 0) return 0;
     if (!blocks || !qmat || !dest || !dest_off || (reinterpret_cast<uintptr_t>(dest) & 1) || (!line_size && (uniform_line_size & 1))) return B200_EINVAL;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
     const int ret = launch_prores(dev->stream, bits, blocks, nblocks, qmat, dest, dest_off, line_size, uniform_line_size);
     if (ret < 0) return ret;
     B200_CUDA_OK(cudaGetLastError());

@@ -457,7 +457,7 @@ B200_API int b200_me_cmp_batch_device(B200Device *dev, int fn, int idx, const ui
     int ret = decode(fn, idx, &w, &mode);
     if (ret < 0) return ret;
     if (n == 0) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     const long long blocks = (n + 7) / 8;
     if (blocks > 0x7fffffffLL) return B200_EINVAL;
     if (fn >= B200_MECMP_DCT_SAD)                                 // 8x8 blocks like hadamard8_diff: two of them, four when h == 16
@@ -483,7 +483,7 @@ B200_API int b200_me_esa_device(B200Device *dev, const uint8_t *cur, const uint8
     if (b_w == 0 || b_h == 0) return B200_EINVAL;                 // vf_mestimate.c:93-94
     if (b_h > 65535) return B200_ENOSYS;
     if (nframes == 0) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     unsigned long long *cost = reinterpret_cast<unsigned long long *>(out_cost);
     switch (mb_size) {
     case 4:  return launch_esa<4>(dev->stream, cur, ref, linesize, frame_stride, b_w, b_h, nframes, search_param, out_mv, cost);
@@ -545,33 +545,29 @@ namespace {
 
 int host_cmp(int fn, int idx, const uint8_t *blk1, const uint8_t *blk2, ptrdiff_t stride, int h)
 {
-    auto fail = [](const char *what) { fprintf(stderr, "libb200dsp: me_cmp failed: %s (%s)\n", what, b200_last_error()); abort(); };
-    B200Device *dev = b200_default_device();
-    if (!dev) fail("no device");
     int w, mode;
-    if (decode(fn, idx, &w, &mode) < 0) fail("bad index");
+    if (decode(fn, idx, &w, &mode) < 0) B200HostCall::fail("me_cmp", "bad index");
     if (fn == B200_MECMP_HADAMARD8 || fn >= B200_MECMP_DCT_SAD) h = (w == 16 && h == 16) ? 16 : 8;   // the reference reads 8 rows unless 16 wide with h == 16
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) fail("cudaSetDevice");
     const int cw = w + 1, ch = h + 1;                             // x2/y2/xy2 read one extra column / row of blk2
     const size_t pitch = 32;
-    B200_LOCK_DEVICE(dev);      // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, 2 * pitch * (ch + 1) + 64);
-    if (!scr) fail("scratch");
-    uint8_t *d1 = scr, *d2 = scr + pitch * (ch + 1);
-    int64_t *offs = (int64_t *)(scr + 2 * pitch * (ch + 1));
+    B200HostCall call("me_cmp", nullptr, 2 * pitch * (ch + 1) + 64);
+    uint8_t *d1 = call.scratch, *d2 = call.scratch + pitch * (ch + 1);
+    int64_t *offs = (int64_t *)(call.scratch + 2 * pitch * (ch + 1));
     int32_t *dout = (int32_t *)(offs + 2);
-    cudaStream_t st = dev->stream;
-    if (b200_h2d_rows(d1, pitch, blk1, stride, w, h, st) != cudaSuccess) fail("h2d");      // negative strides (flipped frames) are fine
+    cudaStream_t st = call.stream;
+    call.check(b200_h2d_rows(d1, pitch, blk1, stride, w, h, st), "h2d");      // negative strides (flipped frames) are fine
     const int bw = fn == B200_MECMP_PIX_ABS && (mode & 1) ? cw : w, bh = fn == B200_MECMP_PIX_ABS && (mode & 2) ? ch : h;
-    if (b200_h2d_rows(d2, pitch, blk2, stride, bw, bh, st) != cudaSuccess) fail("h2d");
-    if (cudaMemsetAsync(offs, 0, 16, st) != cudaSuccess) fail("memset");
+    call.check(b200_h2d_rows(d2, pitch, blk2, stride, bw, bh, st), "h2d");
+    call.check(cudaMemsetAsync(offs, 0, 16, st), "memset");
     if (fn >= B200_MECMP_DCT_SAD) mecmp_dct_launch(st, 1, 32, fn, w, h, d1, d2, (long long)pitch, offs, offs + 1, 1, dout);
     else if (fn == B200_MECMP_HADAMARD8) me_satd_kernel<<<1, 32, 0, st>>>(w == 8 ? 1 : h == 16 ? 4 : 2, d1, d2, (long long)pitch, offs, offs + 1, 1, dout, mode);
     else if (fn >= B200_MECMP_VSAD) me_cmp2_kernel<<<1, 32, 0, st>>>(fn, w, mode, g_nsse_weight.load(), d1, d2, (long long)pitch, h, offs, offs + 1, 1, dout);
     else me_cmp_kernel<<<1, 32, 0, st>>>(fn, w, mode, d1, d2, (long long)pitch, h, offs, offs + 1, 1, dout);
     B200_LAUNCHED();
+    call.launched();
     int32_t res = 0;
-    if (cudaMemcpyAsync(&res, dout, 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) fail("d2h");
+    call.check(cudaMemcpyAsync(&res, dout, 4, cudaMemcpyDeviceToHost, st), "d2h");
+    call.sync();
     return res;
 }
 
@@ -580,19 +576,15 @@ int tab_fn(void *, const uint8_t *a, const uint8_t *b, ptrdiff_t stride, int h) 
 
 int host_sum_abs_dctelem(const int16_t *block)
 {
-    auto fail = [](const char *what) { fprintf(stderr, "libb200dsp: sum_abs_dctelem failed: %s (%s)\n", what, b200_last_error()); abort(); };
-    B200Device *dev = b200_default_device();
-    if (!dev) fail("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) fail("cudaSetDevice");
-    B200_LOCK_DEVICE(dev);
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, 256);
-    if (!scr) fail("scratch");
-    cudaStream_t st = dev->stream;
-    if (cudaMemcpyAsync(scr, block, 128, cudaMemcpyHostToDevice, st) != cudaSuccess) fail("h2d");
-    sum_abs_dctelem_kernel<<<1, 32, 0, st>>>((const int16_t *)scr, 1, (int32_t *)(scr + 128));
+    B200HostCall call("sum_abs_dctelem", nullptr, 256);
+    cudaStream_t st = call.stream;
+    call.check(cudaMemcpyAsync(call.scratch, block, 128, cudaMemcpyHostToDevice, st), "h2d");
+    sum_abs_dctelem_kernel<<<1, 32, 0, st>>>((const int16_t *)call.scratch, 1, (int32_t *)(call.scratch + 128));
     B200_LAUNCHED();
+    call.launched();
     int32_t res = 0;
-    if (cudaMemcpyAsync(&res, scr + 128, 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) fail("d2h");
+    call.check(cudaMemcpyAsync(&res, call.scratch + 128, 4, cudaMemcpyDeviceToHost, st), "d2h");
+    call.sync();
     return res;
 }
 
@@ -631,7 +623,7 @@ B200_API int b200_sum_abs_dctelem_batch_device(B200Device *dev, const int16_t *b
 {
     if (!dev || !blocks || !out || n < 0 || ((uintptr_t)blocks & 3)) return B200_EINVAL;
     if (n == 0) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     const long long ctas = (n + 7) / 8;
     if (ctas > 0x7fffffffLL) return B200_EINVAL;
     sum_abs_dctelem_kernel<<<(unsigned)ctas, 256, 0, dev->stream>>>(blocks, n, out);

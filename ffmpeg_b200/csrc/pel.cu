@@ -454,46 +454,37 @@ int chroma_launch(cudaStream_t st, int sms, int64_t n, const uint8_t *op, const 
     return 0;
 }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: motion compensation failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 enum HostKind { HOST_QPEL, HOST_HPEL, HOST_CHROMA };
+constexpr const char *kFeature = "motion compensation";
 
 // one block through the device for the drop-in tables.  Only the source rectangle the reference function itself reads is
 // copied from the caller's buffer (bx/ax columns left/right, by/ay rows above/below the block).
 void host_op(HostKind kind, int o, int h, int w, uint8_t *dst, const uint8_t *src, ptrdiff_t stride,
              int bx, int ax, int by, int ay, int fxy = 0)
 {
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
     const int before = kind == HOST_QPEL ? 2 : 0, after = kind == HOST_QPEL ? 3 : 1;   // the window the kernels may touch
     const int sh = h + before + after;
     const size_t pitch = 32;
-    B200_LOCK_DEVICE(dev);      // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, pitch * (sh + h) + 256);
-    if (!scr) die("scratch");
+    B200HostCall call(kFeature, nullptr, pitch * (sh + h) + 256);
+    uint8_t *scr = call.scratch;
     uint8_t *dsrc = scr, *ddst = scr + pitch * sh;
     uint8_t *meta = scr + pitch * (sh + h);           // op, h, offsets
-    cudaStream_t st = dev->stream;
-    if (b200_h2d_rows(dsrc + (before - by) * pitch + (before - bx), pitch, src - by * stride - bx, stride,
-                      w + bx + ax, h + by + ay, st) != cudaSuccess) die("h2d src");
-    if (b200_h2d_rows(ddst, pitch, dst, stride, w, h, st) != cudaSuccess) die("h2d dst");
+    cudaStream_t st = call.stream;
+    call.check(b200_h2d_rows(dsrc + (before - by) * pitch + (before - bx), pitch, src - by * stride - bx, stride, w + bx + ax, h + by + ay, st),
+               "h2d src");
+    call.check(b200_h2d_rows(ddst, pitch, dst, stride, w, h, st), "h2d dst");
     struct { int64_t doff, soff; uint8_t op, h, xy; } m = { 0, (int64_t)(before * pitch + before), (uint8_t)o, (uint8_t)h, (uint8_t)fxy };
-    if (cudaMemcpyAsync(meta, &m, sizeof(m), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d meta");
+    call.check(cudaMemcpyAsync(meta, &m, sizeof(m), cudaMemcpyHostToDevice, st), "h2d meta");
     const int64_t *doff = (const int64_t *)meta, *soff = doff + 1;
     const uint8_t *dop = meta + 16, *dh = meta + 17, *dxy = meta + 18;
     // dst and src live in one buffer with the same pitch, like the reference's single stride
     int err = 0;
     if (kind == HOST_QPEL)        err = qpel_launch(st, 1, dop, ddst, doff, dsrc, soff, pitch);
-    else if (kind == HOST_CHROMA) err = chroma_launch(st, dev->sm_count, 1, dop, dh, dxy, ddst, doff, dsrc, soff, pitch);
+    else if (kind == HOST_CHROMA) err = chroma_launch(st, call.dev->sm_count, 1, dop, dh, dxy, ddst, doff, dsrc, soff, pitch);
     else { hpel_kernel<<<1, 32 * WARPS, 0, st>>>(1, dop, dh, ddst, doff, dsrc, soff, (long long)pitch); B200_LAUNCHED(); }
-    if (err) die("launch");
-    if (b200_d2h_rows(dst, stride, ddst, pitch, w, h, st) != cudaSuccess) die("d2h");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.launched(err);
+    call.check(b200_d2h_rows(dst, stride, ddst, pitch, w, h, st), "d2h");
+    call.sync();
 }
 
 template <int AVG, int SIDX, int POS>
@@ -510,7 +501,7 @@ void hpel_tab(uint8_t *block, const uint8_t *pixels, ptrdiff_t line_size, int h)
 template <int AVG, int IDX>
 void chroma_tab(uint8_t *dst, const uint8_t *src, ptrdiff_t stride, int h, int x, int y)
 {
-    if ((unsigned)x > 7 || (unsigned)y > 7) die("h264chroma: x, y must be in 0..7");     // av_assert2 in the reference
+    if ((unsigned)x > 7 || (unsigned)y > 7) B200HostCall::fail(kFeature, "h264chroma: x, y must be in 0..7");     // av_assert2 in the reference
     host_op(HOST_CHROMA, AVG | (IDX << 1), h, 8 >> IDX, dst, src, stride, 0, x ? 1 : 0, 0, y ? 1 : 0, x | (y << 3));
 }
 
@@ -571,7 +562,7 @@ B200_API int b200_h264chroma_batch_device(B200Device *dev, int64_t n, const uint
 {
     if (!dev || n < 0 || !op || !h || !xy || !dst || !dst_off || !src || !src_off) return B200_EINVAL;
     if (n == 0) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     return chroma_launch(dev->stream, dev->sm_count, n, op, h, xy, dst, dst_off, src, src_off, stride);
 }
 
@@ -580,7 +571,7 @@ B200_API int b200_h264qpel_batch_device(B200Device *dev, int64_t n, const uint8_
 {
     if (!dev || n < 0 || !op || !dst || !dst_off || !src || !src_off) return B200_EINVAL;
     if (n == 0) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     return qpel_launch(dev->stream, n, op, dst, dst_off, src, src_off, stride);
 }
 
@@ -643,7 +634,7 @@ B200_API int b200_hpel_batch_device(B200Device *dev, int64_t n, const uint8_t *o
 {
     if (!dev || n < 0 || !op || !h || !dst || !dst_off || !src || !src_off) return B200_EINVAL;
     if (n == 0) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     const long long blocks = (n + WARPS - 1) / WARPS;
     if (blocks > 0x7fffffffLL) return B200_EINVAL;
     hpel_kernel<<<(unsigned)blocks, 32 * WARPS, 0, dev->stream>>>(n, op, h, dst, dst_off, src, src_off, stride);

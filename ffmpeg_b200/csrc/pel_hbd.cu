@@ -129,11 +129,7 @@ int chroma_hbd_launch(cudaStream_t st, long long n, const uint8_t *op, const uin
     return 0;
 }
 
-void hbd_die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: high-bit-depth motion compensation failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
+constexpr const char *kFeature = "high-bit-depth motion compensation";
 
 // one block through the device for the drop-in tables: only the rectangle the reference function itself reads is copied
 template <int DEPTH, int AVG, int SIDX, int POS>
@@ -141,24 +137,20 @@ void qpel_hbd_tab(uint8_t *dst, const uint8_t *src, ptrdiff_t stride)
 {
     constexpr int X = POS & 3, Y = POS >> 2, size = 16 >> SIDX;
     constexpr int bx = X ? 2 : 0, ax = X ? 3 : 0, by = Y ? 2 : 0, ay = Y ? 3 : 0;
-    B200Device *dev = b200_default_device();
-    if (!dev) hbd_die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) hbd_die("cudaSetDevice");
     const size_t pitch = 64;                                       // 21 samples of 2 bytes
     const int sh = size + 5;
-    B200_LOCK_DEVICE(dev);
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, pitch * (sh + size) + 256);
-    if (!scr) hbd_die("scratch");
+    B200HostCall call(kFeature, nullptr, pitch * (sh + size) + 256);
+    uint8_t *scr = call.scratch;
     uint8_t *dsrc = scr, *ddst = scr + pitch * sh, *meta = scr + pitch * (sh + size);
-    cudaStream_t st = dev->stream;
-    if (b200_h2d_rows(dsrc + (2 - by) * pitch + (2 - bx) * 2, pitch, src - by * stride - bx * 2, stride, (size + bx + ax) * 2, size + by + ay, st) != cudaSuccess)
-        hbd_die("h2d src");
-    if (b200_h2d_rows(ddst, pitch, dst, stride, size * 2, size, st) != cudaSuccess) hbd_die("h2d dst");
+    cudaStream_t st = call.stream;
+    call.check(b200_h2d_rows(dsrc + (2 - by) * pitch + (2 - bx) * 2, pitch, src - by * stride - bx * 2, stride, (size + bx + ax) * 2, size + by + ay, st),
+               "h2d src");
+    call.check(b200_h2d_rows(ddst, pitch, dst, stride, size * 2, size, st), "h2d dst");
     struct { long long doff, soff; uint8_t op; } m = { 0, (long long)(2 * pitch + 4), (uint8_t)(AVG | (SIDX << 1) | (POS << 3)) };
-    if (cudaMemcpyAsync(meta, &m, sizeof(m), cudaMemcpyHostToDevice, st) != cudaSuccess) hbd_die("h2d meta");
-    if (hbd_launch(st, DEPTH, 1, meta + 16, ddst, (const long long *)meta, dsrc, (const long long *)meta + 1, (long long)pitch) < 0) hbd_die("launch");
-    if (b200_d2h_rows(dst, stride, ddst, pitch, size * 2, size, st) != cudaSuccess) hbd_die("d2h");
-    if (cudaStreamSynchronize(st) != cudaSuccess) hbd_die("sync");
+    call.check(cudaMemcpyAsync(meta, &m, sizeof(m), cudaMemcpyHostToDevice, st), "h2d meta");
+    call.launched(hbd_launch(st, DEPTH, 1, meta + 16, ddst, (const long long *)meta, dsrc, (const long long *)meta + 1, (long long)pitch));
+    call.check(b200_d2h_rows(dst, stride, ddst, pitch, size * 2, size, st), "d2h");
+    call.sync();
 }
 
 template <int DEPTH, int AVG, int SIDX>
@@ -182,26 +174,22 @@ void fill_ctx(B200H264QpelContext *c)
 template <int AVG, int IDX>
 void chroma_hbd_tab(uint8_t *dst, const uint8_t *src, ptrdiff_t stride, int h, int x, int y)
 {
-    if ((unsigned)x > 7 || (unsigned)y > 7) hbd_die("h264chroma: x, y must be in 0..7");     // av_assert2 in the reference
+    if ((unsigned)x > 7 || (unsigned)y > 7) B200HostCall::fail(kFeature, "h264chroma: x, y must be in 0..7");     // av_assert2 in the reference
     if (h <= 0) return;
     constexpr int w = 8 >> IDX;
-    B200Device *dev = b200_default_device();
-    if (!dev) hbd_die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) hbd_die("cudaSetDevice");
     const size_t pitch = 32;                                       // 9 samples of 2 bytes
     const int ax = x ? 1 : 0, ay = y ? 1 : 0;
-    B200_LOCK_DEVICE(dev);
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, pitch * (size_t)(2 * h + 1) + 256);
-    if (!scr) hbd_die("scratch");
+    B200HostCall call(kFeature, nullptr, pitch * (size_t)(2 * h + 1) + 256);
+    uint8_t *scr = call.scratch;
     uint8_t *dsrc = scr, *ddst = scr + pitch * (size_t)(h + 1), *meta = ddst + pitch * (size_t)h;
-    cudaStream_t st = dev->stream;
-    if (b200_h2d_rows(dsrc, pitch, src, stride, (size_t)(w + ax) * 2, (size_t)(h + ay), st) != cudaSuccess) hbd_die("h2d src");
-    if (b200_h2d_rows(ddst, pitch, dst, stride, (size_t)w * 2, (size_t)h, st) != cudaSuccess) hbd_die("h2d dst");
+    cudaStream_t st = call.stream;
+    call.check(b200_h2d_rows(dsrc, pitch, src, stride, (size_t)(w + ax) * 2, (size_t)(h + ay), st), "h2d src");
+    call.check(b200_h2d_rows(ddst, pitch, dst, stride, (size_t)w * 2, (size_t)h, st), "h2d dst");
     struct { long long doff, soff; uint8_t op, h, xy; } m = { 0, 0, (uint8_t)(AVG | (IDX << 1)), (uint8_t)h, (uint8_t)(x | (y << 3)) };
-    if (cudaMemcpyAsync(meta, &m, sizeof(m), cudaMemcpyHostToDevice, st) != cudaSuccess) hbd_die("h2d meta");
-    if (chroma_hbd_launch(st, 1, meta + 16, meta + 17, meta + 18, ddst, (const long long *)meta, dsrc, (const long long *)meta + 1, (long long)pitch) < 0) hbd_die("launch");
-    if (b200_d2h_rows(dst, stride, ddst, pitch, (size_t)w * 2, (size_t)h, st) != cudaSuccess) hbd_die("d2h");
-    if (cudaStreamSynchronize(st) != cudaSuccess) hbd_die("sync");
+    call.check(cudaMemcpyAsync(meta, &m, sizeof(m), cudaMemcpyHostToDevice, st), "h2d meta");
+    call.launched(chroma_hbd_launch(st, 1, meta + 16, meta + 17, meta + 18, ddst, (const long long *)meta, dsrc, (const long long *)meta + 1, (long long)pitch));
+    call.check(b200_d2h_rows(dst, stride, ddst, pitch, (size_t)w * 2, (size_t)h, st), "d2h");
+    call.sync();
 }
 
 } // namespace
@@ -224,7 +212,7 @@ B200_API int b200_h264qpel_hbd_batch_device(B200Device *dev, int bit_depth, int6
     if (bit_depth != 9 && bit_depth != 10 && bit_depth != 12 && bit_depth != 14) return B200_ENOSYS;
     if ((stride & 1) || ((reinterpret_cast<uintptr_t>(dst) | reinterpret_cast<uintptr_t>(src)) & 1)) return B200_EINVAL;
     if (n == 0) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     return hbd_launch(dev->stream, bit_depth, n, op, dst, (const long long *)dst_off, src, (const long long *)src_off, (long long)stride);
 }
 
@@ -241,6 +229,6 @@ B200_API int b200_h264chroma_hbd_batch_device(B200Device *dev, int64_t n, const 
     if (!dev || n < 0 || !op || !h || !xy || !dst || !dst_off || !src || !src_off) return B200_EINVAL;
     if ((stride & 1) || ((reinterpret_cast<uintptr_t>(dst) | reinterpret_cast<uintptr_t>(src)) & 1)) return B200_EINVAL;
     if (n == 0) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     return chroma_hbd_launch(dev->stream, n, op, h, xy, dst, (const long long *)dst_off, src, (const long long *)src_off, (long long)stride);
 }

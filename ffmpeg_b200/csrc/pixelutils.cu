@@ -27,26 +27,22 @@ pixelutils_sad_kernel(int bits, const uint8_t *f1, long long stride1, const uint
 
 int host_sad(int bits, const uint8_t *src1, ptrdiff_t stride1, const uint8_t *src2, ptrdiff_t stride2)
 {
-    auto fail = [](const char *what) { fprintf(stderr, "libb200dsp: av_pixelutils_sad_fn failed: %s (%s)\n", what, b200_last_error()); abort(); };
-    B200Device *dev = b200_default_device();
-    if (!dev) fail("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) fail("cudaSetDevice");
     const int size = 1 << bits;
     const size_t pitch = 32;
-    B200_LOCK_DEVICE(dev);      // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, 2 * pitch * 32 + 64);
-    if (!scr) fail("scratch");
-    uint8_t *d1 = scr, *d2 = scr + pitch * 32;
-    int64_t *offs = (int64_t *)(scr + 2 * pitch * 32);
+    B200HostCall call("av_pixelutils_sad_fn", nullptr, 2 * pitch * 32 + 64);
+    uint8_t *d1 = call.scratch, *d2 = call.scratch + pitch * 32;
+    int64_t *offs = (int64_t *)(call.scratch + 2 * pitch * 32);
     int *dout = (int *)(offs + 2);
-    cudaStream_t st = dev->stream;
-    if (b200_h2d_rows(d1, pitch, src1, stride1, size, size, st) != cudaSuccess) fail("h2d");
-    if (b200_h2d_rows(d2, pitch, src2, stride2, size, size, st) != cudaSuccess) fail("h2d");
-    if (cudaMemsetAsync(offs, 0, 24, st) != cudaSuccess) fail("memset");
+    cudaStream_t st = call.stream;
+    call.check(b200_h2d_rows(d1, pitch, src1, stride1, size, size, st), "h2d");
+    call.check(b200_h2d_rows(d2, pitch, src2, stride2, size, size, st), "h2d");
+    call.check(cudaMemsetAsync(offs, 0, 24, st), "memset");
     pixelutils_sad_kernel<<<1, 32, 0, st>>>(bits, d1, (long long)pitch, d2, (long long)pitch, offs, offs + 1, 1, dout);
     B200_LAUNCHED();
+    call.launched();
     int res = 0;
-    if (cudaMemcpyAsync(&res, dout, 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) fail("d2h");
+    call.check(cudaMemcpyAsync(&res, dout, 4, cudaMemcpyDeviceToHost, st), "d2h");
+    call.sync();
     return res;
 }
 
@@ -70,12 +66,10 @@ B200_API b200_pixelutils_sad_fn b200_pixelutils_get_sad_fn(int w_bits, int h_bit
 B200_API int b200_pixelutils_sad_batch_device(B200Device *dev, int w_bits, const uint8_t *frame1, ptrdiff_t stride1, const uint8_t *frame2,
                                               ptrdiff_t stride2, const int64_t *off1, const int64_t *off2, int64_t n, int32_t *out)
 {
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
+    if (int r = b200_use_device(dev)) return r;
     if (w_bits < 1 || w_bits > 5 || n < 0) return B200_EINVAL;
     if (n == 0) return 0;
     if (!frame1 || !frame2 || !off1 || !off2 || !out) return B200_EINVAL;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
     const long long threads = n << w_bits, grid = (threads + 255) / 256;
     if (grid > 0x7fffffffLL) return B200_EINVAL;
     B200_CUDA_OK(cudaMemsetAsync(out, 0, (size_t)n * 4, dev->stream));

@@ -660,9 +660,6 @@ static void tx_host_fn(B200TXContext *c, void *out, void *in, ptrdiff_t stride)
 {
     if (c->i32) { tx_i32_host_fn(c->i32, out, in, stride); return; }
     if (c->dbl) { tx_dbl_host_fn(c->dbl, out, in, stride); return; }
-    auto fail = [](const char *what) { fprintf(stderr, "libb200dsp: av_tx_fn failed: %s (%s)\n", what, b200_last_error()); abort(); };
-    B200Device *d = c->dev;
-    if (cudaSetDevice(d->ordinal) != cudaSuccess) fail("cudaSetDevice");
     const size_t n = c->d.n, len = c->len;
     size_t in_elems, out_elems;            // floats
     if (c->dct) { in_elems = out_elems = (size_t)tx_dct_points(c->dct); }     // DCT-II: len in / len out; DCT-III: 2*len in / 2*len out
@@ -670,26 +667,25 @@ static void tx_host_fn(B200TXContext *c, void *out, void *in, ptrdiff_t stride)
     else if (c->type == 6) { in_elems = c->inv ? len + 2 : len; out_elems = c->inv ? len : len + 2; }
     else if (c->inv) { in_elems = len; out_elems = c->full ? 2 * len : len; }
     else { in_elems = 2 * len; out_elems = len; }
-    if (c->full && stride != 4) fail("AV_TX_FULL_IMDCT takes stride == sizeof(float) (the reference mirrors with the input stride)");
-    B200_LOCK_DEVICE(d);      // scratch + stream are per device: one host-pointer call at a time (released on return)
-    float *scr = (float *)b200_scratch(d, (in_elems + out_elems) * 4 + 512);
-    if (!scr) fail("scratch");
-    float *din = scr, *dout = scr + ((in_elems + 63) & ~(size_t)63);
-    cudaStream_t st = d->stream;
+    if (c->full && stride != 4) B200HostCall::fail("av_tx_fn", "AV_TX_FULL_IMDCT takes stride == sizeof(float) (the reference mirrors with the input stride)");
+    B200HostCall call("av_tx_fn", c->dev, (in_elems + out_elems) * 4 + 512);
+    float *din = (float *)call.scratch, *dout = din + ((in_elems + 63) & ~(size_t)63);
+    cudaStream_t st = call.stream;
     cudaError_t e;
     const bool strided_in = c->type == 1 && c->inv && stride != 4;
     const bool strided_out = c->type == 1 && !c->inv && stride != 4;
     const bool strided_cpx = c->type == 0 && c->pfa && stride != 8;  // ff_tx_fft_pfa stores out[i * stride] (tx_template.c:1078-1079)
     if (strided_in) e = cudaMemcpy2DAsync(din, 4, in, (size_t)stride, 4, in_elems, cudaMemcpyHostToDevice, st);
     else e = cudaMemcpyAsync(din, in, in_elems * 4, cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) fail("h2d");
+    call.check(e, "h2d");
     const bool clobbers = c->type == 6 && c->inv;                    // ff_tx_rdft_c2r rewrites its input (tx_template.c:1670-1696)
-    if (tx_launch(c, st, dout, din, c->type == 0 ? 8 : 4, 1, 0, 0, clobbers ? din : nullptr) < 0) fail("launch");
-    if (clobbers && cudaMemcpyAsync(in, din, (in_elems - 2) * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess) fail("d2h input");
+    call.launched(tx_launch(c, st, dout, din, c->type == 0 ? 8 : 4, 1, 0, 0, clobbers ? din : nullptr));
+    if (clobbers) call.check(cudaMemcpyAsync(in, din, (in_elems - 2) * 4, cudaMemcpyDeviceToHost, st), "d2h input");
     if (strided_out) e = cudaMemcpy2DAsync(out, (size_t)stride, dout, 4, 4, out_elems, cudaMemcpyDeviceToHost, st);
     else if (strided_cpx) e = cudaMemcpy2DAsync(out, (size_t)stride, dout, 8, 8, out_elems / 2, cudaMemcpyDeviceToHost, st);
     else e = cudaMemcpyAsync(out, dout, out_elems * 4, cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) fail("d2h");
+    call.check(e, "d2h");
+    call.sync();
 }
 
 B200_API int b200_tx_init_device(B200Device *dev, B200TXContext **ctx, b200_tx_fn *tx, int type, int inv, int len,

@@ -319,24 +319,20 @@ int tx_dbl_launch(TxDbl *p, cudaStream_t st, void *out, const void *in, ptrdiff_
 // av_tx_fn shaped entry: HOST pointers, one transform
 void tx_dbl_host_fn(TxDbl *p, void *out, void *in, ptrdiff_t stride)
 {
-    auto fail = [](const char *what) { fprintf(stderr, "libb200dsp: av_tx_fn (double) failed: %s (%s)\n", what, b200_last_error()); abort(); };
-    B200Device *d = p->dev;
-    if (cudaSetDevice(d->ordinal) != cudaSuccess) fail("cudaSetDevice");
     const size_t len = p->len;
     const bool mdct = p->type == B200_TX_DOUBLE_MDCT;
     const size_t in_elems = !mdct ? 2 * len : p->inv ? len : 2 * len, out_elems = !mdct ? 2 * len : len;        // doubles
-    B200_LOCK_DEVICE(d);
-    double *scr = (double *)b200_scratch(d, (in_elems + out_elems) * 8 + 1024);
-    if (!scr) fail("scratch");
-    double *din = scr, *dout = scr + ((in_elems + 63) & ~(size_t)63);
-    cudaStream_t st = d->stream;
+    B200HostCall call("av_tx_fn (double)", p->dev, (in_elems + out_elems) * 8 + 1024);
+    double *din = (double *)call.scratch, *dout = din + ((in_elems + 63) & ~(size_t)63);
+    cudaStream_t st = call.stream;
     cudaError_t e;
     const bool strided_in = mdct && p->inv && stride != 8, strided_out = mdct && !p->inv && stride != 8;
     if (strided_in) e = cudaMemcpy2DAsync(din, 8, in, (size_t)stride, 8, in_elems, cudaMemcpyHostToDevice, st);
     else e = cudaMemcpyAsync(din, in, in_elems * 8, cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) fail("h2d");
-    if (tx_dbl_launch(p, st, dout, din, 8, 1, 0, 0) < 0) fail("launch");
+    call.check(e, "h2d");
+    call.launched(tx_dbl_launch(p, st, dout, din, 8, 1, 0, 0));
     if (strided_out) e = cudaMemcpy2DAsync(out, (size_t)stride, dout, 8, 8, out_elems, cudaMemcpyDeviceToHost, st);
     else e = cudaMemcpyAsync(out, dout, out_elems * 8, cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) fail("d2h");
+    call.check(e, "d2h");
+    call.sync();
 }

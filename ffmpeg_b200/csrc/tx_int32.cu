@@ -328,24 +328,20 @@ int tx_i32_launch(TxI32 *p, cudaStream_t st, void *out, const void *in, ptrdiff_
 
 void tx_i32_host_fn(TxI32 *p, void *out, void *in, ptrdiff_t stride)
 {
-    auto fail = [](const char *what) { fprintf(stderr, "libb200dsp: av_tx_fn (int32) failed: %s (%s)\n", what, b200_last_error()); abort(); };
-    B200Device *d = p->dev;
-    if (cudaSetDevice(d->ordinal) != cudaSuccess) fail("cudaSetDevice");
     const size_t len = p->len;
     const bool mdct = p->type == B200_TX_INT32_MDCT;
     const size_t in_elems = !mdct ? 2 * len : p->inv ? len : 2 * len, out_elems = !mdct ? 2 * len : len;        // 32-bit words
-    B200_LOCK_DEVICE(d);      // scratch + stream are per device: one host-pointer call at a time (released on return)
-    int32_t *scr = (int32_t *)b200_scratch(d, (in_elems + out_elems) * 4 + 512);
-    if (!scr) fail("scratch");
-    int32_t *din = scr, *dout = scr + ((in_elems + 63) & ~(size_t)63);
-    cudaStream_t st = d->stream;
+    B200HostCall call("av_tx_fn (int32)", p->dev, (in_elems + out_elems) * 4 + 512);
+    int32_t *din = (int32_t *)call.scratch, *dout = din + ((in_elems + 63) & ~(size_t)63);
+    cudaStream_t st = call.stream;
     cudaError_t e;
     const bool strided_in = mdct && p->inv && stride != 4, strided_out = mdct && !p->inv && stride != 4;
     if (strided_in) e = cudaMemcpy2DAsync(din, 4, in, (size_t)stride, 4, in_elems, cudaMemcpyHostToDevice, st);
     else e = cudaMemcpyAsync(din, in, in_elems * 4, cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) fail("h2d");
-    if (tx_i32_launch(p, st, dout, din, 4, 1, 0, 0) < 0) fail("launch");
+    call.check(e, "h2d");
+    call.launched(tx_i32_launch(p, st, dout, din, 4, 1, 0, 0));
     if (strided_out) e = cudaMemcpy2DAsync(out, (size_t)stride, dout, 4, 4, out_elems, cudaMemcpyDeviceToHost, st);
     else e = cudaMemcpyAsync(out, dout, out_elems * 4, cudaMemcpyDeviceToHost, st);
-    if (e != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) fail("d2h");
+    call.check(e, "d2h");
+    call.sync();
 }

@@ -61,14 +61,12 @@ mpv_unquant_kernel(const __grid_constant__ UnquantDev P, int16_t *blocks, long l
 B200_API int b200_mpv_unquantize_batch_device(B200Device *dev, int variant, const B200MpvUnquant *p, int16_t *blocks, int64_t nblocks,
                                               const uint8_t *blk_n, const uint8_t *qscale, const int8_t *last_index)
 {
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
+    if (int r = b200_use_device(dev)) return r;
     if (!p || nblocks < 0 || variant < 0 || variant > B200_UNQUANT_H263_INTER) return B200_EINVAL;
     if (nblocks == 0) return 0;
     if (!blocks || !qscale || !last_index || (reinterpret_cast<uintptr_t>(blocks) & 3)) return B200_EINVAL;
     UnquantDev P;
     if (!mpv_unquant_params(p, &P)) { b200_set_error("b200_mpv_unquantize: permutated[] is not a permutation of 0..63"); return B200_EINVAL; }
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
     long long grid = (nblocks + WARPS - 1) / WARPS;
     const long long cap = (long long)(dev->sm_count > 0 ? dev->sm_count : 132) * 16 * 8;      // persistent warps: each walks nblocks / (grid * WARPS) blocks
     if (grid > cap) grid = cap;

@@ -52,12 +52,6 @@ int launch(cudaStream_t st, long long n, uint8_t *buf, const int64_t *buf_off, l
     return 0;
 }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: emulated_edge_mc failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 // VideoDSPContext.emulated_edge_mc (host pointers): only the part of the picture the window reaches is copied
 template <typename P>
 void edge_tab(uint8_t *buf, const uint8_t *src, ptrdiff_t buf_linesize, ptrdiff_t src_linesize, int block_w, int block_h,
@@ -66,28 +60,23 @@ void edge_tab(uint8_t *buf, const uint8_t *src, ptrdiff_t buf_linesize, ptrdiff_
     constexpr int BPS = sizeof(P);                                 // bytes per sample
     if (!w || !h) return;                                          // videodsp_template.c:33-34
     if (block_w <= 0 || block_h <= 0) return;
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
     // the part of the picture the window can reach after clamping
     const int x0 = std::min(std::max(src_x, 0), w - 1), x1 = std::min(std::max(src_x + block_w - 1, 0), w - 1);
     const int y0 = std::min(std::max(src_y, 0), h - 1), y1 = std::min(std::max(src_y + block_h - 1, 0), h - 1);
     const size_t rw = (size_t)(x1 - x0 + 1) * BPS, rh = (size_t)(y1 - y0 + 1);
     const size_t rp = (rw + 15) & ~(size_t)15, bp = ((size_t)block_w * BPS + 15) & ~(size_t)15;
-    B200_LOCK_DEVICE(dev);      // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, rp * rh + bp * block_h + 256);
-    if (!scr) die("scratch");
-    uint8_t *drect = scr, *dbuf = scr + rp * rh, *meta = dbuf + bp * block_h;
+    B200HostCall call("emulated_edge_mc", nullptr, rp * rh + bp * block_h + 256);
+    uint8_t *drect = call.scratch, *dbuf = drect + rp * rh, *meta = dbuf + bp * block_h;
     meta += (16 - ((uintptr_t)meta & 15)) & 15;
-    cudaStream_t st = dev->stream;
+    cudaStream_t st = call.stream;
     const uint8_t *pic = src - (ptrdiff_t)src_y * src_linesize - (ptrdiff_t)src_x * BPS;
-    if (b200_h2d_rows(drect, rp, pic + (ptrdiff_t)y0 * src_linesize + (ptrdiff_t)x0 * BPS, src_linesize, rw, rh, st) != cudaSuccess) die("h2d");
+    call.check(b200_h2d_rows(drect, rp, pic + (ptrdiff_t)y0 * src_linesize + (ptrdiff_t)x0 * BPS, src_linesize, rw, rh, st), "h2d");
     struct { int32_t g[4]; int64_t boff, origin; } m = { { block_w, block_h, src_x, src_y }, 0, -((int64_t)y0 * (int64_t)rp + (int64_t)x0 * BPS) };
-    if (cudaMemcpyAsync(meta, &m, sizeof(m), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d meta");
-    if (launch<P>(st, 1, dbuf, (const int64_t *)(meta + 16), (long long)bp, drect, (const int64_t *)(meta + 24), (long long)rp,
-                  (const int32_t *)meta, w, h) < 0) die("launch");
-    if (b200_d2h_rows(buf, buf_linesize, dbuf, bp, (size_t)block_w * BPS, (size_t)block_h, st) != cudaSuccess) die("d2h");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.check(cudaMemcpyAsync(meta, &m, sizeof(m), cudaMemcpyHostToDevice, st), "h2d meta");
+    call.launched(launch<P>(st, 1, dbuf, (const int64_t *)(meta + 16), (long long)bp, drect, (const int64_t *)(meta + 24), (long long)rp,
+                            (const int32_t *)meta, w, h));
+    call.check(b200_d2h_rows(buf, buf_linesize, dbuf, bp, (size_t)block_w * BPS, (size_t)block_h, st), "d2h");
+    call.sync();
 }
 
 void prefetch_nop(const uint8_t *, ptrdiff_t, int) {}
@@ -110,7 +99,7 @@ B200_API int b200_emulated_edge_mc_batch_device(B200Device *dev, int64_t n, uint
     if (!dev || n < 0 || !buf || !buf_off || !src || !origin || !geom || w < 0 || h < 0) return B200_EINVAL;
     if (((uintptr_t)geom & 15) != 0) return B200_EINVAL;
     if (n == 0 || !w || !h) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     return launch<uint8_t>(dev->stream, n, buf, buf_off, buf_linesize, src, origin, src_linesize, geom, w, h);
 }
 
@@ -121,6 +110,6 @@ B200_API int b200_emulated_edge_mc_hbd_batch_device(B200Device *dev, int64_t n, 
     if (((buf_linesize | src_linesize) & 1) || ((reinterpret_cast<uintptr_t>(buf) | reinterpret_cast<uintptr_t>(src)) & 1)) return B200_EINVAL;
     if ((uintptr_t)geom & 3) return B200_EINVAL;                   // the kernel reads geom as int32
     if (n == 0 || !w || !h) return 0;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     return launch<uint16_t>(dev->stream, n, buf, buf_off, buf_linesize, src, origin, src_linesize, geom, w, h);
 }

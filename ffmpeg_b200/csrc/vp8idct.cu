@@ -236,12 +236,6 @@ __global__ void vp8_idct_member_kernel(int kind, int is_vp7, int16_t *blocks, co
     for (int k = 0; k < 16; k++) blk[k] = 0;
 }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: vp8 residual member failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 // kind's member on host memory: dst rows x cols (0 for the WHT members), the coefficients it reads (`coef`, 16 per block, nblk blocks,
 // only coefficient 0 of each where dc0_only), dc (the WHT members)
 void member_host(int kind, int is_vp7, uint8_t *dst, ptrdiff_t stride, int16_t *coef, int16_t *dc)
@@ -249,30 +243,24 @@ void member_host(int kind, int is_vp7, uint8_t *dst, ptrdiff_t stride, int16_t *
     const int rows = kind == M_DC4UV ? 8 : 4, cols = kind == M_DC4Y ? 16 : kind == M_DC4UV ? 8 : 4;
     const int nblk = kind == M_WHT || kind == M_WHT_DC ? 16 : kind == M_DC4Y || kind == M_DC4UV ? 4 : 1;
     const bool wht = kind == M_WHT || kind == M_WHT_DC, dc0_only = kind != M_IDCT;
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
-    B200_LOCK_DEVICE(dev);            // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, 1024);
-    if (!scr) die("scratch");
-    cudaStream_t st = dev->stream;
+    B200HostCall call("vp8 residual member", nullptr, 1024);
+    uint8_t *scr = call.scratch;
+    cudaStream_t st = call.stream;
     int16_t *dblk = (int16_t *)scr, *ddc = (int16_t *)(scr + 512);
     uint8_t *ddst = scr + 576;
     const size_t bpitch = 16 * sizeof(int16_t);
     if (!wht) {
-        if (b200_h2d_rows(ddst, kMemberPitch, dst, stride, (size_t)cols, (size_t)rows, st) != cudaSuccess) die("h2d dst");
-        if (b200_h2d_rows(dblk, bpitch, coef, (ptrdiff_t)bpitch, dc0_only ? sizeof(int16_t) : bpitch, (size_t)nblk, st) != cudaSuccess)
-            die("h2d coef");
-    } else if (cudaMemcpyAsync(ddc, dc, (kind == M_WHT ? 16 : 1) * sizeof(int16_t), cudaMemcpyHostToDevice, st) != cudaSuccess) {
-        die("h2d dc");
+        call.check(b200_h2d_rows(ddst, kMemberPitch, dst, stride, (size_t)cols, (size_t)rows, st), "h2d dst");
+        call.check(b200_h2d_rows(dblk, bpitch, coef, (ptrdiff_t)bpitch, dc0_only ? sizeof(int16_t) : bpitch, (size_t)nblk, st), "h2d coef");
+    } else {
+        call.check(cudaMemcpyAsync(ddc, dc, (kind == M_WHT ? 16 : 1) * sizeof(int16_t), cudaMemcpyHostToDevice, st), "h2d dc");
     }
     vp8_idct_member_kernel<<<1, 32, 0, st>>>(kind, is_vp7, dblk, ddc, ddst);
     B200_LAUNCHED();
-    if (cudaGetLastError() != cudaSuccess) die("launch");
-    if (!wht && b200_d2h_rows(dst, stride, ddst, kMemberPitch, (size_t)cols, (size_t)rows, st) != cudaSuccess) die("d2h dst");
-    if (b200_d2h_rows(coef, (ptrdiff_t)bpitch, dblk, bpitch, dc0_only ? sizeof(int16_t) : bpitch, (size_t)nblk, st) != cudaSuccess)
-        die("d2h coef");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.launched();
+    if (!wht) call.check(b200_d2h_rows(dst, stride, ddst, kMemberPitch, (size_t)cols, (size_t)rows, st), "d2h dst");
+    call.check(b200_d2h_rows(coef, (ptrdiff_t)bpitch, dblk, bpitch, dc0_only ? sizeof(int16_t) : bpitch, (size_t)nblk, st), "d2h coef");
+    call.sync();
     if (kind == M_WHT) memset(dc, 0, 16 * sizeof(int16_t));                // the reference clears dc[0..15] (wht) / dc[0] (wht_dc)
     if (kind == M_WHT_DC) dc[0] = 0;
 }
@@ -315,9 +303,7 @@ B200_API int b200_vp8_residual_frame_device(B200Device *dev, int is_vp7, int64_t
     if ((ls_y & 3) || (ls_uv & 3)) { b200_set_error("vp8 residual frame: line size not a multiple of 4"); return B200_EINVAL; }
     for (int p = 0; p < 3; p++)
         if (!dst[p] || ((uintptr_t)dst[p] & 3)) { b200_set_error("vp8 residual frame: plane %d NULL or not 4-byte aligned", p); return B200_EINVAL; }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     ResArgs a;
     memset(&a, 0, sizeof(a));
     a.coef = coef;

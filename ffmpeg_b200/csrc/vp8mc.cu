@@ -144,12 +144,6 @@ cudaError_t launch(McArgs a, cudaStream_t st)
     return cudaSuccess;
 }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: vp8 motion compensation failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 // ---- drop-in members (host pointers).  vt / ht: 0 no filter, 4 / 6 taps (epel), 1 bilinear.  The samples the reference function
 // reads are copied into a dense device window that is the op's whole reference plane (the kernel's other reads clamp into it and
 // meet zero taps), the block is predicted into a dense device buffer and copied back.
@@ -166,15 +160,11 @@ void member_host(int W, int vt, int ht, uint8_t *dst, ptrdiff_t dststride, const
     const int top = vt == 6 ? 2 : vt == 4 ? 1 : 0, bottom = vt == 6 ? 3 : vt == 4 ? 2 : vt == 1 ? 1 : 0;
     const int wc = left + W + right, wr = top + h + bottom;
     const size_t wpitch = 32, wbytes = (wpitch * wr + 255) & ~(size_t)255;
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
-    B200_LOCK_DEVICE(dev);            // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, wbytes + 256 + 16 * 32);
-    if (!scr) die("scratch");
-    cudaStream_t st = dev->stream;
+    B200HostCall call("vp8 motion compensation", nullptr, wbytes + 256 + 16 * 32);
+    uint8_t *scr = call.scratch;
+    cudaStream_t st = call.stream;
     uint8_t *dwin = scr, *dop = scr + wbytes, *ddst = dop + 256;
-    if (b200_h2d_rows(dwin, wpitch, src - top * srcstride - left, srcstride, (size_t)wc, (size_t)wr, st) != cudaSuccess) die("h2d window");
+    call.check(b200_h2d_rows(dwin, wpitch, src - top * srcstride - left, srcstride, (size_t)wc, (size_t)wr, st), "h2d window");
     B200Vp8McOp op[2];                                                   // ops take h <= 16: a taller call is two ops
     memset(op, 0, sizeof(op));
     const int nops = h > 16 ? 2 : 1;
@@ -188,7 +178,7 @@ void member_host(int W, int vt, int ht, uint8_t *dst, ptrdiff_t dststride, const
         op[k].mx = (uint8_t)mx;
         op[k].my = (uint8_t)my;
     }
-    if (cudaMemcpyAsync(dop, op, sizeof(op), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d op");
+    call.check(cudaMemcpyAsync(dop, op, sizeof(op), cudaMemcpyHostToDevice, st), "h2d op");
     McArgs a;
     memset(&a, 0, sizeof(a));
     a.ops = (const B200Vp8McOp *)dop;
@@ -205,9 +195,9 @@ void member_host(int W, int vt, int ht, uint8_t *dst, ptrdiff_t dststride, const
     a.bank_v = vt == 4 ? 1 : 0;
     a.refs[0].y = dwin;
     a.refs[0].ls_y = (ptrdiff_t)wpitch;
-    if (launch(a, st) != cudaSuccess) die("launch");
-    if (b200_d2h_rows(dst, dststride, ddst, 16, (size_t)W, (size_t)h, st) != cudaSuccess) die("d2h");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.check(launch(a, st), "launch");
+    call.check(b200_d2h_rows(dst, dststride, ddst, 16, (size_t)W, (size_t)h, st), "d2h");
+    call.sync();
 }
 
 template <int W, int VT, int HT>
@@ -273,9 +263,7 @@ B200_API int b200_vp8_mc_frame_device(B200Device *dev, int bilinear, int mb_widt
         if (!refs[r].y || !refs[r].u || !refs[r].v) { b200_set_error("vp8 mc frame: reference %d has a NULL plane", r); return B200_EINVAL; }
         a.refs[r] = refs[r];
     }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     a.ops = ops;
     a.nops = (long long)nops;
     for (int p = 0; p < 3; p++) a.dst[p] = dst[p];

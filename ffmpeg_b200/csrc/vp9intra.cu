@@ -320,12 +320,6 @@ __global__ void __launch_bounds__(32 * kWarps) vp9_intra_kernel(const __grid_con
 
 bool depth_ok(int d) { return d == 8 || d == 10 || d == 12; }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: vp9 intra prediction failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 // ---- drop-in members (host pointers): the samples the reference function reads go to a device scratch (top[-1 ..] at sample 0, left[]
 // at sample kTop), one warp predicts the block with pred_px, and the block comes back.
 struct MemberArgs {
@@ -369,27 +363,23 @@ void footprint(int mode, int n, int &t0, int &t1, int &l0, int &l1)
 void member_host(int depth, int tx, int mode, uint8_t *dst, ptrdiff_t stride, const uint8_t *left, const uint8_t *top)
 {
     const int n = 4 << tx, bps = depth > 8 ? 2 : 1;
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
-    B200_LOCK_DEVICE(dev);            // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, (size_t)(kTop + 32 + 32 * 32) * bps);
-    if (!scr) die("scratch");
-    cudaStream_t st = dev->stream;
+    B200HostCall call("vp9 intra prediction", nullptr, (size_t)(kTop + 32 + 32 * 32) * bps);
+    uint8_t *scr = call.scratch;
+    cudaStream_t st = call.stream;
     int t0, t1, l0, l1;
     footprint(mode, n, t0, t1, l0, l1);
-    if (cudaMemsetAsync(scr, 0, (size_t)(kTop + 32) * bps, st) != cudaSuccess) die("memset");
-    if (t1 > t0 && cudaMemcpyAsync(scr + (size_t)(t0 + 1) * bps, top + (ptrdiff_t)t0 * bps, (size_t)(t1 - t0) * bps, cudaMemcpyHostToDevice, st) != cudaSuccess)
-        die("h2d top");
-    if (l1 > l0 && cudaMemcpyAsync(scr + (size_t)(kTop + l0) * bps, left + (ptrdiff_t)l0 * bps, (size_t)(l1 - l0) * bps, cudaMemcpyHostToDevice, st) != cudaSuccess)
-        die("h2d left");
+    call.check(cudaMemsetAsync(scr, 0, (size_t)(kTop + 32) * bps, st), "memset");
+    if (t1 > t0)
+        call.check(cudaMemcpyAsync(scr + (size_t)(t0 + 1) * bps, top + (ptrdiff_t)t0 * bps, (size_t)(t1 - t0) * bps, cudaMemcpyHostToDevice, st), "h2d top");
+    if (l1 > l0)
+        call.check(cudaMemcpyAsync(scr + (size_t)(kTop + l0) * bps, left + (ptrdiff_t)l0 * bps, (size_t)(l1 - l0) * bps, cudaMemcpyHostToDevice, st), "h2d left");
     const MemberArgs m = { scr, mode, tx + 2, depth };
     if (depth == 8) vp9_intra_member_kernel<uint8_t><<<1, 32, 0, st>>>(m);
     else vp9_intra_member_kernel<uint16_t><<<1, 32, 0, st>>>(m);
     B200_LAUNCHED();
-    if (cudaGetLastError() != cudaSuccess) die("launch");
-    if (b200_d2h_rows(dst, stride, scr + (size_t)(kTop + 32) * bps, (size_t)n * bps, (size_t)n * bps, (size_t)n, st) != cudaSuccess) die("d2h block");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.launched();
+    call.check(b200_d2h_rows(dst, stride, scr + (size_t)(kTop + 32) * bps, (size_t)n * bps, (size_t)n * bps, (size_t)n, st), "d2h block");
+    call.sync();
 }
 
 template <int D, int TX, int MODE>
@@ -460,9 +450,7 @@ B200_API int b200_vp9_intra_recon_frame_device(B200Device *dev, int bit_depth, i
         b200_set_error("vp9 intra frame: ops / coef NULL or misaligned");
         return B200_EINVAL;
     }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     B200_LOCK_DEVICE(dev);
     int *timeouts = b200_wait_timeouts_word(dev->ordinal, B200_WAIT_VP9_INTRA, true);
     if (!timeouts) { b200_set_error("vp9 intra frame: no timeout counter for device %d", dev->ordinal); return B200_ENOMEM; }
@@ -510,9 +498,7 @@ B200_API int b200_vp9_intra_recon_frame_device(B200Device *dev, int bit_depth, i
 B200_API int b200_vp9_intra_timeouts(B200Device *dev, int64_t *count)
 {
     if (!count) { b200_set_error("vp9 intra timeouts: NULL pointer"); return B200_EINVAL; }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     B200_CUDA_OK(cudaStreamSynchronize(dev->stream));
     int v = 0;
     int *w = b200_wait_timeouts_word(dev->ordinal, B200_WAIT_VP9_INTRA, false);

@@ -257,38 +257,28 @@ cudaError_t launch(ItxArgs a, cudaStream_t st)
     return cudaSuccess;
 }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: vp9 inverse transform failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 // ---- drop-in members (host pointers): the block's coefficients and the sz x sz block of dst through the device scratch, one op, the
 // block back; the coefficients are then left as the reference leaves them (only block[0] cleared on the DC-only path, all else zeroed)
 void member_host(int depth, int tx, int type, uint8_t *dst, ptrdiff_t stride, int16_t *block, int eob)
 {
     const int N = tx == 4 ? 4 : 4 << tx, bps = depth > 8 ? 2 : 1, cs = depth > 8 ? 4 : 2;
     const size_t cbytes = (size_t)N * N * cs, dpitch = (size_t)N * bps;
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
-    B200_LOCK_DEVICE(dev);            // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, 256 + 4096 + 2048);
-    if (!scr) die("scratch");
-    cudaStream_t st = dev->stream;
+    B200HostCall call("vp9 inverse transform", nullptr, 256 + 4096 + 2048);
+    uint8_t *scr = call.scratch;
+    cudaStream_t st = call.stream;
     uint8_t *dop = scr, *dcoef = scr + 256, *ddst = dcoef + 4096;
     B200Vp9TxOp op;
     memset(&op, 0, sizeof(op));
     op.tx = (uint8_t)tx;
     op.type = (uint8_t)type;
     op.eob = (uint16_t)(eob == 1);   // only eob == 1 means anything to the members; any other int runs the full transform
-    if (cudaMemcpyAsync(dop, &op, sizeof(op), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d op");
-    if (cudaMemcpyAsync(dcoef, block, cbytes, cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d coefficients");
-    if (b200_h2d_rows(ddst, dpitch, dst, stride, dpitch, (size_t)N, st) != cudaSuccess) die("h2d block");
+    call.check(cudaMemcpyAsync(dop, &op, sizeof(op), cudaMemcpyHostToDevice, st), "h2d op");
+    call.check(cudaMemcpyAsync(dcoef, block, cbytes, cudaMemcpyHostToDevice, st), "h2d coefficients");
+    call.check(b200_h2d_rows(ddst, dpitch, dst, stride, dpitch, (size_t)N, st), "h2d block");
     ItxArgs a = { (const B200Vp9TxOp *)dop, 1, dcoef, ddst, (long long)dpitch, depth, 1 };
-    if (launch(a, st) != cudaSuccess) die("launch");
-    if (b200_d2h_rows(dst, stride, ddst, dpitch, dpitch, (size_t)N, st) != cudaSuccess) die("d2h block");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.check(launch(a, st), "launch");
+    call.check(b200_d2h_rows(dst, stride, ddst, dpitch, dpitch, (size_t)N, st), "d2h block");
+    call.sync();
     memset(block, 0, dc_only(tx, type, eob) ? (size_t)cs : cbytes);
 }
 
@@ -341,9 +331,7 @@ B200_API int b200_vp9_itxfm_add_batch_device(B200Device *dev, int bit_depth, int
         b200_set_error("vp9 itxfm batch: NULL or misaligned pointer");
         return B200_EINVAL;
     }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     ItxArgs a = { ops, (long long)nops, coef, dst, (long long)dst_stride, bit_depth, 1 };
     B200_CUDA_OK(launch(a, dev->stream));
     return 0;

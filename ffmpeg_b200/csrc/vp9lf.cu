@@ -293,12 +293,6 @@ __global__ void __launch_bounds__(kThreads) vp9_lf_kernel(const __grid_constant_
 
 bool depth_ok(int d) { return d == 8 || d == 10 || d == 12; }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: vp9 loop filter failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 // ---- drop-in members (host pointers): the footprint of each 8-line half (dst[-4..3] across for widths 4 / 8, dst[-8..7] for 16) goes
 // to a 16 x 16 device scratch laid out like the host's (dir 0: line l is scratch row l, q0 at column 8; dir 1: across-offset k is
 // scratch row 8 + k, line l column l); one CTA filters the lines with lf_apply, and the samples the width may write come back.
@@ -321,13 +315,9 @@ void member_host(int depth, int dir, int wd1, int wd2, uint8_t *dst, ptrdiff_t s
 {
     const int bps = depth > 8 ? 2 : 1;
     const size_t dpitch = 16 * (size_t)bps;
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
-    B200_LOCK_DEVICE(dev);            // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, 16 * dpitch);
-    if (!scr) die("scratch");
-    cudaStream_t st = dev->stream;
+    B200HostCall call("vp9 loop filter", nullptr, 16 * dpitch);
+    uint8_t *scr = call.scratch;
+    cudaStream_t st = call.stream;
     const int wd[2] = { wd1, wd2 };
     // the block of lines 8h..8h+7 and across-offsets -n..n-1: host address, scratch address, bytes per copied row, rows
     auto copy = [&](int h, int n, bool up) {
@@ -337,15 +327,15 @@ void member_host(int depth, int dir, int wd1, int wd2, uint8_t *dst, ptrdiff_t s
         return up ? b200_h2d_rows(ds, dpitch, hs, stride, w, rows, st) : b200_d2h_rows(hs, stride, ds, dpitch, w, rows, st);
     };
     for (int h = 0; h < 2; h++)
-        if (wd[h] && copy(h, wd[h] == 16 ? 8 : 4, true) != cudaSuccess) die("h2d edge");
+        if (wd[h]) call.check(copy(h, wd[h] == 16 ? 8 : 4, true), "h2d edge");
     const MemberArgs m = { scr, dir, depth, { wd1, wd2 }, { E1, E2 }, { I1, I2 }, { H1, H2 } };
     if (depth == 8) vp9_lf_member_kernel<uint8_t><<<1, 16, 0, st>>>(m);
     else vp9_lf_member_kernel<uint16_t><<<1, 16, 0, st>>>(m);
     B200_LAUNCHED();
-    if (cudaGetLastError() != cudaSuccess) die("launch");
+    call.launched();
     for (int h = 0; h < 2; h++)
-        if (wd[h] && copy(h, wd[h] == 16 ? 7 : wd[h] == 8 ? 3 : 2, false) != cudaSuccess) die("d2h edge");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+        if (wd[h]) call.check(copy(h, wd[h] == 16 ? 7 : wd[h] == 8 ? 3 : 2, false), "d2h edge");
+    call.sync();
 }
 
 template <int D, int WD, int DIR>
@@ -416,9 +406,7 @@ B200_API int b200_vp9_loopfilter_frame_device(B200Device *dev, int bit_depth, in
     for (int p = 0; p < 3; p++)
         if ((uintptr_t)planes[p] % bps) { b200_set_error("vp9 loop filter frame: plane %d not aligned to a sample", p); return B200_EINVAL; }
     if (lflvl_stride < sb_cols) { b200_set_error("vp9 loop filter frame: lflvl_stride %lld below %d", (long long)lflvl_stride, sb_cols); return B200_EINVAL; }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     B200_LOCK_DEVICE(dev);
     int *timeouts = b200_wait_timeouts_word(dev->ordinal, B200_WAIT_VP9_LOOPFILTER, true);
     if (!timeouts) { b200_set_error("vp9 loop filter frame: no timeout counter for device %d", dev->ordinal); return B200_ENOMEM; }
@@ -455,9 +443,7 @@ B200_API int b200_vp9_loopfilter_frame_device(B200Device *dev, int bit_depth, in
 B200_API int b200_vp9_loopfilter_timeouts(B200Device *dev, int64_t *count)
 {
     if (!count) { b200_set_error("vp9 loop filter timeouts: NULL pointer"); return B200_EINVAL; }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     B200_CUDA_OK(cudaStreamSynchronize(dev->stream));
     int v = 0;
     int *w = b200_wait_timeouts_word(dev->ordinal, B200_WAIT_VP9_LOOPFILTER, false);

@@ -232,12 +232,6 @@ cudaError_t launch(McArgs a, cudaStream_t st)
     return cudaSuccess;
 }
 
-void die(const char *what)
-{
-    fprintf(stderr, "libb200dsp: vp9 motion compensation failed: %s (%s)\n", what, b200_last_error());
-    abort();
-}
-
 // ---- drop-in members (host pointers).  The samples the reference function reads are copied into a dense device window that is the
 // op's whole reference plane (for an 8-tap bank the clamped reads never clamp; for bilinear they clamp only under zero taps), the
 // caller's dst block next to it for an avg member, one op, and the block back.
@@ -255,16 +249,12 @@ void member_host(int depth, int w, int bank, int avg, bool hdir, bool vdir, uint
     const int wc = hdir ? (((w - 1) * dx + mx) >> 4) + span : w, wr = vdir ? (((h - 1) * dy + my) >> 4) + span : h;
     const size_t wpitch = ((size_t)wc * bps + 15) & ~(size_t)15, wbytes = (wpitch * wr + 255) & ~(size_t)255;
     const size_t dpitch = (size_t)64 * bps;
-    B200Device *dev = b200_default_device();
-    if (!dev) die("no device");
-    if (cudaSetDevice(dev->ordinal) != cudaSuccess) die("cudaSetDevice");
-    B200_LOCK_DEVICE(dev);            // scratch + stream are per device: one host-pointer call at a time (released on return)
-    uint8_t *scr = (uint8_t *)b200_scratch(dev, wbytes + 256 + dpitch * 64);
-    if (!scr) die("scratch");
-    cudaStream_t st = dev->stream;
+    B200HostCall call("vp9 motion compensation", nullptr, wbytes + 256 + dpitch * 64);
+    uint8_t *scr = call.scratch;
+    cudaStream_t st = call.stream;
     uint8_t *dwin = scr, *dop = scr + wbytes, *ddst = dop + 256;
-    if (b200_h2d_rows(dwin, wpitch, src - y0 * srcstride - x0 * bps, srcstride, (size_t)wc * bps, (size_t)wr, st) != cudaSuccess) die("h2d window");
-    if (avg && b200_h2d_rows(ddst, dpitch, dst, dststride, (size_t)w * bps, (size_t)h, st) != cudaSuccess) die("h2d dst");
+    call.check(b200_h2d_rows(dwin, wpitch, src - y0 * srcstride - x0 * bps, srcstride, (size_t)wc * bps, (size_t)wr, st), "h2d window");
+    if (avg) call.check(b200_h2d_rows(ddst, dpitch, dst, dststride, (size_t)w * bps, (size_t)h, st), "h2d dst");
     B200Vp9McOp op;
     memset(&op, 0, sizeof(op));
     const int r = avg ? 1 : 0;
@@ -276,7 +266,7 @@ void member_host(int depth, int w, int bank, int avg, bool hdir, bool vdir, uint
     op.h = (uint8_t)h;
     op.filter = (uint8_t)bank;
     op.kind = (uint8_t)(avg ? kAvgMember : B200_VP9_MC_SINGLE);
-    if (cudaMemcpyAsync(dop, &op, sizeof(op), cudaMemcpyHostToDevice, st) != cudaSuccess) die("h2d op");
+    call.check(cudaMemcpyAsync(dop, &op, sizeof(op), cudaMemcpyHostToDevice, st), "h2d op");
     McArgs a;
     memset(&a, 0, sizeof(a));
     a.ops = (const B200Vp9McOp *)dop;
@@ -293,9 +283,9 @@ void member_host(int depth, int w, int bank, int avg, bool hdir, bool vdir, uint
     a.refs[0].h = wr;
     a.refs[0].dx = dx;
     a.refs[0].dy = dy;
-    if (launch(a, st) != cudaSuccess) die("launch");
-    if (b200_d2h_rows(dst, dststride, ddst, dpitch, (size_t)w * bps, (size_t)h, st) != cudaSuccess) die("d2h");
-    if (cudaStreamSynchronize(st) != cudaSuccess) die("sync");
+    call.check(launch(a, st), "launch");
+    call.check(b200_d2h_rows(dst, dststride, ddst, dpitch, (size_t)w * bps, (size_t)h, st), "d2h");
+    call.sync();
 }
 
 template <int D, int W, int F, int A, int H, int V>
@@ -372,9 +362,7 @@ B200_API int b200_vp9_mc_batch_device(B200Device *dev, int bit_depth, int nrefs,
         }
         a.refs[r] = f;
     }
-    if (!dev) dev = b200_default_device();
-    if (!dev) return B200_ENODEV;
-    B200_CUDA_OK(cudaSetDevice(dev->ordinal));
+    if (int r = b200_use_device(dev)) return r;
     a.ops = ops;
     a.nops = (long long)nops;
     a.dst = dst;

@@ -256,14 +256,21 @@ class Vp9IntraOp(C.Structure):
 VP8_MC_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_void_p, C.c_ssize_t, C.c_int, C.c_int, C.c_int)
 VP8_WHT_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p)
 VP8_IDCT_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t)
+VP8_LF_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_int, C.c_int, C.c_int)               # 16y, 16y_inner: dst, stride, E, I, H
+VP8_LF_UV_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_int, C.c_int, C.c_int)  # 8uv, 8uv_inner: dstU, dstV, ...
+VP8_LF_SIMPLE_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_int)                         # simple: dst, stride, flim
 
 
 class VP8DSPContext(C.Structure):
-    """libavcodec/vp8dsp.h:37-82 (same member order; the loop-filter members, which this library does not fill, are plain pointers)"""
+    """libavcodec/vp8dsp.h:37-82 (same member order and member types)"""
     _fields_ = [("vp8_luma_dc_wht", VP8_WHT_FUNC), ("vp8_luma_dc_wht_dc", VP8_WHT_FUNC), ("vp8_idct_add", VP8_IDCT_FUNC),
                 ("vp8_idct_dc_add", VP8_IDCT_FUNC), ("vp8_idct_dc_add4y", VP8_IDCT_FUNC), ("vp8_idct_dc_add4uv", VP8_IDCT_FUNC),
-                ("loop_filter", vp * 10), ("put_vp8_epel_pixels_tab", VP8_MC_FUNC * 3 * 3 * 3),
-                ("put_vp8_bilinear_pixels_tab", VP8_MC_FUNC * 3 * 3 * 3)]
+                ("vp8_v_loop_filter16y", VP8_LF_FUNC), ("vp8_h_loop_filter16y", VP8_LF_FUNC),
+                ("vp8_v_loop_filter8uv", VP8_LF_UV_FUNC), ("vp8_h_loop_filter8uv", VP8_LF_UV_FUNC),
+                ("vp8_v_loop_filter16y_inner", VP8_LF_FUNC), ("vp8_h_loop_filter16y_inner", VP8_LF_FUNC),
+                ("vp8_v_loop_filter8uv_inner", VP8_LF_UV_FUNC), ("vp8_h_loop_filter8uv_inner", VP8_LF_UV_FUNC),
+                ("vp8_v_loop_filter_simple", VP8_LF_SIMPLE_FUNC), ("vp8_h_loop_filter_simple", VP8_LF_SIMPLE_FUNC),
+                ("put_vp8_epel_pixels_tab", VP8_MC_FUNC * 3 * 3 * 3), ("put_vp8_bilinear_pixels_tab", VP8_MC_FUNC * 3 * 3 * 3)]
 
 
 class Vp8McRef(C.Structure):
@@ -281,6 +288,11 @@ class Vp8ResidualOp(C.Structure):
     """B200Vp8ResidualOp (include/b200dsp.h), 48 bytes"""
     _fields_ = [("coef_off", C.c_int64), ("mb_x", C.c_int32), ("mb_y", C.c_int32), ("nnz", C.c_uint8 * 4 * 6), ("y2_nnz", C.c_uint8),
                 ("flags", C.c_uint8), ("reserved", C.c_uint8 * 6)]
+
+
+class Vp8FilterStrength(C.Structure):
+    """B200Vp8FilterStrength (include/b200dsp.h) = VP8FilterStrength (libavcodec/vp8.h:90-94), 3 bytes"""
+    _fields_ = [("filter_level", C.c_uint8), ("inner_limit", C.c_uint8), ("inner_filter", C.c_uint8)]
 
 
 class ProresDSPContext(C.Structure):
@@ -421,6 +433,10 @@ PROTOTYPES = {
     "b200_vp8_dsp_init": (C.c_int, [vp, C.c_int]),
     "b200_vp8_mc_frame_device": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_int64, vp, vp, C.c_ssize_t, C.c_ssize_t]),
     "b200_vp8_residual_frame_device": (C.c_int, [vp, C.c_int, C.c_int64, vp, vp, vp, C.c_ssize_t, C.c_ssize_t]),
+    "b200_vp8_dsp_init_loopfilter": (C.c_int, [vp, C.c_int]),
+    "b200_vp8_loopfilter_frame_device": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_ssize_t, C.c_ssize_t, vp,
+                                                   C.c_int64]),
+    "b200_vp8_loopfilter_timeouts": (C.c_int, [vp, vp]),
     "b200_proresdsp_init": (C.c_int, [vp, C.c_int]),
     "b200_prores_idct_put_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, vp, vp, vp, C.c_int]),
     "b200_float_dsp_init": (C.c_int, [vp]),

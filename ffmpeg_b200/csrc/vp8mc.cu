@@ -237,7 +237,7 @@ B200_API int b200_vp8_dsp_init(B200VP8DSPContext *c, int is_vp7)
 {
     if (!c || (is_vp7 != 0 && is_vp7 != 1)) { b200_set_error("vp8 dsp init: NULL context or is_vp7 not 0 / 1"); return B200_EINVAL; }
     if (!b200_default_device()) return B200_ENODEV;
-    memset(c, 0, sizeof(*c));                                            // the loop-filter members: not built, NULL
+    memset(c, 0, sizeof(*c));                                            // the loop-filter members: NULL (b200_vp8_dsp_init_loopfilter fills them)
     fill_size<0, 16>(c);
     fill_size<1, 8>(c);
     fill_size<2, 4>(c);

@@ -945,7 +945,7 @@ int  b200_vp9_intra_timeouts(B200Device *dev, int64_t *count);
 
 /* VP8 / VP7 motion compensation and residual: VP8DSPContext (libavcodec/vp8dsp.h:37-82) in the reference's member order and types.
  * b200_vp8_dsp_init() fills what ff_vp78dsp_init and ff_vp8dsp_init (is_vp7 = 0) / ff_vp7dsp_init (is_vp7 = 1) fill (vp8dsp.c:663-760)
- * except the ten loop-filter members, which stay NULL:
+ * except the ten loop-filter members, which it leaves NULL (b200_vp8_dsp_init_loopfilter fills them):
  *   vp8_luma_dc_wht, _wht_dc, vp8_idct_add, _dc_add, _dc_add4y, _dc_add4uv   the VP8 or the VP7 arithmetic
  *   put_vp8_epel_pixels_tab[size][v][h]       size 0..2 = 16, 8, 4 columns; v / h: 0 none, 1 4-tap, 2 6-tap; [0][1][*] and [0][*][1]
  *                                             NULL, as in the reference
@@ -1060,6 +1060,66 @@ _Static_assert(sizeof(B200Vp8ResidualOp) == 48, "B200Vp8ResidualOp is 48 bytes")
  * aligned to 16 bytes, or a dst plane or line size that is not a multiple of 4; nops == 0 returns 0. */
 int  b200_vp8_residual_frame_device(B200Device *dev, int is_vp7, int64_t nops, const B200Vp8ResidualOp *ops, const int16_t *coef,
                                     uint8_t *const dst[3], ptrdiff_t ls_y, ptrdiff_t ls_uv);
+
+/* VP8 / VP7 loop filter: b200_vp8_dsp_init_loopfilter() fills the ten loop-filter members of a B200VP8DSPContext (vp8_v_loop_filter16y
+ * .. vp8_h_loop_filter_simple) as ff_vp8dsp_init (is_vp7 = 0) / ff_vp7dsp_init (is_vp7 = 1) fill them (vp8dsp.c:702-713, :733-744):
+ * ten distinct functions per codec, twenty in all; it touches no other member.  v filters the edge between two rows (samples across it
+ * are dst[-4 stride .. 3 stride], the lines run along the row), h the edge between two columns (dst[-4..3], the lines run down).  HOST
+ * pointers and the reference's signatures; 16y filters 16 lines, 8uv 8 lines of U and 8 of V in one call, simple 16 lines.
+ * Per line (vp8dsp.c:263-457): the simple limit is 2 |p0 - q0| + (|p1 - q1| >> 1) <= E for VP8 and |p0 - q0| <= E for VP7; the normal
+ * limit adds every neighbour difference of p3..q3 <= I; hev is |p1 - p0| > H or |q1 - q0| > H.
+ *   common     a = clip_int8(3 (q0 - p0) + clip_int8(p1 - q1)) (the 4-tap form; without it the p1 - q1 term is left out), f1 = min(a + 4,
+ *              127) >> 3, f2 = min(a + 3, 127) >> 3 for VP8 and f1 - ((a & 7) == 4) for VP7; p0 += f2, q0 -= f1, and without the 4-tap
+ *              form p1 += (f1 + 1) >> 1, q1 -= (f1 + 1) >> 1, each clipped to 0..255
+ *   mbedge     w = clip_int8(clip_int8(p1 - q1) + 3 (q0 - p0)); p2 / q2, p1 / q1, p0 / q0 moved by (9 w + 63) >> 7, (18 w + 63) >> 7,
+ *              (27 w + 63) >> 7
+ *   16y, 8uv          normal limit, then hev ? common 4-tap : mbedge; reads dst[-4..3] across, writes dst[-3..2]
+ *   16y_inner, 8uv_inner   normal limit, then hev ? common 4-tap : common without it; reads dst[-4..3], writes dst[-2..1]
+ *   simple     simple limit, then common 4-tap; reads dst[-2..1], writes dst[-1..0]
+ * 0; B200_EINVAL for c == NULL or is_vp7 not 0 / 1; B200_ENODEV. */
+int  b200_vp8_dsp_init_loopfilter(B200VP8DSPContext *c, int is_vp7);
+
+/* One macroblock's loop-filter strength: VP8FilterStrength's layout (libavcodec/vp8.h:90-94), 3 bytes, byte alignment, as
+ * filter_level_for_mb leaves it (vp8.c:2149-2179). */
+typedef struct B200Vp8FilterStrength {
+    uint8_t filter_level;   /* 0: the MB is not filtered; above 63: left untouched (the decoder clips the level to 6 bits) */
+    uint8_t inner_limit;    /* I, and part of the VP8 edge limits */
+    uint8_t inner_filter;   /* nonzero: the inner edges are filtered */
+} B200Vp8FilterStrength;
+#ifdef __cplusplus
+static_assert(sizeof(B200Vp8FilterStrength) == 3, "B200Vp8FilterStrength is 3 bytes");
+#else
+_Static_assert(sizeof(B200Vp8FilterStrength) == 3, "B200Vp8FilterStrength is 3 bytes");
+#endif
+/* Loop-filters a whole VP8 / VP7 frame in place, DEVICE pointers (planes[0..2], f), asynchronous on the device's stream.  The result is
+ * what filter_mb_row (vp8.c:2523-2574) gives run over every MB row in order: per macroblock (mb_x, mb_y) with record
+ * f[mb_y * f_stride + mb_x] of level L, inner limit I and inner filter F,
+ *   normal (simple = 0)  filter_mb (vp8.c:2181-2266): VP8 edge limits bedge = 2 L + I, mbedge = bedge + 4; VP7 bedge_y = L,
+ *                        bedge_uv = 2 L, mbedge = L + 2; hev_thresh 1 from L = 15, one more from 40, and on inter frames (keyframe = 0)
+ *                        one more from 20.  h_loop_filter16y / 8uv at the left MB edge when mb_x > 0; with F the inner column edges
+ *                        (4, 8, 12 in luma, 4 in chroma); v_loop_filter16y / 8uv at the top MB edge when mb_y > 0; with F the inner
+ *                        row edges.  VP7 filters its inner column edges after the row edges (vp8.c:2265), VP8 before them.
+ *   simple (simple = 1)  filter_mb_simple (vp8.c:2268-2299) on luma only, the chroma planes untouched: the same edges with the simple
+ *                        members, and the VP8 limits 2 L + I / + 4 for VP7 too (with the VP7 members).
+ * An MB with L = 0 is skipped; an MB with L > 63 is left untouched too (the reference would index hev_thresh_lut out of bounds; the
+ * decoder clips L to 6 bits).  A nonzero inner_filter counts as true.
+ * Filtering the fully reconstructed frame once is exact: the decoder filters row r - 1 before it decodes row r, but row r's intra
+ * prediction reads the unfiltered top border that backup_mb_border / xchg_mb_border saved (vp8.c:1701-1706, :2556-2561), and its left
+ * neighbours unfiltered too, so this gives the single-threaded decoder's picture.  Call it after b200_vp8_residual_frame_device.
+ * The work runs as a wavefront: MB (r, c) starts once (r, c - 1) and (r - 1, c + 1) are done (the decoder's own check_thread_pos rule),
+ * the order the result depends on: a frame-wide order (all column edges, then all row edges) or a slope-1 wavefront give other pictures.
+ * Only the 16 mb_width x 16 mb_height luma and 8 mb_width x 8 mb_height chroma samples are read or written.  f needs no alignment
+ * beyond a byte.  Offsets are 64-bit.
+ * Returns 0, or B200_EINVAL (launching nothing) for NULL pointers, is_vp7, simple or keyframe not 0 / 1, mb_width or mb_height < 1,
+ * ls_y < 16 mb_width, ls_uv < 8 mb_width, or f_stride < mb_width. */
+int  b200_vp8_loopfilter_frame_device(B200Device *dev, int is_vp7, int simple, int keyframe, int mb_width, int mb_height,
+                                      uint8_t *const planes[3], ptrdiff_t ls_y, ptrdiff_t ls_uv, const B200Vp8FilterStrength *f,
+                                      int64_t f_stride);
+/* The frame entry's MB rows wait on the row above; every such wait is bounded by about one second, after which the MB is filtered
+ * anyway (wrong samples rather than a hung GPU) and a per-device counter is incremented.  This waits for the device's stream and stores
+ * the number of the VP8 loop filter's waits that ran out on that device since the process started in *count.  0; B200_EINVAL for
+ * count == NULL; B200_ENODEV; B200_EEXTERNAL. */
+int  b200_vp8_loopfilter_timeouts(B200Device *dev, int64_t *count);
 
 /* mpegvideo inverse quantisers: the members of MPVUnquantDSPContext (libavcodec/mpegvideo_unquantize.h:31-44) as
  * ff_mpv_unquantize_init() installs them (libavcodec/mpegvideo_unquantize.c:50-290), i.e. what runs in front of the IDCT in

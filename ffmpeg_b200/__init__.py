@@ -6,6 +6,6 @@ the first call does, and it raises if the library was not built or no GPU is usa
 """
 from ._lib import B200Error, SO_PATH, lib  # noqa: F401
 from .device import Device, launch_count  # noqa: F401
-from . import swscale, idctdsp, fdctdsp, me_cmp, pel, tx, mpegvideo, float_dsp, hevcdsp, vp9dsp, vp8dsp  # noqa: F401
+from . import swscale, idctdsp, fdctdsp, me_cmp, pel, tx, mpegvideo, float_dsp, hevcdsp, vp9dsp, vp8dsp, vc1dsp  # noqa: F401
 
-__all__ = ["B200Error", "Device", "launch_count", "swscale", "idctdsp", "fdctdsp", "me_cmp", "pel", "tx", "mpegvideo", "float_dsp", "hevcdsp", "vp9dsp", "vp8dsp", "lib", "SO_PATH"]
+__all__ = ["B200Error", "Device", "launch_count", "swscale", "idctdsp", "fdctdsp", "me_cmp", "pel", "tx", "mpegvideo", "float_dsp", "hevcdsp", "vp9dsp", "vp8dsp", "vc1dsp", "lib", "SO_PATH"]

@@ -295,6 +295,50 @@ class Vp8FilterStrength(C.Structure):
     _fields_ = [("filter_level", C.c_uint8), ("inner_limit", C.c_uint8), ("inner_filter", C.c_uint8)]
 
 
+VC1_MSPEL_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_int)                     # dst, src, stride, rnd
+VC1_CHROMA_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_ssize_t, C.c_int, C.c_int, C.c_int)    # dst, src, stride, h, x, y
+VC1_ITX8_FUNC = C.CFUNCTYPE(None, C.c_void_p)                                                         # vc1_inv_trans_8x8(block)
+VC1_ITX_FUNC = C.CFUNCTYPE(None, C.c_void_p, C.c_ssize_t, C.c_void_p)                                 # dest, stride, block
+
+
+class VC1DSPContext(C.Structure):
+    """libavcodec/vc1dsp.h:37-97 (same member order and member types; the members b200_vc1_dsp_init leaves NULL as untyped pointers)"""
+    _fields_ = ([("vc1_inv_trans_8x8", VC1_ITX8_FUNC)] +
+                [(f"vc1_inv_trans_{n}", VC1_ITX_FUNC) for n in ("8x4", "4x8", "4x4", "8x8_dc", "8x4_dc", "4x8_dc", "4x4_dc")] +
+                [(n, C.c_void_p) for n in ("vc1_v_overlap", "vc1_h_overlap", "vc1_v_s_overlap", "vc1_h_s_overlap", "vc1_v_loop_filter4",
+                                           "vc1_h_loop_filter4", "vc1_v_loop_filter8", "vc1_h_loop_filter8", "vc1_v_loop_filter16",
+                                           "vc1_h_loop_filter16")] +
+                [("put_vc1_mspel_pixels_tab", VC1_MSPEL_FUNC * 16 * 2), ("avg_vc1_mspel_pixels_tab", VC1_MSPEL_FUNC * 16 * 2),
+                 ("put_no_rnd_vc1_chroma_pixels_tab", VC1_CHROMA_FUNC * 3), ("avg_no_rnd_vc1_chroma_pixels_tab", VC1_CHROMA_FUNC * 3)] +
+                [(n, C.c_void_p) for n in ("sprite_h", "sprite_v_single", "sprite_v_double_noscale", "sprite_v_double_onescale",
+                                           "sprite_v_double_twoscale", "startcode_find_candidate", "vc1_unescape_buffer")])
+
+
+class Vc1McRef(C.Structure):
+    """B200Vc1McRef (include/b200dsp.h), 1080 bytes"""
+    _fields_ = [("y", C.c_void_p), ("u", C.c_void_p), ("v", C.c_void_p), ("ls_y", C.c_ssize_t), ("ls_uv", C.c_ssize_t),
+                ("rangeredfrm", C.c_int32), ("use_ic", C.c_int32), ("interlaced", C.c_int32), ("reserved", C.c_int32),
+                ("luty", C.c_uint8 * 256 * 2), ("lutuv", C.c_uint8 * 256 * 2)]
+
+
+class Vc1McSrc(C.Structure):
+    """B200Vc1McSrc (include/b200dsp.h), 16 bytes"""
+    _fields_ = [("x", C.c_int16), ("y", C.c_int16), ("uvx", C.c_int16), ("uvy", C.c_int16), ("ref", C.c_uint8), ("mx", C.c_uint8),
+                ("my", C.c_uint8), ("uvmx", C.c_uint8), ("uvmy", C.c_uint8), ("reserved", C.c_uint8 * 3)]
+
+
+class Vc1McOp(C.Structure):
+    """B200Vc1McOp (include/b200dsp.h), 40 bytes"""
+    _fields_ = [("dst_x", C.c_int16), ("dst_y", C.c_int16), ("kind", C.c_uint8), ("flags", C.c_uint8), ("reserved", C.c_uint8 * 2),
+                ("src", Vc1McSrc * 2)]
+
+
+class Vc1ResidualOp(C.Structure):
+    """B200Vc1ResidualOp (include/b200dsp.h), 16 bytes"""
+    _fields_ = [("coef_off", C.c_int64), ("x", C.c_int16), ("y", C.c_int16), ("plane", C.c_uint8), ("ttblk", C.c_uint8),
+                ("subblkpat", C.c_uint8), ("dc", C.c_uint8)]
+
+
 class ProresDSPContext(C.Structure):
     """libavcodec/proresdsp.h:28-35"""
     _fields_ = [("idct_permutation_type", C.c_int), ("idct_permutation", C.c_uint8 * 64),
@@ -437,6 +481,9 @@ PROTOTYPES = {
     "b200_vp8_loopfilter_frame_device": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_ssize_t, C.c_ssize_t, vp,
                                                    C.c_int64]),
     "b200_vp8_loopfilter_timeouts": (C.c_int, [vp, vp]),
+    "b200_vc1_dsp_init": (C.c_int, [vp]),
+    "b200_vc1_mc_frame_device": (C.c_int, [vp, C.c_int, vp, vp, C.c_ssize_t, C.c_ssize_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64, vp]),
+    "b200_vc1_residual_frame_device": (C.c_int, [vp, vp, C.c_ssize_t, C.c_ssize_t, C.c_int, C.c_int, vp, C.c_int64, vp]),
     "b200_proresdsp_init": (C.c_int, [vp, C.c_int]),
     "b200_prores_idct_put_batch_device": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, vp, vp, vp, C.c_int]),
     "b200_float_dsp_init": (C.c_int, [vp]),

@@ -1492,6 +1492,151 @@ int  b200_tx_batch_device(B200TXContext *ctx, void *out, const void *in, ptrdiff
 int  b200_tx_batch_host(B200TXContext *ctx, void *out, const void *in, ptrdiff_t stride, int64_t count,
                         ptrdiff_t out_step, ptrdiff_t in_step);
 
+/* VC-1 / WMV3 motion compensation and inverse transforms: VC1DSPContext (libavcodec/vc1dsp.h:37-97) in the reference's member order and
+ * types.  b200_vc1_dsp_init() fills what ff_vc1dsp_init fills (vc1dsp.c:968-1017) of these members, sharing functions as it does:
+ *   vc1_inv_trans_{8x8,8x4,4x8,4x4} and their _dc forms            the eight transforms
+ *   put_vc1_mspel_pixels_tab[size][dxy], avg_vc1_mspel_pixels_tab    size 0 = 16x16, 1 = 8x8; dxy = hmode + 4 vmode (mx & 3, my & 3);
+ *                                                                    [size][0] is the plain copy (put_pixels16x16_c / 8x8_c), which
+ *                                                                    ignores its last argument
+ *   put_no_rnd_vc1_chroma_pixels_tab[0..1], avg_no_rnd_...[0..1]    8 and 4 wide; [2] NULL as in the reference
+ * The overlap members, the six loop filters, the five sprite members, startcode_find_candidate and vc1_unescape_buffer stay NULL.  HOST
+ * pointers, the reference's signatures; a member reads only what its reference function reads and writes only what it writes.
+ *   mspel      4-tap rows {-4, 53, 18, -3}, {-1, 9, 9, -1}, {-3, 18, 53, -4} for modes 1..3 (vc1dsp.c:542-584); horizontal only
+ *              (taps + 32 - rnd) >> 6 (+ 8 - rnd >> 4 at mode 2); vertical only the same with 1 - rnd for rnd; both: vertical pass over
+ *              columns -1 .. w + 1 with shift (s[h] + s[v]) >> 1, s = {0, 5, 1, 5}, rounding (1 << (shift - 1)) + rnd - 1, into int16,
+ *              then the horizontal pass (+ 64 - rnd) >> 7; clipped to 0..255; avg (dst + x + 1) >> 1
+ *   chroma     (A s00 + B s01 + C s10 + D s11 + 28) >> 6 with A = (8 - x)(8 - y), B = x (8 - y), C = (8 - x) y, D = x y over h rows; avg
+ *              (dst + x + 1) >> 1; x, y 0..7, h 0..4096 (outside: the member writes nothing and records why in b200_last_error())
+ *   8x8        in place on block: column pass (+ 4) >> 3 into int16, row pass (+ 64) >> 7, + 1 on outputs 4..7, into int16 block
+ *   8x4, 4x8, 4x4   row pass (+ 4) >> 3 written back into block (int16), column pass (+ 64) >> 7 added to dest and clipped
+ *   _dc        dest += the DC of block[0] (vc1dsp.c:241-260, :332-351, :409-424, :482-497); block untouched
+ * 0; B200_EINVAL for c == NULL; B200_ENODEV. */
+typedef void (*b200_vc1op_pixels_func)(uint8_t *block, const uint8_t *pixels, ptrdiff_t line_size, int round);
+typedef struct B200VC1DSPContext {
+    void (*vc1_inv_trans_8x8)(int16_t *b);
+    void (*vc1_inv_trans_8x4)(uint8_t *dest, ptrdiff_t stride, int16_t *block);
+    void (*vc1_inv_trans_4x8)(uint8_t *dest, ptrdiff_t stride, int16_t *block);
+    void (*vc1_inv_trans_4x4)(uint8_t *dest, ptrdiff_t stride, int16_t *block);
+    void (*vc1_inv_trans_8x8_dc)(uint8_t *dest, ptrdiff_t stride, int16_t *block);
+    void (*vc1_inv_trans_8x4_dc)(uint8_t *dest, ptrdiff_t stride, int16_t *block);
+    void (*vc1_inv_trans_4x8_dc)(uint8_t *dest, ptrdiff_t stride, int16_t *block);
+    void (*vc1_inv_trans_4x4_dc)(uint8_t *dest, ptrdiff_t stride, int16_t *block);
+    void (*vc1_v_overlap)(uint8_t *src, ptrdiff_t stride);
+    void (*vc1_h_overlap)(uint8_t *src, ptrdiff_t stride);
+    void (*vc1_v_s_overlap)(int16_t *top, int16_t *bottom);
+    void (*vc1_h_s_overlap)(int16_t *left, int16_t *right, ptrdiff_t left_stride, ptrdiff_t right_stride, int flags);
+    void (*vc1_v_loop_filter4)(uint8_t *src, ptrdiff_t stride, int pq);
+    void (*vc1_h_loop_filter4)(uint8_t *src, ptrdiff_t stride, int pq);
+    void (*vc1_v_loop_filter8)(uint8_t *src, ptrdiff_t stride, int pq);
+    void (*vc1_h_loop_filter8)(uint8_t *src, ptrdiff_t stride, int pq);
+    void (*vc1_v_loop_filter16)(uint8_t *src, ptrdiff_t stride, int pq);
+    void (*vc1_h_loop_filter16)(uint8_t *src, ptrdiff_t stride, int pq);
+    b200_vc1op_pixels_func put_vc1_mspel_pixels_tab[2][16];
+    b200_vc1op_pixels_func avg_vc1_mspel_pixels_tab[2][16];
+    b200_h264_chroma_mc_func put_no_rnd_vc1_chroma_pixels_tab[3];
+    b200_h264_chroma_mc_func avg_no_rnd_vc1_chroma_pixels_tab[3];
+    void (*sprite_h)(uint8_t *dst, const uint8_t *src, int offset, int advance, int count);
+    void (*sprite_v_single)(uint8_t *dst, const uint8_t *src1a, const uint8_t *src1b, int offset, int width);
+    void (*sprite_v_double_noscale)(uint8_t *dst, const uint8_t *src1a, const uint8_t *src2a, int alpha, int width);
+    void (*sprite_v_double_onescale)(uint8_t *dst, const uint8_t *src1a, const uint8_t *src1b, int offset1, const uint8_t *src2a, int alpha,
+                                     int width);
+    void (*sprite_v_double_twoscale)(uint8_t *dst, const uint8_t *src1a, const uint8_t *src1b, int offset1, const uint8_t *src2a,
+                                     const uint8_t *src2b, int offset2, int alpha, int width);
+    int (*startcode_find_candidate)(const uint8_t *buf, int size);
+    int (*vc1_unescape_buffer)(const uint8_t *src, int size, uint8_t *dst);
+} B200VC1DSPContext;
+int  b200_vc1_dsp_init(B200VC1DSPContext *c);
+
+/* One reference picture of b200_vc1_mc_frame_device: DEVICE addresses of sample (0, 0) of its three planes, line sizes in bytes, and
+ * the state the decoder keeps per reference (v->last_* / v->next_*): rangeredfrm, use_ic with luty / lutuv indexed by source-row
+ * parity, and whether the reference is interlaced (refused: interlaced MC is not implemented). */
+typedef struct B200Vc1McRef {
+    const uint8_t *y, *u, *v;
+    ptrdiff_t ls_y, ls_uv;
+    int32_t rangeredfrm, use_ic, interlaced, reserved;
+    uint8_t luty[2][256], lutuv[2][256];
+} B200Vc1McRef;
+/* One prediction source of an op: reference index, the luma position src_x / src_y after the decoder's clip (vc1_mc.c:258-273) with
+ * mx & 3 / my & 3, and the chroma position uvsrc_x / uvsrc_y with uvmx & 3 / uvmy & 3 (after fastuvmc).  An op reads the fields of
+ * the planes it writes. */
+typedef struct B200Vc1McSrc {
+    int16_t x, y;           /* luma: src_x, src_y */
+    int16_t uvx, uvy;       /* chroma: uvsrc_x, uvsrc_y */
+    uint8_t ref;            /* index into the call's refs */
+    uint8_t mx, my;         /* mx & 3, my & 3 */
+    uint8_t uvmx, uvmy;     /* uvmx & 3, uvmy & 3 */
+    uint8_t reserved[3];
+} B200Vc1McSrc;
+/* One op of b200_vc1_mc_frame_device.  kind 1MV is one call of ff_vc1_mc_1mv (vc1_mc.c:172-449): Y 16x16 at (dst_x, dst_y) and U, V
+ * 8x8 at (dst_x / 2, dst_y / 2), the chroma window copied exactly when the luma edge test fires; with B200_VC1_MC_AVG src[1] is then
+ * averaged in as ff_vc1_interp_mc does (vc1_mc.c:1004-1230, B-frame interpolation, its own edge test).  LUMA8 is ff_vc1_mc_4mv_luma
+ * (:452-631, avg 0): Y 8x8 at (dst_x, dst_y).  CHROMA8 is the MC half of ff_vc1_mc_4mv_chroma (:634-836): U and V 8x8 at (dst_x, dst_y)
+ * in chroma samples, from the uv fields.  The chroma vector averaging of 4MV stays with the caller. */
+enum { B200_VC1_MC_1MV = 0, B200_VC1_MC_LUMA8 = 1, B200_VC1_MC_CHROMA8 = 2 };
+enum { B200_VC1_MC_MSPEL = 1, B200_VC1_MC_RND = 2, B200_VC1_MC_AVG = 4 };   /* flags: s->mspel, v->rnd, src[1] averaged in (1MV only) */
+typedef struct B200Vc1McOp {
+    int16_t dst_x, dst_y;   /* top-left sample of the block in the plane it writes; multiples of 8 */
+    uint8_t kind;           /* B200_VC1_MC_* kind */
+    uint8_t flags;          /* B200_VC1_MC_MSPEL | B200_VC1_MC_RND | B200_VC1_MC_AVG */
+    uint8_t reserved[2];
+    B200Vc1McSrc src[2];
+} B200Vc1McOp;
+#ifdef __cplusplus
+static_assert(sizeof(B200Vc1McSrc) == 16 && sizeof(B200Vc1McOp) == 40, "B200Vc1McOp is 40 bytes");
+static_assert(sizeof(B200Vc1McRef) == 1080, "B200Vc1McRef is 1080 bytes");
+#else
+_Static_assert(sizeof(B200Vc1McSrc) == 16 && sizeof(B200Vc1McOp) == 40, "B200Vc1McOp is 40 bytes");
+_Static_assert(sizeof(B200Vc1McRef) == 1080, "B200Vc1McRef is 1080 bytes");
+#endif
+/* Inter prediction of a whole progressive VC-1 picture in one call: `refs` is a HOST array of 1 <= nrefs <= 2 references (copied into
+ * the launch), `ops` and the dst planes are DEVICE pointers; asynchronous on the device's stream.  Each op's result is the reference
+ * sequence for progressive pictures (field_mode 0, interlace 0):
+ *   1. the decoder's edge test, on the luma fields for 1MV (ff_vc1_mc_1mv: x against mspel, y against 1; src[1] as ff_vc1_interp_mc:
+ *      both against 1) and LUMA8, on the uv fields for CHROMA8; rangeredfrm or use_ic of the op's reference always fire it;
+ *   2. where it fires, the emulated_edge_mc window: 17 + 2 mspel (1MV) / 9 + 2 mspel (LUMA8) samples square from (x - mspel,
+ *      y - mspel), 9 x 9 from (uvx, uvy), coordinates clamped to h_edge_pos x v_edge_pos (chroma: halves); where it does not, the
+ *      plane is read directly (so planes must be readable wherever the decoder reads them);
+ *   3. in the window, range reduction ((s - 128) >> 1) + 128 when rangeredfrm, then with use_ic luty / lutuv of the window row's
+ *      source-row parity;
+ *   4. the member: with MSPEL put_vc1_mspel_pixels_tab[size][dxy] (avg_ for src[1]); else hpeldsp put_pixels_tab / put_no_rnd_ (avg_ /
+ *      avg_no_rnd_ for src[1]) as rnd is 0 / 1 at dxy = (my & 2) | (mx & 2) >> 1; chroma put_h264_chroma_pixels_tab[0] (avg_ for
+ *      src[1]) with rnd 0 and put_no_rnd_vc1_chroma_pixels_tab[0] (avg_no_rnd_) with rnd 1, at ((uvmx & 3) << 1, (uvmy & 3) << 1).
+ * The caller guarantees that the ops of one call write disjoint blocks and that no op reads what another op of the call writes.
+ * An op writes nothing if its kind is undefined, a phase is above 3, a reference index is >= nrefs, AVG is set on a kind other than
+ * 1MV, dst_x or dst_y is not a multiple of 8, or its blocks are not inside 16 mb_width x 16 mb_height luma / 8 mb_width x 8 mb_height
+ * chroma.  More ops than one launch takes are split inside the entry.
+ * Returns 0, or B200_EINVAL (launching nothing) for NULL pointers, nops < 0, nrefs outside 1..2, mb_width or mb_height outside 1..2047,
+ * h_edge_pos or v_edge_pos outside 1..32767, ops not aligned to 4 bytes, or a dst plane or line size that is not a multiple of 4;
+ * B200_ENOSYS (launching nothing) for an interlaced reference; nops == 0 returns 0. */
+int  b200_vc1_mc_frame_device(B200Device *dev, int nrefs, const B200Vc1McRef *refs, uint8_t *const dst[3], ptrdiff_t ls_y, ptrdiff_t ls_uv,
+                              int mb_width, int mb_height, int h_edge_pos, int v_edge_pos, int64_t nops, const B200Vc1McOp *ops);
+
+/* One inter 8x8 block of b200_vc1_residual_frame_device: the transform calls vc1_decode_p_block makes (vc1_block.c:1124-1240). */
+enum { B200_VC1_TT_8X8 = 0, B200_VC1_TT_8X4 = 1, B200_VC1_TT_4X8 = 2, B200_VC1_TT_4X4 = 3 };
+typedef struct B200Vc1ResidualOp {
+    int64_t coef_off;       /* element offset in coef of the block's 64 int16, dequantised, raster order as in block[]; a multiple of 8 */
+    int16_t x, y;           /* top-left sample of the block in its plane; multiples of 8 */
+    uint8_t plane;          /* 0 Y, 1 U, 2 V */
+    uint8_t ttblk;          /* B200_VC1_TT_*: the generic type after the decoder's TT_8X4_TOP / ... conversion */
+    uint8_t subblkpat;      /* 8x4 / 4x8: bit 1 - j skips sub-block j; 4x4: bit 3 - j skips sub-block j (j in raster order) */
+    uint8_t dc;             /* bit j: sub-block j takes the _dc form (the decoder's i == 1) */
+} B200Vc1ResidualOp;
+#ifdef __cplusplus
+static_assert(sizeof(B200Vc1ResidualOp) == 16, "B200Vc1ResidualOp is 16 bytes");
+#else
+_Static_assert(sizeof(B200Vc1ResidualOp) == 16, "B200Vc1ResidualOp is 16 bytes");
+#endif
+/* The inter residual of a whole picture in one call, DEVICE pointers (ops, coef, dst[0..2]), asynchronous on the device's stream.  Per
+ * op, for every sub-block j that subblkpat does not mask: with dc bit j vc1_inv_trans_<tt>_dc, else vc1_inv_trans_<tt> (8x8:
+ * vc1_inv_trans_8x8 followed by add_pixels_clamped), at the sub-block's place; int16 truncation exactly where the reference stores, so
+ * every int16 coefficient value is accepted.  `coef` is read only.  The ops of one call write disjoint blocks.  An op writes nothing if
+ * its plane or ttblk is undefined, coef_off is negative or not a multiple of 8, x or y is not a multiple of 8, or its block is not
+ * inside 16 mb_width x 16 mb_height luma / 8 mb_width x 8 mb_height chroma.  Intra blocks are not covered.
+ * Returns 0, or B200_EINVAL (launching nothing) for NULL pointers, nops < 0, mb_width or mb_height outside 1..2047, ops not aligned
+ * to 8 bytes, coef not aligned to 16 bytes, or a dst plane or line size that is not a multiple of 4; nops == 0 returns 0. */
+int  b200_vc1_residual_frame_device(B200Device *dev, uint8_t *const dst[3], ptrdiff_t ls_y, ptrdiff_t ls_uv, int mb_width, int mb_height,
+                                    const int16_t *coef, int64_t nops, const B200Vc1ResidualOp *ops);
+
 #ifdef __cplusplus
 }
 #endif
